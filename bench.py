@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — headline benchmark of the SVSDF cost+gradient hot path (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 A *step* is one pass of the hot path over one batch of synthetic input: one evaluation of
 TrajOptimizer::addSaftyPenaOnSweptVolumeParallelTrueSDF (reference: back_end_optimizer.hpp:774-869) over the
@@ -17,14 +17,14 @@ Reported on ONE JSON line by rank 0:
                    host->device copy of the points and of the trajectory, device->host copy of cost/gradients inside
                    the timed region)
   lbfgs            full L-BFGS optimisation from x0 through svsdf_optimize (iterations/s, evaluations/s)
-  roofline         FP64 (non-tensor) roofline of the dominant kernel k_outer: achieved = flop_per_launch / t, with
-                   flop_per_launch (DADD + DMUL + 2 DFMA thread instructions) from the committed ncu capture of the same
-                   workload (profiles/r2_k_outer_roofline.json, scripts/roofline_from_ncu.py) and t measured here with
-                   CUDA events; the capture's FP64-pipe-active and issue-active percentages are reported next to it
+  roofline         the dominant kernel k_outer: its time (CUDA events), the FP64 FMA peak measured in the same run by a
+                   micro-benchmark, and the algorithmic HBM traffic (the query points) over the H100's bandwidth
   cpu_baseline     the reference's CPU path timed on this box's host cores: the reference's OWN code compiled where it
                    lies (oracle/_ref/libref_path_glibc.so, kind "reference") when that library travelled with the
                    snapshot, else the line-for-line restatement under oracle/ (kind "port")
 `--impl reference` times that CPU path alone on the same workload with the same metric / config keys.
+`--dump-outputs DIR` writes what the last timed step returned (cost, gradients, inside count) as float64 DIR/<name>.npy; the
+inputs are seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -45,7 +45,6 @@ sys.path.insert(0, ROOT)
 P_POINTS = 200_000
 N_PIECES = 8
 SHAPE = "star"
-ROOFLINE_JSON = os.path.join(ROOT, "profiles", "r2_k_outer_roofline.json")  # ncu-derived, scripts/roofline_from_ncu.py
 METRIC = "svsdf_query_pts_per_sec"
 UNIT = "pts/s"
 
@@ -58,7 +57,7 @@ def dist_env():
 
 
 class ClockSampler:
-    """Samples nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md clocks line)."""
+    """Samples nvidia-smi clocks / throttle reasons during the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -86,6 +85,7 @@ class ClockSampler:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
         time.sleep(0.15)
         self.proc.terminate()
+        self.proc.wait()
         rows = [ln for (ts, ln) in self.lines if t0 - 0.05 <= ts <= t1 + 0.15] or [ln for (_, ln) in self.lines]
         sm, mx, reasons = [], [], set()
         for ln in rows:
@@ -271,6 +271,8 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-lbfgs", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float64)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     if args.impl == "reference":
@@ -306,7 +308,7 @@ def main():
 
     def problem_of(step):
         return sc, ctx, co
-    flush = torch.empty(160 * 1024 * 1024, dtype=torch.float16, device=f"cuda:{local}")  # 320 MB > 126 MB L2
+    flush = torch.empty(160 * 1024 * 1024, dtype=torch.float16, device=f"cuda:{local}")  # 320 MB > the H100's 50 MB L2
 
     def barrier():
         torch.cuda.synchronize()
@@ -324,17 +326,26 @@ def main():
     barrier()
     t_wall0 = time.time()
     ms_steps, outer_ms = [], []
+    last_out = None
     for s_ in range(args.steps):
         pr, c, cc = problem_of(s_)
         flush.zero_()  # flush L2 between timed iterations (untimed)
         torch.cuda.synchronize()
-        ms, _ = c.cost_grad_device(pr.T, cc, repeats=1, fetch=False)  # CUDA events on the launching stream
+        # CUDA events on the launching stream; the result is always copied back after the end event, fetching it costs no timed work
+        ms, last_out = c.cost_grad_device(pr.T, cc, repeats=1, fetch=s_ == args.steps - 1)
         ms_steps.append(ms)
         if c is ctx:
             outer_ms.append(c.last_kernel_ms()[1])
     barrier()
     t_wall1 = time.time()
     clocks = sampler.stop(t_wall0, t_wall1)
+    if args.dump_outputs and rank == 0 and last_out is not None:
+        # out = [cost, gradC (18N, Eigen column-major), gradT (N), n_inside]
+        N = sc.N
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, arr in (("cost", last_out[:1]), ("grad_coeffs", last_out[1:1 + 18 * N]),
+                          ("grad_durations", last_out[1 + 18 * N:1 + 19 * N]), ("n_inside", last_out[1 + 19 * N:])):
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), np.asarray(arr, dtype=np.float64))
     launches = sum(c.kernel_launches() for c in ctxs) - launches0
     my_ms = float(sum(ms_steps))
     t = torch.tensor([my_ms], dtype=torch.float64, device=f"cuda:{local}")
@@ -379,30 +390,19 @@ def main():
         lane_evals = ctx.executed_evals(False)
         peak = ctx.fp64_peak_tflops()
         t_outer = statistics.mean(outer_ms) * 1e-3
-        cap = json.load(open(ROOFLINE_JSON)) if os.path.exists(ROOFLINE_JSON) else None
         peaks = {}
         ppath = os.path.join(ROOT, "MEASURED_PEAKS.json")
         if os.path.exists(ppath):
             peaks = json.load(open(ppath))
-        hbm_peak = peaks.get("hbm_gbs", 6650.0)
+        hbm_peak = peaks.get("hbm_gbs", 3350.0)
         alg_bytes = sc.P * 16
-        achieved = (cap["flop_per_launch"] / t_outer / 1e12) if cap else None
         extra["roofline"] = {
-            "bound": "fp64", "kernel": "k_outer", "achieved": achieved, "peak": peak, "unit": "TFLOP/s",
-            "frac": (achieved / peak) if achieved else None,
+            "bound": "fp64", "kernel": "k_outer", "peak": peak, "unit": "TFLOP/s",
             "peak_source": "DFMA micro-benchmark in this run (svsdf_fp64_peak); MEASURED_PEAKS.json has no FP64 figure",
-            "flop_per_launch": cap["flop_per_launch"] if cap else None,
-            "flop_source": "profiles/r2_k_outer_roofline.json: DADD + DMUL + 2 DFMA thread instructions of one launch (ncu --set full capture of this workload); "
-                           "the strict build issues DMUL + DADD where an FMA build would issue one DFMA, so the DFMA-based peak is reachable "
-                           "only at half rate by this instruction mix - see fp64_pipe_active_pct",
-            "fp64_pipe_active_pct": cap.get("fp64_pipe_active_pct") if cap else None,
-            "issue_active_pct": cap.get("issue_active_pct") if cap else None,
-            "traffic": cap.get("dram_bytes_per_launch") if cap else None,
             "evals_per_point_executed": lane_evals / sc.P, "kernel_ms": t_outer * 1e3,
-            "flop_per_lane_eval": (cap["flop_per_launch"] / lane_evals) if cap else None,
             "kernel_share_of_step": t_outer * 1e3 / statistics.mean(ms_steps),
             "hbm": {"achieved": alg_bytes / t_outer / 1e9, "peak": hbm_peak, "unit": "GB/s", "frac": alg_bytes / t_outer / 1e9 / hbm_peak,
-                    "peak_source": "MEASURED_PEAKS.json (measured)" if peaks else "fallback", "algorithmic_bytes": alg_bytes},
+                    "peak_source": "MEASURED_PEAKS.json (measured)" if peaks else "H100 SXM data sheet (3.35 TB/s)", "algorithmic_bytes": alg_bytes},
         }
         km = ctx.last_kernel_ms()
         extra["kernel_ms"] = {"k_pose_table": km[0], "k_outer": km[1], "k_compact+k_gsip": km[2], "k_finalize": km[3]}

@@ -10,7 +10,7 @@ The classes mirror the reference's call surface for this path so tests read like
   (src/planner_algorithm/include/planner_algorithm/back_end_optimizer.hpp:344-408, 774-869, 877-945;
   src/planner_algorithm/src/back_end_optimizer.cpp:3-97).
 
-There is no CPU fallback: if the CUDA library is missing or no B200 is visible, construction raises.
+There is no CPU fallback: if the CUDA library is missing or no H100 is visible, construction raises.
 """
 from __future__ import annotations
 
@@ -425,7 +425,7 @@ class Context:
         h = C.c_void_p()
         rc = L.svsdf_create(C.byref(cfg), C.byref(h))
         if rc != 0 or not h:
-            raise SvsdfError(f"svsdf_create failed with status {rc} (no usable sm_100 CUDA device? no CPU fallback)")
+            raise SvsdfError(f"svsdf_create failed with status {rc} (no usable sm_90 (H100) CUDA device? no CPU fallback)")
         self.h = h
         self.P = 0
 

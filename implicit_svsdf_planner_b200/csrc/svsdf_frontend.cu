@@ -1,6 +1,6 @@
 // svsdf_frontend.cu — K5: the collision kernels of the reference's A* front end on the device (SURVEY.md §8f rank 3).
 //
-// Reference (paths relative to /root/reference/src):
+// Reference (paths relative to the reference project's src/):
 //   BasicShape::initShape                 utils/include/utils/Shape.hpp:386-430   yaw-indexed occupancy kernels of the robot shape:
 //                                         cell (a, b) of kernel k is set iff getonlySDF((x_a, y_b, 0), Rz(yaw_k)) <= safemargin
 //   getonlySDF(pos_rel, R_obj)            Shape.hpp:481-485 ... (every analytic class): ((p - trans) * Rotate * R_obj).head(2)
@@ -9,7 +9,7 @@
 //                                         kernel with the window of the inflated, byte-packed map kernel (generateMapKernel2D)
 //   visit_kernels_by_distance, checkKernelValue   sw_manager.hpp:1099-1169
 //
-// B200 formulation.  The A* calls kernelConv once per (expanded cell, yaw) — 51 byte operations each, latency bound on
+// GPU formulation.  The A* calls kernelConv once per (expanded cell, yaw) — 51 byte operations each, latency bound on
 // the host.  Here the whole configuration-space obstacle map is produced in one pass instead: free[k][x][y] for every yaw
 // kernel k and every cell, 32 cells (one output word) per thread, each kernel row applied as shifted ORs of the two map
 // words under it (funnel shifts; the map's MSB-first bit order is kept so the words are the map's own bytes).  Integer

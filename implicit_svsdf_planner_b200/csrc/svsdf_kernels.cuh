@@ -1,4 +1,4 @@
-// svsdf_kernels.cuh — sm_100a kernels for the SVSDF collision cost + gradient hot path.
+// svsdf_kernels.cuh — sm_90a (H100) kernels for the SVSDF collision cost + gradient hot path.
 //
 // Replaces the OpenMP loop  TrajOptimizer::addSaftyPenaOnSweptVolumeParallelTrueSDF
 // (src/planner_algorithm/include/planner_algorithm/back_end_optimizer.hpp:774-869) and everything it calls in

@@ -1,7 +1,7 @@
 // svsdf_runtime.cpp — host runtime and C ABI (include/svsdf.h) of libsvsdf_b200.so.
 //
 // Owns the device buffers (query points resident in HBM, trajectory blob, per-CTA partials, inside-point lists),
-// the CUDA stream, pinned staging memory, the host MINCO spline and the host L-BFGS; launches the sm_100a kernels
+// the CUDA stream, pinned staging memory, the host MINCO spline and the host L-BFGS; launches the sm_90a kernels
 // of svsdf_kernels.cuh.  There is deliberately no CPU implementation of the hot path in this library: if CUDA is
 // unavailable svsdf_create fails.
 #include <cuda_runtime.h>
@@ -41,7 +41,7 @@ struct svsdf_ctx {
     double rho = 3.8;
     int device = 0;
     bool strict = false;
-    int sm_count = 148;
+    int sm_count = 132;
     cudaStream_t stream = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     cudaEvent_t evk[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};  // per-kernel timing marks
@@ -1009,8 +1009,8 @@ int svsdf_create(const svsdf_config *cfg, svsdf_ctx **out) {
     if ((e = cudaSetDevice(ctx->device)) != cudaSuccess) return fail(e);
     cudaDeviceProp prop;
     if ((e = cudaGetDeviceProperties(&prop, ctx->device)) != cudaSuccess) return fail(e);
-    if (prop.major < 10) {
-        std::fprintf(stderr, "svsdf_create: device sm_%d%d is not Blackwell (kernels are built for sm_100a only)\n",
+    if (prop.major != 9 || prop.minor != 0) {  // sm_90a code loads on compute capability 9.0 only
+        std::fprintf(stderr, "svsdf_create: device sm_%d%d is not a Hopper H100 (kernels are built for sm_90a only)\n",
                      prop.major, prop.minor);
         svsdf_destroy(ctx);
         return SVSDF_ERR_CUDA;

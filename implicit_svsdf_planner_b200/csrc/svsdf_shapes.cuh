@@ -459,8 +459,13 @@ struct ShapeFn<SH_MESH> {
         int d = -1, next = 0;
         float ret = 0.0f;
         bool have_ret = false;
+        // A valid hierarchy ends within 2 nn - 1 iterations (every node entered once, returned from once); past the bound the
+        // hierarchy is corrupt and the result is NaN rather than a spinning warp.  The bounded loop is also what the sm_90a
+        // code of the standalone shape kernel needs: built without this exit, k_shape_sdf<SH_MESH> never returned on the H100.
+        const int max_iter = 4 * (S.fwn_nn + 1);
 #pragma unroll 1
-        for (;;) {
+        for (int iter = 0;; ++iter) {
+            if (iter > max_iter) return __int_as_float(0x7fc00000);
             if (!have_ret) {  // enter node `next` as a new frame
                 ++d;
                 f_node[d] = next;
@@ -582,8 +587,12 @@ struct ShapeFn<SH_MESH> {
         double best = __longlong_as_double(0x7ff0000000000000LL);
         float bestf = INF;  // >= best * (1 + 1e-12)
         int node = 0;
+        // every node is processed at most once and every stack entry popped at most once: <= 2 nn + 1 iterations on a valid
+        // hierarchy (bounded for the same two reasons as fwn_solid_angle's loop)
+        const int max_iter = 4 * (S.fwn_nn + 1);
 #pragma unroll 1
-        for (;;) {
+        for (int iter = 0;; ++iter) {
+            if (iter > max_iter) return __longlong_as_double(0x7ff8000000000000LL);
             if (node < 0) {
                 if (top == 0) break;
                 --top;

@@ -2,7 +2,7 @@
 //
 // The reference calls the platform libm here (glibc `sin`/`cos` through Eigen::AngleAxisd, sw_manager.hpp:465-474 and
 // back_end_optimizer.hpp:1058-1061; `atan2` in SampleSet2D::initSet :80 and Polygon::isCrossRayOnXDir
-// Shape.hpp:1374-1375).  libm is a third-party dependency outside /root/reference whose last-bit behaviour is
+// Shape.hpp:1374-1375).  libm is a third-party dependency outside the reference project whose last-bit behaviour is
 // unspecified, and that last bit decides which way the reference's sign-descent falls at flat minima (DESIGN.md §Parity).
 // This build therefore pins ONE algorithm, made only of IEEE-exact operations (+, -, *, /, fma), on both sides — the
 // CPU oracle carries its own copy in oracle/portable_sincos.hpp — so the strict build reproduces the oracle bit for bit:

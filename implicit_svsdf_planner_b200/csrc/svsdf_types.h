@@ -1,4 +1,4 @@
-// svsdf_types.h — POD types shared by the host runtime and the sm_100a kernels.
+// svsdf_types.h — POD types shared by the host runtime and the sm_90a kernels.
 #pragma once
 #include <stdint.h>
 

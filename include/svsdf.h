@@ -1,9 +1,9 @@
-/* svsdf.h — C ABI of libsvsdf_b200.so: the B200-native drop-in for the SVSDF collision cost + gradient path of
+/* svsdf.h — C ABI of libsvsdf_b200.so: the H100-native drop-in for the SVSDF collision cost + gradient path of
  * ZJU-FAST-Lab/Implicit-SVSDF-Planner.  Plain pointers and sizes only; no C++/torch types cross this boundary.
  * All matrices use the reference's memory layouts (Eigen default column-major) so a maintainer can pass
  * `.data()` of the existing Eigen objects (see INTEGRATION.md for the binding stubs).
  *
- * Reference interfaces replaced (paths relative to /root/reference/src):
+ * Reference interfaces replaced (paths relative to the reference project's src/):
  *   R1  TrajOptimizer::addSaftyPenaOnSweptVolumeParallelTrueSDF(void*, const VectorXd& T, const MatrixX3d& coeffs,
  *         double& cost, VectorXd& gradT, MatrixX3d& gradC)
  *         planner_algorithm/include/planner_algorithm/back_end_optimizer.hpp:774-869      -> svsdf_cost_grad

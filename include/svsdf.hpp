@@ -11,7 +11,7 @@
 //                                         setParam :877-932, setEnvironment :935, parallel_points(_num), costFunctionLmbmParallel :344-408,
 //                                         addSaftyPenaOnSweptVolumeParallelTrueSDF :774-869, optimize_traj_lmbm (back_end_optimizer.cpp:3-97)
 // Errors: like the reference there are no exceptions on the hot path; methods return the solver / status code and
-// last_error() gives the text.  Construction throws std::runtime_error when no sm_100 GPU is usable (no CPU fallback).
+// last_error() gives the text.  Construction throws std::runtime_error when no sm_90 (H100) GPU is usable (no CPU fallback).
 #pragma once
 #include <array>
 #include <cstdint>
@@ -78,7 +78,7 @@ struct Ctx {
         const int rc_create = svsdf_create(&cfg, &h);
         svsdf_free(fv); svsdf_free(ff);
         if (rc_create != SVSDF_OK) h = nullptr;
-        if (!h) throw std::runtime_error("svsdf_create failed (no sm_100 CUDA device? there is no CPU fallback)");
+        if (!h) throw std::runtime_error("svsdf_create failed (no sm_90 (H100) CUDA device? there is no CPU fallback)");
     }
     ~Ctx() { svsdf_destroy(h); }
     Ctx(const Ctx &) = delete;

@@ -8,7 +8,7 @@ tmp = tempfile.mkdtemp()
 src_csv = os.path.join(tmp, "src.csv")
 subprocess.run(f"ncu -i {rep} --page source --csv > {src_csv} 2>/dev/null", shell=True, check=True)
 subprocess.run(f"cd {tmp} && cuobjdump -xelf svsdf_kernels_{unit} {root}/implicit_svsdf_planner_b200/lib/libsvsdf_b200.so > /dev/null 2>&1 && "
-               f"nvdisasm --print-line-info svsdf_kernels_{unit}.sm_100a.cubin > sass.txt 2>/dev/null", shell=True, check=True)
+               f"nvdisasm --print-line-info svsdf_kernels_{unit}.sm_90a.cubin > sass.txt 2>/dev/null", shell=True, check=True)
 # function extents from the source file
 lines = open(os.path.join(root, "implicit_svsdf_planner_b200", "csrc", "svsdf_kernels.cuh")).read().split("\n")
 marks = []

@@ -1,6 +1,6 @@
 """One whole plan on the reference's own star scene (pcds/map_star.pcd + pcds/trajectory_star.txt + config/star.yaml, carried as
 tests/golden/map_star_pcd.npz): point cloud -> map -> A* front end -> waypoints / query points -> mid-end warm start -> SVSDF back end.
-Prints one JSON line.  Needs a B200:  python scripts/run_plan.py [--shape star]"""
+Prints one JSON line.  Needs an H100:  python scripts/run_plan.py [--shape star]"""
 import argparse
 import json
 import os

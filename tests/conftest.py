@@ -10,7 +10,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA (B200) device; run with -m gpu on the GPU box")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA (H100) device; run with -m gpu on a machine that has one")
 
 
 def _has_gpu():

@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on a B200): the CUDA path, called through the C ABI (include/svsdf.h via
+"""GPU parity tests (run with -m gpu on an H100): the CUDA path, called through the C ABI (include/svsdf.h via
 implicit_svsdf_planner_b200.api), against the CPU oracle on the same seeded inputs and against the committed golden
 vectors.
 

@@ -92,21 +92,19 @@ def test_own_solver_reaches_at_least_what_the_reference_reaches(gold, cname, N):
 
 
 def test_live_reference_library_when_present(gold):
-    from oracle import ref_py as R
+    """Perturbed x around two more problems; the reference library's cost and gradient there are in tests/golden/ref_live.npz
+    (make_live_golden.py)."""
+    import make_live_golden as mkl
 
-    if not R.mid_available():
-        pytest.skip("oracle/_ref/libref_mid.so not present")
-    rng = np.random.default_rng(3)
-    for N in (4, 9):
-        init_s, final_s, Q, rots, x = mk.problem(N, 500 + N)
-        for over in mk.CONFIGS.values():
-            cfg = api.mid_default_config(**over)
-            i_s, f_s, q, r, _ = api._mid_args(init_s, final_s, Q, rots)
-            for _ in range(3):
-                xx = x + rng.normal(0, 0.2, x.shape)
-                c, g = api.mid_cost(init_s, final_s, Q, rots, xx, cfg)
-                cr, gr = R.mid_cost(cfg, N, i_s, f_s, q, r, xx)
-                assert abs(c - cr) <= 1e-13 * abs(cr) and np.linalg.norm(g - gr) <= 1e-11 * np.linalg.norm(gr)
+    live = np.load(os.path.join(HERE, "golden", "ref_live.npz"))
+    n = 0
+    for key, N, over, prob, xx in mkl.mid_draws():
+        assert np.array_equal(xx, live[key + "_x"]), key
+        c, g = api.mid_cost(*prob, xx, api.mid_default_config(**over))
+        cr, gr = float(live[key + "_cost"]), live[key + "_grad"]
+        assert abs(c - cr) <= 1e-13 * abs(cr) and np.linalg.norm(g - gr) <= 1e-11 * np.linalg.norm(gr), key
+        n += 1
+    assert n == 12
 
 
 def test_mid_end_argument_checks():

@@ -1,5 +1,9 @@
-"""Host-only check of the LMBM plug-in (svsdf_lmbm_*): run by tests/test_capi_host.py in a subprocess whose loader path holds a
-libgfortran.so.5 (the reference's prebuilt lmbm.so needs one; scipy bundles a copy).  Prints one JSON line.
+"""Host-only check of the LMBM plug-in (svsdf_lmbm_*), run by tests/test_capi_host.py in a subprocess.  Prints one JSON line.
+
+    python tests/tools/lmbm_plugin_check.py [--lib PATH]
+
+PATH is any library exporting lmbm::lmbm_optimize: tests/cpp/lmbm_standin.cpp built by the test, or by default oracle/_ref/lmbm.so
+(the reference's prebuilt binary, which needs a libgfortran.so.5 on the loader path; scipy bundles a copy).
 
 1. svsdf_lmbm_minimize on a non-smooth test function == calling lmbm::lmbm_optimize of the same file directly (ctypes), bit for bit.
 2. Two handles opened as PRIVATE COPIES minimise two different functions concurrently from two threads and each returns what it returns
@@ -38,10 +42,14 @@ def ensure_loader_path():
 
 
 def main():
-    if not os.path.exists(LMBM):
+    global LMBM
+    if "--lib" in sys.argv:  # a self-contained library: no Fortran runtime to find
+        LMBM = os.path.abspath(sys.argv[sys.argv.index("--lib") + 1])
+    elif not os.path.exists(LMBM):
         print(json.dumps({"unavailable": "oracle/_ref/lmbm.so not present"}))
         return
-    ensure_loader_path()
+    else:
+        ensure_loader_path()
     import numpy as np
 
     sys.path.insert(0, ROOT)

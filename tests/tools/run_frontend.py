@@ -24,7 +24,7 @@ peaks = {}
 pp = os.path.join(os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))), "MEASURED_PEAKS.json")
 if os.path.exists(pp):
     peaks = json.load(open(pp))
-hbm = peaks.get("hbm_gbs", 6650.0)
+hbm = peaks.get("hbm_gbs", 3350.0)
 # CPU: the oracle's kernelConv<true> over a crop, all host threads (OpenMP), scaled by cell count
 n = 400
 crop = gm.occ[:n, :n]
@@ -34,7 +34,7 @@ rec = {"kernel": "k_cspace", "map_cells": [X, Y], "yaw_kernels": K, "kernel_size
        "kernel_conv_per_s_gpu": cells / (ms_med * 1e-3), "front_init_s": t_init,
        "roofline": {"bound": "hbm", "algorithmic_bytes": out_bytes + in_bytes, "achieved": (out_bytes + in_bytes) / (ms_med * 1e-3) / 1e9,
                     "peak": hbm, "unit": "GB/s", "frac": (out_bytes + in_bytes) / (ms_med * 1e-3) / 1e9 / hbm,
-                    "peak_source": "MEASURED_PEAKS.json" if peaks else "fallback 6650 GB/s"},
+                    "peak_source": "MEASURED_PEAKS.json" if peaks else "H100 SXM data sheet, 3350 GB/s"},
        "cpu": {"kernel_conv_per_s": K * n * n / t_cpu, "threads": O.num_procs(), "sample": f"{n} x {n} crop, {K} kernels, oracle kernelConv<true> restatement"},
        "speedup": (cells / (ms_med * 1e-3)) / (K * n * n / t_cpu)}
 # node expansion (AstarPathSearcher::process neighbour loop) for 4096 nodes at once — one node per problem of the batch mode —

@@ -3,10 +3,11 @@ back_end_optimizer.cpp:29) driving THIS library's cost callback on the GPU: `svs
 signature (lmbm.h:206-209), so its address is handed to lmbm_optimize as is — no Python in the loop (INTEGRATION.md §2).
 
     python tests/tools/run_lmbm_gpu.py [--points 400 --pieces 8 --clearance 2.6 --seed-map 777 --max-evals 400] [--trace out.npz]
+                                       [--lib PATH]
 
-Needs oracle/_ref/lmbm.so (copied there from /root/reference by __graft_entry__.build(); git-ignored, travels to the GPU
-box) and a libgfortran.so.5 (scipy bundles one; symlinked into oracle/_ref/).  The script re-executes itself with
-LD_LIBRARY_PATH set.  --trace records every (x, f) through a thin Python wrapper instead (slower; used by the tests).
+By default it needs oracle/_ref/lmbm.so (copied there by __graft_entry__.build() where the reference checkout is present;
+git-ignored) and a libgfortran.so.5 (scipy bundles one; symlinked into oracle/_ref/), and re-executes itself with
+LD_LIBRARY_PATH set.  --lib runs any other library exporting lmbm::lmbm_optimize instead (tests/cpp/lmbm_standin.cpp).  --trace records every (x, f) through a thin Python wrapper instead (slower; used by the tests).
 Prints one JSON line."""
 import argparse
 import ctypes as C
@@ -58,13 +59,18 @@ def main():
     ap.add_argument("--seed-map", type=int, default=777)
     ap.add_argument("--max-evals", type=int, default=400)
     ap.add_argument("--trace", default=None)
+    ap.add_argument("--lib", default=None, help="library exporting lmbm::lmbm_optimize (default: oracle/_ref/lmbm.so)")
     ap.add_argument("--plugin", action="store_true", help="go through the library's own plug-in (svsdf_set_lmbm_library + svsdf_optimize) "
                                                           "instead of calling lmbm_optimize from here")
     args = ap.parse_args()
-    if not os.path.exists(LMBM):
-        print(json.dumps({"unavailable": "oracle/_ref/lmbm.so not present (built only where /root/reference exists)"}))
+    global LMBM
+    if args.lib:  # a self-contained library: no Fortran runtime to find
+        LMBM = os.path.abspath(args.lib)
+    elif not os.path.exists(LMBM):
+        print(json.dumps({"unavailable": "oracle/_ref/lmbm.so not present (copied there only where the reference checkout is present)"}))
         return
-    ensure_loader_path()
+    else:
+        ensure_loader_path()
     import numpy as np
 
     sys.path.insert(0, ROOT)
