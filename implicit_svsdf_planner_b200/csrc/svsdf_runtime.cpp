@@ -139,6 +139,11 @@ struct svsdf_ctx {
     // on small inputs; -1 = not set
     int force_grid_outer = -1;
     int force_batched = -1;
+    // test hooks of the interior branch, read ONCE at svsdf_create (SVSDF_FORCE_GSIP_WIDE = 0 / 1: the 8-warp or the 22-warp
+    // k_gsip for queries and cost evaluations alike; SVSDF_FORCE_GRID_GSIP = n > 0: k_gsip grid, 1 = one CTA walks every
+    // slot); -1 = not set
+    int force_gsip_wide = -1;
+    int force_grid_gsip = -1;
 };
 
 namespace {
@@ -425,8 +430,10 @@ int run_kernels(svsdf_ctx *ctx, const double *d_points, int64_t P, bool reduce, 
     A.gsip_piece = ctx->d_gsip_piece;
     A.eval_counter = ctx->count_evals ? ctx->d_eval_counter : nullptr;
     // previous evaluation had few interior points -> 22-warp CTAs (one warp per ring sample, lower latency)
-    const int gsip_wide = (reduce && ctx->last_n_inside >= 0 && ctx->last_n_inside <= ctx->sm_count) ? 1 : 0;
-    const int grid_gsip = gsip_wide ? ctx->sm_count : ctx->sm_count * ctx->occ_gsip;
+    int gsip_wide = (reduce && ctx->last_n_inside >= 0 && ctx->last_n_inside <= ctx->sm_count) ? 1 : 0;
+    if (ctx->force_gsip_wide >= 0) gsip_wide = ctx->force_gsip_wide ? 1 : 0;  // test hook
+    int grid_gsip = gsip_wide ? ctx->sm_count : ctx->sm_count * ctx->occ_gsip;
+    if (ctx->force_grid_gsip > 0) grid_gsip = ctx->force_grid_gsip;  // test hook
     if (!gsip) CK(cudaMemsetAsync(ctx->d_n_inside, 0, sizeof(int), ctx->stream));
     size_t smem = outer_smem_doubles(A.blob_doubles, N) * sizeof(double);
     if (smem > 200 * 1024) {
@@ -1000,6 +1007,8 @@ int svsdf_create(const svsdf_config *cfg, svsdf_ctx **out) {
     ctx->strict = cfg->strict_fp != 0;
     if (const char *fg = std::getenv("SVSDF_FORCE_GRID_OUTER")) ctx->force_grid_outer = std::atoi(fg);
     if (const char *fb = std::getenv("SVSDF_FORCE_BATCHED")) ctx->force_batched = std::atoi(fb);
+    if (const char *fw = std::getenv("SVSDF_FORCE_GSIP_WIDE")) ctx->force_gsip_wide = std::atoi(fw);
+    if (const char *fg = std::getenv("SVSDF_FORCE_GRID_GSIP")) ctx->force_grid_gsip = std::atoi(fg);
     auto fail = [&](cudaError_t e) {
         std::fprintf(stderr, "svsdf_create: %s\n", cudaGetErrorString(e));
         svsdf_destroy(ctx);

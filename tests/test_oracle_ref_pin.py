@@ -6,7 +6,8 @@ Two layers:
     the reference's code (tests/golden/make_ref_pin_golden.py); the oracle must reproduce every per-point quantity BIT FOR
     BIT — shape values and FD gradients for all 18 functors, initShape byte kernels, Piece<5>/Trajectory<5> samples,
     getTrueSDFofSweptVolume (sdf, t*, gradient; outside and GSIP points), smoothedL1, tau<->T — and every summed quantity
-    (cost, gradC, gradT, f, g, MINCO) to summation-order rounding;
+    (cost, gradC, gradT, f, g, MINCO) to summation-order rounding; tests/golden/ref_pin_gsip_edges.npz
+    (tests/golden/make_gsip_edges_golden.py) adds the edge cases of the interior branch, per point and bit for bit;
   * 1e5 seeded random points per shape against digests of the reference's outputs on them (tests/golden/ref_live.npz,
     tests/golden/make_live_golden.py).
 Variant mapping: reference "glibc" <-> oracle "glibc"; reference "portable" (its libm calls redirected to the pinned
@@ -23,6 +24,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 GOLD = os.path.join(HERE, "golden")
 sys.path.insert(0, GOLD)
 import make_live_golden as mkl  # noqa: E402  (the seeded inputs of the digest comparison)
+import make_gsip_edges_golden as mkg  # noqa: E402  (the edge scenes of the interior branch)
 PAIRS = [("glibc", "glibc"), ("portable", "default")]  # (reference variant, oracle variant)
 
 
@@ -165,6 +167,27 @@ def test_path_matches_reference_code(oracle_mod, gpath, key, rv, ov):
     gq, gt = oracle_mod.minco_propagate(g[f"{key}_init_s"], g[f"{key}_final_s"], g[f"{key}_q"], T, g[f"{key}_gdC_{rv}"].reshape(3, 6 * N).T, g[f"{key}_gdT_{rv}"])
     assert np.linalg.norm(np.asarray(gq) - g[f"{key}_adjP_{rv}"]) <= 1e-12 * np.linalg.norm(g[f"{key}_adjP_{rv}"])
     assert np.linalg.norm(np.asarray(gt) - g[f"{key}_adjT_{rv}"]) <= 1e-12 * np.linalg.norm(g[f"{key}_adjT_{rv}"])
+
+
+@pytest.mark.parametrize("key", mkg.SCENES)
+@pytest.mark.parametrize("rv,ov", PAIRS)
+def test_gsip_edge_scenes_match_reference_code_bitwise(oracle_mod, key, rv, ov):
+    """The interior branch's own edge cases (tests/golden/make_gsip_edges_golden.py): the velocity fallback scanning forward,
+    backward or not at all, the ring origin at zero velocity, ring samples that tie, an outer sdf of exactly 0.0 and the 9-round
+    cap.  The oracle must compute what the reference's code does there, per point and bit for bit, outer solve and GSIP alike."""
+    g = np.load(os.path.join(GOLD, "ref_pin_gsip_edges.npz"))
+    shape, T, co, pts = mkg.scene(key)
+    assert str(g[f"{key}_shape"]) == shape and np.array_equal(g[f"{key}_T"], T) and np.array_equal(g[f"{key}_coeffs"], co)
+    assert np.array_equal(g[f"{key}_points"], pts)  # the builders still make the committed inputs
+    orc = oracle_mod.Oracle(shape, threads=min(8, oracle_mod.num_procs()), variant=ov)
+    orc.set_traj(T, co)
+    sdf, tstar, grad, rounds = orc.query(pts)
+    assert bits_differ(sdf, g[f"{key}_sdf_{rv}"]) == 0
+    assert bits_differ(tstar, g[f"{key}_tstar_{rv}"]) == 0
+    assert bits_differ(grad, g[f"{key}_grad_{rv}"]) == 0
+    assert (rounds > 0).sum() >= 20
+    so, to, go = orc.query_outer(pts)
+    assert bits_differ(so, g[f"{key}_osdf_{rv}"]) + bits_differ(to, g[f"{key}_otstar_{rv}"]) + bits_differ(go, g[f"{key}_ograd_{rv}"]) == 0
 
 
 @pytest.mark.parametrize("rv,ov", PAIRS)
