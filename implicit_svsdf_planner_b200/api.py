@@ -110,6 +110,7 @@ EXPORTED_SYMBOLS = [
     "svsdf_mid_default_config", "svsdf_mid_cost", "svsdf_mid_get_ori_traj",
     "svsdf_lmbm_default_params", "svsdf_lmbm_open", "svsdf_lmbm_close", "svsdf_lmbm_last_error", "svsdf_lmbm_minimize", "svsdf_set_lmbm_library", "svsdf_read_obj", "svsdf_free", "svsdf_mesh_fwn_host",
     "svsdf_front_init", "svsdf_front_get_kernels", "svsdf_front_cspace", "svsdf_front_check_kernel_value", "svsdf_front_expand", "svsdf_front_astar",
+    "svsdf_front_astar_device",
 ]
 
 
@@ -139,6 +140,7 @@ def lib():
     L.svsdf_front_check_kernel_value.argtypes = [vp, C.c_int64, dp, vp, vp, dp]
     L.svsdf_front_expand.argtypes = [vp, C.c_int64, vp, dp, vp, dp, vp]
     L.svsdf_front_astar.argtypes = [vp, C.c_int, dp, dp, C.c_int, dp, vp, vp, C.POINTER(C.c_int64)]
+    L.svsdf_front_astar_device.argtypes = [vp, C.c_int, dp, dp, C.c_int, C.c_int64, dp, vp, vp, vp, C.POINTER(C.c_float)]
     L.svsdf_set_points.argtypes = [vp, dp, C.c_int64, C.c_int]
     L.svsdf_set_points_device.argtypes = [vp, vp, C.c_int64]
     L.svsdf_set_traj.argtypes = [vp, C.c_int, dp, dp]
@@ -662,6 +664,23 @@ class Context:
         self._ck(lib().svsdf_front_astar(self.h, n, _p(st), _p(go), int(max_path), _p(path), ln.ctypes.data_as(C.c_void_p),
                                          ex.ctypes.data_as(C.c_void_p), C.byref(rounds)), "svsdf_front_astar")
         return [path[q, : ln[q]].copy() if ln[q] else None for q in range(n)], ex, rounds.value
+
+    def front_astar_device(self, start_xy, goal_xy, max_path=1024, max_expansions=1 << 30):
+        """The searches of front_astar, each run whole on the device in one launch: (paths: list of [len, 3] arrays or None,
+        expansions [n], status [n] (0 outside the map, 1 found, 2 open list empty, 3 max_expansions reached, 4 longer than
+        max_path, -1 internal guard), kernel ms)."""
+        st = _f64(start_xy).reshape(-1, 2)
+        go = _f64(goal_xy).reshape(-1, 2)
+        n = st.shape[0]
+        path = np.zeros((n, max(int(max_path), 0), 3))
+        ln = np.zeros(n, dtype=np.int32)
+        ex = np.zeros(n, dtype=np.int32)
+        status = np.zeros(n, dtype=np.int32)
+        ms = C.c_float()
+        self._ck(lib().svsdf_front_astar_device(self.h, n, _p(st), _p(go), int(max_path), int(max_expansions), _p(path),
+                                                ln.ctypes.data_as(C.c_void_p), ex.ctypes.data_as(C.c_void_p),
+                                                status.ctypes.data_as(C.c_void_p), C.byref(ms)), "svsdf_front_astar_device")
+        return [path[q, : ln[q]].copy() if ln[q] else None for q in range(n)], ex, status, ms.value
 
     def sincos(self, x):
         x = _f64(x).reshape(-1)

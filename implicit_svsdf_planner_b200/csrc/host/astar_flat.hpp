@@ -1,9 +1,9 @@
 // host/astar_flat.hpp — the per-search bookkeeping of the A* front end WITHOUT containers: flat arrays and a binary heap, written so
-// that the same code compiles for the device (SVSDF_HD).  It is the core a device-side search needs — one search per warp / CTA keeping
-// its open list in global memory, no host round trip per expansion (DESIGN.md §7 rank 3 (v): the lock-step host version spends ~0.1 ms
-// per round on launches, copies and the host's open-list pass).  The device kernel around it is not built yet; this file is checked on
-// the host: tests/cpp/astar_host_main.cpp runs it beside host/astar.hpp and the oracle's literal AstarPathSearch and requires identical
-// paths and expansion counts.
+// that the same code compiles for the device (SVSDF_HD).  k_astar_search (csrc/svsdf_frontend.cu, svsdf_front_astar_device) runs it in
+// thread 0 of one CTA per search, with its arrays and heap in global memory and the node test spread over the CTA's warps: no host
+// round trip per expansion (DESIGN.md §7 rank 3 (vi); the lock-step host version of (v) pays a launch, two copies and the host's
+// open-list pass per round).  The same code is also checked on the host: tests/cpp/astar_host_main.cpp runs it beside host/astar.hpp
+// and the oracle's literal AstarPathSearch and requires identical paths and expansion counts.
 //
 // Same semantics as host/astar.hpp (AstarPathSearcher::AstarPathSearch / getPath, front_end_Astar.hpp:243-390):
 //   * node states 0 unseen / 1 open / -1 closed, yaw fixed when a node is first seen, open nodes improved in place WITHOUT re-keying,
@@ -43,6 +43,11 @@ struct FlatSearch {
     int cur;
     int64_t expansions;
     int status;  // 0 running, 1 path found (cur = goal slot), 2 open list empty, 3 expansion limit, -1 heap overflow
+
+    // Only id[] has to be cleared between searches (and father[] of slots a path can reach is written when they are first
+    // opened): g / f / yaw / father of a slot are written when its id goes from 0 to 1 and read only while it is non-zero.  The
+    // start cell's grid slot is marked open without a father; it is never pushed (nothing improves g = 0), so never popped and
+    // never a father.
 
     SVSDF_HD static double heuristic(int ax, int ay, int bx, int by) {  // getHeu (front_end_Astar.hpp:165-183), dz = 0
         const double p = 1.0 / 1000;
@@ -88,7 +93,7 @@ struct FlatSearch {
     SVSDF_HD void slot_xy(int s, int &x, int &y) const {
         if (s == NS) { x = sx; y = sy; } else { x = s / Y; y = s % Y; }
     }
-    // AstarPathSearch up to the first pop (:243-300).  The caller has zeroed id[] and set father[] to -1.
+    // AstarPathSearch up to the first pop (:243-300).  The caller has zeroed id[].
     SVSDF_HD void begin(int sx_, int sy_, int gx_, int gy_) {
         sx = sx_; sy = sy_; gx = gx_; gy = gy_;
         heap_n = 0; seq = 0; cur = -1; expansions = 0; status = 0;
@@ -134,19 +139,22 @@ struct FlatSearch {
                 }
             }
     }
-    // getPath (:370-390): number of nodes from the start to `cur`; out (optional, capacity max_path): (x, y, yaw) per node, start first
+    // getPath (:370-390): number of nodes from the start to `cur`; out (optional, capacity max_path): (x, y, yaw) per node, start first.
+    // Both walks stop after NS + 1 nodes (there are only NS + 1 slots); a longer father chain returns -1.  A valid search has none:
+    // edge costs are positive and the self-neighbour never improves g, so father pointers cannot form a cycle.
     SVSDF_HD int path(double ox, double oy, double res, int max_path, double *out) const {
         int n = 1;
-        for (int s = cur; father[s] != -1; s = father[s]) ++n;
+        for (int s = cur; father[s] != -1; s = father[s])
+            if (++n > NS + 1) return -1;
         if (n > max_path || !out) return n;
-        int k = n - 1;
-        for (int s = cur;; s = father[s], --k) {
+        int s = cur;
+        for (int k = n - 1; k >= 0; --k) {
             int x, y;
             slot_xy(s, x, y);
             out[3 * k] = (x + 0.5) * res + ox;  // getGridCubeCenter
             out[3 * k + 1] = (y + 0.5) * res + oy;
             out[3 * k + 2] = yaw[s];
-            if (father[s] == -1) break;
+            s = father[s];
         }
         return n;
     }

@@ -19,6 +19,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "host/astar_flat.hpp"
 #include "svsdf_shapes.cuh"
 #include "svsdf_types.h"
 
@@ -157,25 +158,18 @@ __device__ __forceinline__ int grid_index_1d(double p, double lo, double hi, dou
     return i;
 }
 
-// The neighbour loop of AstarPathSearcher::process (front_end_Astar.hpp:192-240), one warp per (node, neighbour cell):
+// The neighbour loop of AstarPathSearcher::process (front_end_Astar.hpp:192-240) for ONE (node, neighbour cell), run by a whole warp
+// (every lane passes the same arguments):
 //   cond = isIndexValid(vi) && !isIndexOccupiedFlate(vi, 0) && checkKernelValue(fy, cy, vi) && checkSubSWCollision(state1, state2, aabb)
 // The kernel test is the literal byte-wise one (all lanes in lockstep); the sub-swept-volume test (sw_manager.hpp:1171-1210)
 // spreads the occupied cells of the box around the child (getPointsInAABB2D, PCSmap_manager.h:137-158) over the lanes,
-// each lane walking the kt samples of its cell.
+// each lane walking the kt samples of its cell.  Returns the parts mask (bit 0 valid and free, bit 1 kernel test, bit 2
+// sub-swept-volume test; the node passes iff it is 7) and the child yaw in cy.  Shared by k_expand_nodes and k_astar_search.
 template <int SHAPE, bool XFORM>
-__global__ void __launch_bounds__(256) k_expand_nodes(const __grid_constant__ ShapeParams S, const __grid_constant__ FrontParams F,
-                                                      const __grid_constant__ SubSwParams P, const unsigned char *map,
-                                                      const unsigned char *kbytes, int64_t n, const int *node_ij, const double *node_yaw,
-                                                      unsigned char *ok_out, double *child_yaw_out, unsigned char *parts_out) {
-    const int lane = threadIdx.x & 31;
-    const int64_t w = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    if (w >= 9 * n) return;
-    const int64_t q = w / 9;
-    const int nb = (int)(w % 9);
-    const int ix = node_ij[2 * q], iy = node_ij[2 * q + 1];
+__device__ __forceinline__ unsigned node_test(const ShapeParams &S, const FrontParams &F, const SubSwParams &P, const unsigned char *map,
+                                              const unsigned char *kbytes, int ix, int iy, double fy, int nb, int lane, double &cy) {
     const int vx = ix + (nb / 3 - 1), vy = iy + (nb % 3 - 1);
-    const double fy = node_yaw[q];
-    double cy = fy;
+    cy = fy;
     unsigned parts = 0;
     const bool valid = vx >= 0 && vx < F.X && vy >= 0 && vy < F.Y;
     if (valid) {
@@ -247,10 +241,108 @@ __global__ void __launch_bounds__(256) k_expand_nodes(const __grid_constant__ Sh
         }
         if (!hit) parts |= 4u;
     }
+    return parts;
+}
+
+// svsdf_front_expand: one warp per (node, neighbour cell)
+template <int SHAPE, bool XFORM>
+__global__ void __launch_bounds__(256) k_expand_nodes(const __grid_constant__ ShapeParams S, const __grid_constant__ FrontParams F,
+                                                      const __grid_constant__ SubSwParams P, const unsigned char *map,
+                                                      const unsigned char *kbytes, int64_t n, const int *node_ij, const double *node_yaw,
+                                                      unsigned char *ok_out, double *child_yaw_out, unsigned char *parts_out) {
+    const int lane = threadIdx.x & 31;
+    const int64_t w = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (w >= 9 * n) return;
+    const int64_t q = w / 9;
+    double cy;
+    const unsigned parts = node_test<SHAPE, XFORM>(S, F, P, map, kbytes, node_ij[2 * q], node_ij[2 * q + 1], node_yaw[q], (int)(w % 9), lane, cy);
     if (lane == 0) {
         ok_out[w] = (parts == 7u) ? 1 : 0;
         child_yaw_out[w] = cy;
         if (parts_out) parts_out[w] = (unsigned char)parts;
+    }
+}
+
+// svsdf_front_astar_device: whole searches, one CTA per search in flight (AstarPathSearch / getPath, front_end_Astar.hpp:243-390).
+// Thread 0 runs the bookkeeping of host/astar_flat.hpp (pop, goal and budget tests, neighbour updates, path walk); the popped
+// node goes through shared memory to the 9 warps, warp w tests neighbour w with node_test, and ok9 / yaw9 come back the same way.
+// The grid is persistent and takes search indices from a global counter (reset by the host before the launch): no CTA waits
+// for another, so nothing depends on how many CTAs are resident.  CTA b owns slot b of the pool: id int8, g / f / yaw double,
+// father int32 and the heap, each NS + 1 long (NS = X * Y; slot NS is the start-node object).
+//   * Only id[] is cleared (by the whole CTA) before each search: every other array is written before it is read (see FlatSearch).
+//   * Heap capacity NS + 1 is enough: a slot is pushed only when its id goes from 0 (unseen) or -1 (closed) to 1 (open) and
+//     leaves the heap when it is popped (id = -1), so each of the NS + 1 slots has at most one live entry; the start cell is marked
+//     open but never pushed.  The overflow status (-1) stays as a guard.
+//   * Every loop is bounded: the expansion loop by max_expansions + 1 pops (pop_next stops at the budget), the path walk by NS + 1.
+constexpr int kAstarWarps = 9;
+
+template <int SHAPE, bool XFORM>
+__global__ void __launch_bounds__(kAstarWarps * 32, 2) k_astar_search(const __grid_constant__ ShapeParams S, const __grid_constant__ FrontParams F,
+                                                                   const __grid_constant__ SubSwParams P, const unsigned char *map,
+                                                                   const unsigned char *kbytes, const __grid_constant__ AstarArgs A) {
+    __shared__ host::FlatSearch fs;  // thread 0's search state: in shared memory, so that it costs the node test no registers
+    __shared__ int s_q, s_go, s_cx, s_cy;
+    __shared__ double s_yaw;
+    __shared__ unsigned char s_ok[9];
+    __shared__ double s_cyaw[9];
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int NS = F.X * F.Y;
+    int8_t *id;
+    {
+        unsigned char *slot = A.pool + (size_t)blockIdx.x * A.slot_bytes;
+        host::FlatHeapEntry *heap = reinterpret_cast<host::FlatHeapEntry *>(slot);
+        double *g = reinterpret_cast<double *>(heap + (NS + 1));
+        int32_t *father = reinterpret_cast<int32_t *>(g + 3 * (NS + 1));
+        id = reinterpret_cast<int8_t *>(father + (NS + 1));
+        if (tid == 0) {
+            fs.X = F.X; fs.Y = F.Y; fs.NS = NS;
+            fs.heap = heap; fs.heap_cap = NS + 1;
+            fs.g = g; fs.f = g + (NS + 1); fs.yaw = g + 2 * (NS + 1);
+            fs.father = father; fs.id = id;
+        }
+    }
+    for (int round = 0; round < A.n; ++round) {  // a CTA runs at most n searches
+        if (tid == 0) s_q = atomicAdd(A.next, 1);
+        __syncthreads();
+        const int q = s_q;
+        if (q >= A.n) break;
+        const int4 c = reinterpret_cast<const int4 *>(A.cells)[q];
+        if (c.x < 0) {  // start or goal outside the map (isInMap): the search does not run
+            if (tid == 0) { A.len[q] = 0; A.expansions[q] = 0; A.status[q] = 0; }
+            __syncthreads();
+            continue;
+        }
+        for (int i = tid; i <= NS; i += blockDim.x) id[i] = 0;
+        __syncthreads();
+        if (tid == 0) fs.begin(c.x, c.y, c.z, c.w);
+        for (int64_t it = 0; it <= A.max_expansions; ++it) {
+            if (tid == 0) {
+                int cx = 0, cy = 0;
+                double cyaw = 0.0;
+                s_go = fs.pop_next(A.max_expansions, cx, cy, cyaw) ? 1 : 0;
+                s_cx = cx; s_cy = cy; s_yaw = cyaw;
+            }
+            __syncthreads();
+            if (!s_go) break;
+            {
+                double cyw;
+                const unsigned parts = node_test<SHAPE, XFORM>(S, F, P, map, kbytes, s_cx, s_cy, s_yaw, warp, lane, cyw);
+                if (lane == 0) { s_ok[warp] = (parts == 7u) ? 1 : 0; s_cyaw[warp] = cyw; }
+            }
+            __syncthreads();
+            if (tid == 0) fs.apply(s_cx, s_cy, s_ok, s_cyaw);
+        }
+        if (tid == 0) {
+            int st = fs.status == 0 ? -1 : fs.status, len = 0;  // still running after max_expansions + 1 pops: cannot happen
+            if (st == 1) {
+                const int np = fs.path(F.ox, F.oy, F.map_res, A.max_path, A.paths + (size_t)q * A.max_path * 3);
+                if (np < 0) st = -1;
+                else if (np > A.max_path) st = 4;
+                else len = np;
+            }
+            A.len[q] = len; A.expansions[q] = (int)fs.expansions; A.status[q] = st;
+        }
+        __syncthreads();  // the next search clears this slot's id[] only after thread 0 is done with it
     }
 }
 
@@ -271,31 +363,30 @@ cudaError_t launch_cells_t(const ShapeParams &S, const FrontParams &F, const dou
     return cudaGetLastError();
 }
 
+// grid <= 0: only report the resident CTAs per SM (occupancy query) in *ctas_per_sm
+template <int SHAPE, bool XFORM>
+cudaError_t launch_astar_t(const ShapeParams &S, const FrontParams &F, const SubSwParams &P, const unsigned char *map, const unsigned char *kbytes,
+                           const AstarArgs &A, int grid, int *ctas_per_sm, cudaStream_t st) {
+    if (grid <= 0) return cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, k_astar_search<SHAPE, XFORM>, kAstarWarps * 32, 0);
+    k_astar_search<SHAPE, XFORM><<<grid, kAstarWarps * 32, 0, st>>>(S, F, P, map, kbytes, A);
+    return cudaGetLastError();
+}
+
 }  // namespace
+
+// The analytic functors the front end is defined for; Polygon / mesh: the reference defines no rotated kernels for them
+#define SVSDF_FRONT_SHAPES(CASE)                                                                                                 \
+    CASE(SH_STAR) CASE(SH_HORSESHOE) CASE(SH_PIE) CASE(SH_PIE2) CASE(SH_ARC) CASE(SH_TUNNEL) CASE(SH_CUTDISK) CASE(SH_TRAPEZOID) \
+    CASE(SH_RHOMBUS) CASE(SH_HEART) CASE(SH_ROUNDEDX) CASE(SH_BIGX) CASE(SH_ROUNDEDCROSS) CASE(SH_VESICA) CASE(SH_MOON)         \
+    CASE(SH_UNEVENCAPSULE) CASE(SH_CIRCLE)
 
 cudaError_t launch_front_cells(const ShapeParams &S, const FrontParams &F, const double *yaws, unsigned char *cells, cudaStream_t st) {
     switch (S.id) {
 #define SVSDF_CASE(ID) \
     case ID: return S.has_xform ? launch_cells_t<ID, true>(S, F, yaws, cells, st) : launch_cells_t<ID, false>(S, F, yaws, cells, st);
-        SVSDF_CASE(SH_STAR)
-        SVSDF_CASE(SH_HORSESHOE)
-        SVSDF_CASE(SH_PIE)
-        SVSDF_CASE(SH_PIE2)
-        SVSDF_CASE(SH_ARC)
-        SVSDF_CASE(SH_TUNNEL)
-        SVSDF_CASE(SH_CUTDISK)
-        SVSDF_CASE(SH_TRAPEZOID)
-        SVSDF_CASE(SH_RHOMBUS)
-        SVSDF_CASE(SH_HEART)
-        SVSDF_CASE(SH_ROUNDEDX)
-        SVSDF_CASE(SH_BIGX)
-        SVSDF_CASE(SH_ROUNDEDCROSS)
-        SVSDF_CASE(SH_VESICA)
-        SVSDF_CASE(SH_MOON)
-        SVSDF_CASE(SH_UNEVENCAPSULE)
-        SVSDF_CASE(SH_CIRCLE)
+        SVSDF_FRONT_SHAPES(SVSDF_CASE)
 #undef SVSDF_CASE
-        default: return cudaErrorInvalidValue;  // Polygon / mesh: the reference defines no rotated kernels for them
+        default: return cudaErrorInvalidValue;
     }
 }
 
@@ -308,27 +399,25 @@ cudaError_t launch_front_expand(const ShapeParams &S, const FrontParams &F, cons
     case ID:                                                                                                                        \
         return S.has_xform ? launch_expand_t<ID, true>(S, F, P, map, kbytes, n, node_ij, node_yaw, ok_out, child_yaw_out, parts_out, st) \
                            : launch_expand_t<ID, false>(S, F, P, map, kbytes, n, node_ij, node_yaw, ok_out, child_yaw_out, parts_out, st);
-        SVSDF_CASE(SH_STAR)
-        SVSDF_CASE(SH_HORSESHOE)
-        SVSDF_CASE(SH_PIE)
-        SVSDF_CASE(SH_PIE2)
-        SVSDF_CASE(SH_ARC)
-        SVSDF_CASE(SH_TUNNEL)
-        SVSDF_CASE(SH_CUTDISK)
-        SVSDF_CASE(SH_TRAPEZOID)
-        SVSDF_CASE(SH_RHOMBUS)
-        SVSDF_CASE(SH_HEART)
-        SVSDF_CASE(SH_ROUNDEDX)
-        SVSDF_CASE(SH_BIGX)
-        SVSDF_CASE(SH_ROUNDEDCROSS)
-        SVSDF_CASE(SH_VESICA)
-        SVSDF_CASE(SH_MOON)
-        SVSDF_CASE(SH_UNEVENCAPSULE)
-        SVSDF_CASE(SH_CIRCLE)
+        SVSDF_FRONT_SHAPES(SVSDF_CASE)
 #undef SVSDF_CASE
         default: return cudaErrorInvalidValue;
     }
 }
+
+cudaError_t launch_front_astar(const ShapeParams &S, const FrontParams &F, const SubSwParams &P, const unsigned char *map,
+                               const unsigned char *kbytes, const AstarArgs &A, int grid, int *ctas_per_sm, cudaStream_t st) {
+    switch (S.id) {
+#define SVSDF_CASE(ID)                                                                                            \
+    case ID:                                                                                                      \
+        return S.has_xform ? launch_astar_t<ID, true>(S, F, P, map, kbytes, A, grid, ctas_per_sm, st)             \
+                           : launch_astar_t<ID, false>(S, F, P, map, kbytes, A, grid, ctas_per_sm, st);
+        SVSDF_FRONT_SHAPES(SVSDF_CASE)
+#undef SVSDF_CASE
+        default: return cudaErrorInvalidValue;
+    }
+}
+#undef SVSDF_FRONT_SHAPES
 
 cudaError_t launch_front_cspace(const FrontParams &F, const unsigned char *map, const unsigned *rowmask, unsigned *out, cudaStream_t st) {
     const int64_t n = (int64_t)F.kernel_count * F.X * F.out_words;

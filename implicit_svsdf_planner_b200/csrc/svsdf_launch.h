@@ -33,6 +33,9 @@ cudaError_t launch_front_cells(const ShapeParams &S, const FrontParams &F, const
 cudaError_t launch_front_expand(const ShapeParams &S, const FrontParams &F, const SubSwParams &P, const unsigned char *map,
                                 const unsigned char *kbytes, int64_t n, const int *node_ij, const double *node_yaw, unsigned char *ok_out,
                                 double *child_yaw_out, unsigned char *parts_out, cudaStream_t st);
+// grid <= 0: no launch, *ctas_per_sm = resident k_astar_search CTAs per SM for this shape
+cudaError_t launch_front_astar(const ShapeParams &S, const FrontParams &F, const SubSwParams &P, const unsigned char *map,
+                               const unsigned char *kbytes, const AstarArgs &A, int grid, int *ctas_per_sm, cudaStream_t st);
 cudaError_t launch_front_cspace(const FrontParams &F, const unsigned char *map, const unsigned *rowmask, unsigned *out, cudaStream_t st);
 cudaError_t launch_front_check(const FrontParams &F, const unsigned char *map, const unsigned char *kbytes, int64_t n, const double *father_yaw,
                                const int *ind_xy, unsigned char *ok_out, double *child_yaw_out, cudaStream_t st);

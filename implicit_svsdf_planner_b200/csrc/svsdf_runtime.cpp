@@ -65,6 +65,8 @@ struct svsdf_ctx {
     size_t cap_cspace = 0;
     unsigned char *d_front_scratch = nullptr;  // grow-only device scratch of the batched front-end calls
     size_t cap_front_scratch = 0;
+    unsigned char *d_astar_pool = nullptr;     // grow-only search slots of svsdf_front_astar_device
+    size_t cap_astar_pool = 0;
     double *d_points = nullptr;  // packed xy
     bool own_points = true;
     int64_t P = 0;
@@ -144,6 +146,9 @@ struct svsdf_ctx {
     // slot); -1 = not set
     int force_gsip_wide = -1;
     int force_grid_gsip = -1;
+    // test hook of the device A*, read ONCE at svsdf_create: SVSDF_FORCE_GRID_ASTAR = n > 0 sets k_astar_search's grid (1 = one
+    // CTA runs every search on the same slot); -1 = not set
+    int force_grid_astar = -1;
 };
 
 namespace {
@@ -951,6 +956,96 @@ int svsdf_front_astar(svsdf_ctx *ctx, int n, const double *start_xy, const doubl
     return rc;
 }
 
+int svsdf_front_astar_device(svsdf_ctx *ctx, int n, const double *start_xy, const double *goal_xy, int max_path, int64_t max_expansions,
+                             double *paths_out, int32_t *len_out, int32_t *expansions_out, int32_t *status_out, float *ms_out) {
+    if (!ctx) return SVSDF_ERR_INVALID;
+    if (n < 0 || max_path < 1 || max_expansions < 1 || (n > 0 && (!start_xy || !goal_xy || !paths_out || !len_out))) {
+        ctx->err = "svsdf_front_astar_device: needs n >= 0, max_path >= 1, max_expansions >= 1 and the start, goal, path and length arrays";
+        return SVSDF_ERR_INVALID;
+    }
+    FrontParams F;
+    int rc = front_params_with_map(ctx, F, "svsdf_front_astar_device");
+    if (rc != SVSDF_OK) return rc;
+    if (ms_out) *ms_out = 0.0f;
+    if (n == 0) return SVSDF_OK;
+    CK(cudaSetDevice(ctx->device));
+    // start / goal cells exactly as astar_batch finds them (isInMap, getGridIndex); -1: the search does not run
+    const size_t un = (size_t)n;
+    std::vector<int32_t> cells(4 * un);
+    const double xmax = F.ox + F.X * F.map_res, ymax = F.oy + F.Y * F.map_res;
+    auto in_map = [&](const double *v) { return !(v[0] < F.ox || v[1] < F.oy || v[0] > xmax || v[1] > ymax); };
+    for (size_t q = 0; q < un; ++q) {
+        const double *s = start_xy + 2 * q, *g = goal_xy + 2 * q;
+        int32_t *c = &cells[4 * q];
+        if (!in_map(s) || !in_map(g)) { c[0] = c[1] = c[2] = c[3] = -1; continue; }
+        c[0] = host::astar_grid_index(s[0], F.ox, F.map_res, F.X); c[1] = host::astar_grid_index(s[1], F.oy, F.map_res, F.Y);
+        c[2] = host::astar_grid_index(g[0], F.ox, F.map_res, F.X); c[3] = host::astar_grid_index(g[1], F.oy, F.map_res, F.Y);
+    }
+    SubSwParams P{};
+    P.half_box = (double)(F.kernel_size / 2 + 1);
+    for (double kt = 0.0; kt <= 1.0 && P.nkt < 64; kt += 0.02) P.kt[P.nkt++] = kt;  // sw_manager.hpp:1190
+    // Grid: min(n, resident CTAs, pool slots).  One slot per CTA: heap 16 B + g / f / yaw 24 B + father 4 B + id 1 B per entry, NS + 1
+    // entries, rounded to 16 bytes; the pool is grow-only and capped at kAstarPoolCap (2 GiB: 8 slots of a 2400 x 2400 map).
+    const int64_t NS = (int64_t)F.X * F.Y;
+    const int64_t slot_bytes = ((NS + 1) * 45 + 15) & ~(int64_t)15;
+    const int64_t kAstarPoolCap = (int64_t)2 << 30;
+    const int64_t fit = kAstarPoolCap / slot_bytes;
+    if (fit < 1) {
+        ctx->err = "svsdf_front_astar_device: the map is too large for one search slot of the 2 GiB pool";
+        return SVSDF_ERR_INVALID;
+    }
+    AstarArgs A{};
+    int per_sm = 0;
+    CK(launch_front_astar(ctx->shape, F, P, ctx->d_map, ctx->d_front_bytes, A, 0, &per_sm, ctx->stream));
+    int64_t grid = ctx->force_grid_astar > 0 ? ctx->force_grid_astar : std::min<int64_t>(n, (int64_t)std::max(per_sm, 1) * ctx->sm_count);
+    grid = std::min(grid, fit);
+    if ((size_t)(grid * slot_bytes) > ctx->cap_astar_pool) {
+        cudaFree(ctx->d_astar_pool);
+        ctx->d_astar_pool = nullptr;
+        ctx->cap_astar_pool = 0;
+        CK(cudaMalloc(&ctx->d_astar_pool, (size_t)(grid * slot_bytes)));
+        ctx->cap_astar_pool = (size_t)(grid * slot_bytes);
+    }
+    // One device block: cells [4n] i32 | len, expansions, status [3n] i32 | counter (padded to 16 bytes) | paths [n][max_path][3] f64.
+    // Only the lengths come back first, then at most the longest returned path of every row.
+    const size_t cells_bytes = 16 * un, out_bytes = 12 * un, head = (cells_bytes + out_bytes + 16 + 15) & ~(size_t)15;
+    const size_t row = (size_t)max_path * 3 * sizeof(double);
+    rc = front_scratch(ctx, head + un * row);
+    if (rc != SVSDF_OK) return rc;
+    rc = ensure_stage(ctx, cells_bytes + out_bytes);
+    if (rc != SVSDF_OK) return rc;
+    unsigned char *db = ctx->d_front_scratch;
+    int32_t *hb = reinterpret_cast<int32_t *>(ctx->h_stage);
+    std::memcpy(hb, cells.data(), cells_bytes);
+    A.n = n; A.max_path = max_path; A.max_expansions = max_expansions;
+    A.cells = reinterpret_cast<const int *>(db);
+    A.len = reinterpret_cast<int *>(db + cells_bytes);
+    A.expansions = A.len + un;
+    A.status = A.len + 2 * un;
+    A.next = reinterpret_cast<int *>(db + cells_bytes + out_bytes);
+    A.paths = reinterpret_cast<double *>(db + head);
+    A.pool = ctx->d_astar_pool;
+    A.slot_bytes = slot_bytes;
+    cudaError_t e = cudaMemcpyAsync(db, hb, cells_bytes, cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(A.next, 0, sizeof(int), ctx->stream);
+    if (e == cudaSuccess) e = cudaEventRecord(ctx->ev0, ctx->stream);
+    if (e == cudaSuccess) e = launch_front_astar(ctx->shape, F, P, ctx->d_map, ctx->d_front_bytes, A, (int)grid, nullptr, ctx->stream);
+    if (e == cudaSuccess) e = cudaEventRecord(ctx->ev1, ctx->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(hb, A.len, out_bytes, cudaMemcpyDeviceToHost, ctx->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+    if (e != cudaSuccess) { ctx->err = std::string("svsdf_front_astar_device: ") + cudaGetErrorString(e); return SVSDF_ERR_CUDA; }
+    ctx->launches += 1;
+    int32_t lmax = 0;
+    for (size_t q = 0; q < un; ++q) lmax = std::max(lmax, hb[q]);
+    std::memcpy(len_out, hb, un * 4);
+    if (expansions_out) std::memcpy(expansions_out, hb + un, un * 4);
+    if (status_out) std::memcpy(status_out, hb + 2 * un, un * 4);
+    if (lmax > 0) CK(cudaMemcpy2DAsync(paths_out, row, A.paths, row, (size_t)lmax * 3 * sizeof(double), un, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    if (ms_out) CK(cudaEventElapsedTime(ms_out, ctx->ev0, ctx->ev1));
+    return SVSDF_OK;
+}
+
 int svsdf_front_check_kernel_value(svsdf_ctx *ctx, int64_t n, const double *father_yaw, const int32_t *ind_xy, unsigned char *ok_out,
                                    double *child_yaw_out) {
     if (!ctx || n < 0 || (n > 0 && (!father_yaw || !ind_xy || !ok_out || !child_yaw_out))) return SVSDF_ERR_INVALID;
@@ -1009,6 +1104,7 @@ int svsdf_create(const svsdf_config *cfg, svsdf_ctx **out) {
     if (const char *fb = std::getenv("SVSDF_FORCE_BATCHED")) ctx->force_batched = std::atoi(fb);
     if (const char *fw = std::getenv("SVSDF_FORCE_GSIP_WIDE")) ctx->force_gsip_wide = std::atoi(fw);
     if (const char *fg = std::getenv("SVSDF_FORCE_GRID_GSIP")) ctx->force_grid_gsip = std::atoi(fg);
+    if (const char *fg = std::getenv("SVSDF_FORCE_GRID_ASTAR")) ctx->force_grid_astar = std::atoi(fg);
     auto fail = [&](cudaError_t e) {
         std::fprintf(stderr, "svsdf_create: %s\n", cudaGetErrorString(e));
         svsdf_destroy(ctx);
@@ -1169,7 +1265,7 @@ void svsdf_destroy(svsdf_ctx *ctx) {
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);
     if (ctx->own_points) cudaFree(ctx->d_points);
     cudaFree(ctx->d_mesh_tri); cudaFree(ctx->d_fwn_child); cudaFree(ctx->d_fwn_data); cudaFree(ctx->d_fwn_cbox); cudaFree(ctx->d_fwn_trif);
-    cudaFree(ctx->d_front_bytes); cudaFree(ctx->d_front_rowmask); cudaFree(ctx->d_cspace); cudaFree(ctx->d_front_scratch);
+    cudaFree(ctx->d_front_bytes); cudaFree(ctx->d_front_rowmask); cudaFree(ctx->d_cspace); cudaFree(ctx->d_front_scratch); cudaFree(ctx->d_astar_pool);
     cudaFree(ctx->d_flag); cudaFree(ctx->d_inside_tstar); cudaFree(ctx->d_inside_list);
     cudaFree(ctx->d_gsip_contrib); cudaFree(ctx->d_gsip_piece); cudaFree(ctx->d_n_inside);
     cudaFree(ctx->d_eval_counter); cudaFree(ctx->d_tot); cudaFree(ctx->d_ticket); cudaFree(ctx->d_blob); cudaFree(ctx->d_partials); cudaFree(ctx->d_out);

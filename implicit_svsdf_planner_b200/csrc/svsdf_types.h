@@ -183,5 +183,16 @@ struct SubSwParams {
     double half_box;             // kernel_size / 2 + 1 (integer division), world units (front_end_Astar.hpp:224)
     double kt[64];
 };
+// k_astar_search: n whole searches (svsdf_front_astar_device)
+struct AstarArgs {
+    int n, max_path;
+    int64_t max_expansions;
+    const int *cells;          // [n][4] start x, y, goal x, y cell indices (16-byte aligned); start x = -1: start or goal outside the map
+    unsigned char *pool;       // one slot per CTA, slot_bytes each (16-byte aligned): heap, g, f, yaw, father, id — NS + 1 entries each
+    int64_t slot_bytes;
+    int *next;                 // search counter, zero at launch
+    double *paths;             // [n][max_path][3]
+    int *len, *expansions, *status;  // [n] each
+};
 
 }  // namespace svsdf

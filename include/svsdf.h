@@ -349,6 +349,19 @@ int svsdf_front_expand(svsdf_ctx *ctx, int64_t n, const int32_t *node_ij, const 
  *   longer than max_path); expansions_out[n] / rounds_out (optional): expansions per search / number of lock-step rounds. */
 int svsdf_front_astar(svsdf_ctx *ctx, int n, const double *start_xy, const double *goal_xy, int max_path, double *paths_out,
                       int32_t *len_out, int32_t *expansions_out, int64_t *rounds_out);
+/* svsdf_front_astar_device: the same n searches as svsdf_front_astar (same paths, yaws and expansion counts), each run whole on the
+ *   device in ONE kernel launch — no host step between expansions (k_astar_search: one CTA per search in flight, the bookkeeping of
+ *   csrc/host/astar_flat.hpp in its thread 0, the neighbour tests of svsdf_front_expand on its 9 warps).  Same inputs and layouts:
+ *   paths_out [n][max_path][3], start node first; len_out[q] = 0 when there is no path or it is longer than max_path; entries of a
+ *   row past len_out[q] are unspecified.  max_expansions >= 1 is the per-search budget (the test of the reference's loop: a pop
+ *   that is not the goal ends the search once max_expansions nodes have been expanded).  expansions_out, status_out and ms_out may
+ *   be NULL.  status_out[q]: 0 start or goal outside the map (isInMap; the search did not run), 1 path returned, 2 open list ran
+ *   empty, 3 max_expansions reached, 4 path found but longer than max_path, -1 an internal guard tripped (heap overflow or a father
+ *   chain longer than X * Y + 1; neither happens in a correct search).  ms_out = device time of the search kernel.  Needs
+ *   max_path >= 1 and n >= 0 (n = 0 returns at once); one search slot (45 bytes per map cell) must fit the 2 GiB search pool.
+ *   SVSDF_FORCE_GRID_ASTAR = n > 0 in the environment at svsdf_create sets the kernel's grid (tests). */
+int svsdf_front_astar_device(svsdf_ctx *ctx, int n, const double *start_xy, const double *goal_xy, int max_path, int64_t max_expansions,
+                             double *paths_out, int32_t *len_out, int32_t *expansions_out, int32_t *status_out, float *ms_out);
 int svsdf_front_init(svsdf_ctx *ctx, int kernel_size, int kernel_yaw_num, double occupancy_resolution, double front_end_safeh);
 int svsdf_front_get_kernels(svsdf_ctx *ctx, double *yaw_out, unsigned char *cells_out, unsigned char *bytes_out);
 int svsdf_front_cspace(svsdf_ctx *ctx, uint32_t *words_out, float *ms_out, const uint32_t **dev_words_out);
