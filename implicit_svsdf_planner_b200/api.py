@@ -110,7 +110,7 @@ EXPORTED_SYMBOLS = [
     "svsdf_mid_default_config", "svsdf_mid_cost", "svsdf_mid_get_ori_traj",
     "svsdf_lmbm_default_params", "svsdf_lmbm_open", "svsdf_lmbm_close", "svsdf_lmbm_last_error", "svsdf_lmbm_minimize", "svsdf_set_lmbm_library", "svsdf_read_obj", "svsdf_free", "svsdf_mesh_fwn_host",
     "svsdf_front_init", "svsdf_front_get_kernels", "svsdf_front_cspace", "svsdf_front_check_kernel_value", "svsdf_front_expand", "svsdf_front_astar",
-    "svsdf_front_astar_device",
+    "svsdf_front_astar_device", "svsdf_set_scale", "svsdf_scale_matrix",
 ]
 
 
@@ -185,12 +185,43 @@ def lib():
     L.svsdf_executed_evals.argtypes = [vp, C.c_int, C.POINTER(C.c_uint64)]
     L.svsdf_fp64_peak.argtypes = [vp, dp]
     L.svsdf_device_ptr_points.argtypes = [vp, C.POINTER(vp)]
+    L.svsdf_set_scale.argtypes = [vp, C.POINTER(Scale)]
+    L.svsdf_scale_matrix.argtypes = [C.POINTER(Scale), C.c_double, dp, dp]
     _lib = L
     return L
 
 
 def _f64(a):
     return np.ascontiguousarray(a, dtype=np.float64)
+
+
+class Scale(C.Structure):
+    """svsdf_scale: deformable robot, s_d(t) = a_d + sin(w_d t + phi_d) b_d for d = x, y; s_z = 1."""
+    _fields_ = [("a", C.c_double * 2), ("b", C.c_double * 2), ("w", C.c_double * 2), ("phi", C.c_double * 2)]
+
+
+# the reference's commented getScale example (sw_manager.hpp:498-500): diag(0.8 + sin(1.5 t - 1.0) 0.6, sin(1.8 t) 0.4 + 0.8, 1)
+EXAMPLE_SCALE = dict(a=(0.8, 0.8), b=(0.6, 0.4), w=(1.5, 1.8), phi=(-1.0, 0.0))
+
+
+def _scale(a, b=(0.0, 0.0), w=(0.0, 0.0), phi=(0.0, 0.0)) -> Scale:
+    z = Scale()
+    for name, v in (("a", a), ("b", b), ("w", w), ("phi", phi)):
+        v = [float(x) for x in v]
+        if len(v) != 2:
+            raise ValueError(f"scale.{name} needs two values (x, y)")
+        getattr(z, name)[:] = v
+    return z
+
+
+def scale_matrix(t, a, b=(0.0, 0.0), w=(0.0, 0.0), phi=(0.0, 0.0)):
+    """(S(t), St.inverse()) as 3 x 3 arrays, with the kernels' arithmetic (svsdf_scale_matrix)."""
+    z = _scale(a, b, w, phi)
+    S, Si = np.empty(9), np.empty(9)
+    rc = lib().svsdf_scale_matrix(C.byref(z), float(t), _p(S), _p(Si))
+    if rc != 0:
+        raise SvsdfError(f"svsdf_scale_matrix: status {rc}: invalid schedule or time")
+    return S.reshape(3, 3).T.copy(), Si.reshape(3, 3).T.copy()
 
 
 def _p(a):
@@ -463,6 +494,15 @@ class Context:
         self._ck(lib().svsdf_device_ptr_points(self.h, C.byref(v)), "svsdf_device_ptr_points")
         return v.value or 0
 
+    def set_scale(self, a=None, b=(0.0, 0.0), w=(0.0, 0.0), phi=(0.0, 0.0)):
+        """Deformable robot: S(t) = diag(a_x + sin(w_x t + phi_x) b_x, a_y + sin(w_y t + phi_y) b_y, 1) for every later query,
+        cost and evaluation on this context (e.g. set_scale(**EXAMPLE_SCALE)).  set_scale(None): rigid again (the default)."""
+        if a is None:
+            self._ck(lib().svsdf_set_scale(self.h, None), "svsdf_set_scale")
+            return
+        z = _scale(a, b, w, phi)
+        self._ck(lib().svsdf_set_scale(self.h, C.byref(z)), "svsdf_set_scale")
+
     def set_traj(self, T, coeffs_colmajor):
         T = _f64(T)
         c = _f64(coeffs_colmajor).reshape(-1)
@@ -729,6 +769,16 @@ class SweptVolumeManager:
     def getSDFofSweptVolume(self, pos_eva):  # sw_manager.hpp:844-866 (batched)
         sdf, ts, g, _ = self.ctx.query(self._T, self._coeffs, pos_eva, outer_only=True)
         return sdf, ts, g
+
+    def setScale(self, a=None, b=(0.0, 0.0), w=(0.0, 0.0), phi=(0.0, 0.0)):  # useScale / getScale (sw_manager.hpp:17, :495-503)
+        self._scale = None if a is None else dict(a=a, b=b, w=w, phi=phi)
+        self.ctx.set_scale(a, b, w, phi)
+
+    def getScale(self, t):  # sw_manager.hpp:495-503: S(t) (identity for a rigid robot)
+        z = getattr(self, "_scale", None)
+        if z is None:
+            return np.eye(3)
+        return scale_matrix(t, **z)[0]
 
     def getonlySDF(self, pos_rel):  # Shape.hpp:266
         return self.ctx.shape_sdf(pos_rel)

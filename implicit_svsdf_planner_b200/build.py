@@ -26,6 +26,9 @@ UNITS = [
     # (source, object, extra flags)
     ("svsdf_kernels_fast.cu", "svsdf_kernels_fast.o", []),
     ("svsdf_kernels_strict.cu", "svsdf_kernels_strict.o", ["-fmad=false"]),
+    # deformable robots (svsdf_set_scale): the scaled k_outer / k_gsip instantiations, fast and strict
+    ("svsdf_kernels_scaled_fast.cu", "svsdf_kernels_scaled_fast.o", []),
+    ("svsdf_kernels_scaled_strict.cu", "svsdf_kernels_scaled_strict.o", ["-fmad=false"]),
     ("svsdf_extract.cu", "svsdf_extract.o", ["-fmad=false"]),  # cell centres must round like the host formula
     ("svsdf_frontend.cu", "svsdf_frontend.o", ["-fmad=false"]),  # shape kernels: same rounding as the strict functors
     # host threads for the batch A* bookkeeping; no a*b+c contraction in the float winding-number builder (host/fwn_bvh.hpp)

@@ -191,23 +191,55 @@ __device__ __forceinline__ void rel_from_pose(double px, double py, double x, do
     ry = -sy * d0 + cy * d1;
 }
 
-// getSDFAtTimeStamp<false> (sw_manager.hpp:741-757)
-template <int SHAPE, bool XFORM>
-__device__ __forceinline__ double eval_sdf(const TrajView &tv, const ShapeParams &S, double px, double py, double t) {
+// Deformable robot (useScale == true): getScale(t) = diag(sx, sy, 1) (ScaleSched) and the diagonal (ix, iy) of St.inverse()
+// by Eigen 3.3's size-3 cofactor formula: 1/det with det = sy * sx, then ix = sy * (1/det), iy = sx * (1/det) — not 1/sx.
+// t is the absolute time of the sample.
+__device__ __forceinline__ void scale_inv(const ScaleSched &Z, double t, double &ix, double &iy) {
+    double s0, c0, s1, c1;
+    dev::sincos_portable(Z.w[0] * t + Z.phi[0], s0, c0);
+    dev::sincos_portable(Z.w[1] * t + Z.phi[1], s1, c1);
+    const double sx = Z.a[0] + s0 * Z.b[0], sy = Z.a[1] + s1 * Z.b[1];
+    const double inv = 1.0 / (sy * sx);
+    ix = sy * inv;
+    iy = sx * inv;
+}
+// posEva2Rel(p, xt, Rt, St) (sw_manager.hpp:528-535): rel = (Rt^T St^-1) (p - xt), the 3x3 product first (eager Eigen):
+// its 2x2 block is [[c ix, s iy], [-s ix, c iy]].  SCALED == false: rel_from_pose, Z unused.
+template <bool SCALED>
+__device__ __forceinline__ void rel_at(const ScaleSched *Z, double t, double px, double py, double x, double y, double cy,
+                                       double sy, double &rx, double &ry) {
+    if constexpr (SCALED) {
+        double ix, iy;
+        scale_inv(*Z, t, ix, iy);
+        const double d0 = px - x, d1 = py - y;
+        rx = (cy * ix) * d0 + (sy * iy) * d1;
+        ry = (-sy * ix) * d0 + (cy * iy) * d1;
+    } else {
+        rel_from_pose(px, py, x, y, cy, sy, rx, ry);
+    }
+}
+
+// getSDFAtTimeStamp<SCALED> (sw_manager.hpp:741-757; the mesh functor's _igl variant :760-777)
+template <int SHAPE, bool XFORM, bool SCALED = false>
+__device__ __forceinline__ double eval_sdf(const TrajView &tv, const ShapeParams &S, double px, double py, double t,
+                                           const ScaleSched *Z = nullptr) {
     double x, y, yaw, sy, cy, rx, ry;
+    const double ta = t;
     traj_pos(tv, t, x, y, yaw);
     dev::sincos_portable(yaw, sy, cy);
-    rel_from_pose(px, py, x, y, cy, sy, rx, ry);
+    rel_at<SCALED>(Z, ta, px, py, x, y, cy, sy, rx, ry);
     return dev::shape_sdf<SHAPE, XFORM>(S, rx, ry);
 }
 // same with a piece-index guess carried by the caller from its previous sample
-template <int SHAPE, bool XFORM>
-__device__ __forceinline__ double eval_sdf(const TrajView &tv, const ShapeParams &S, double px, double py, double t, int &hint) {
+template <int SHAPE, bool XFORM, bool SCALED = false>
+__device__ __forceinline__ double eval_sdf(const TrajView &tv, const ShapeParams &S, double px, double py, double t, int &hint,
+                                           const ScaleSched *Z = nullptr) {
     double x, y, yaw, sy, cy, rx, ry;
+    const double ta = t;  // absolute time: locate_piece makes t piece-local
     const int i = locate_piece(tv, t, hint);
     traj_pos_at(tv, i, t, x, y, yaw);
     dev::sincos_portable(yaw, sy, cy);
-    rel_from_pose(px, py, x, y, cy, sy, rx, ry);
+    rel_at<SCALED>(Z, ta, px, py, x, y, cy, sy, rx, ry);
     return dev::shape_sdf<SHAPE, XFORM>(S, rx, ry);
 }
 
@@ -244,9 +276,12 @@ struct OuterResult {
 //   M_M    29 halvings in the actual direction after a misprediction
 // Decisions are the sequential loop's: the slope's sign always comes from the finite difference on lanes 30/31, and the
 // accepted halving is the first (largest step) whose candidate decreases f.
-template <int SHAPE, bool XFORM>
+// SCALED (deformable robot, schedule *Z): only the descent evaluates the scaled shape; choiceTInit's 2-argument overload
+// (:538-581) never reads its template flag, so the four seed layers stay rigid.
+template <int SHAPE, bool XFORM, bool SCALED = false>
 __device__ __forceinline__ OuterResult solve_outer(const TrajView &tv, const ShapeParams &S, double px, double py,
-                                                   bool have_seed = false, double seed_in = 0.0, double min_in = 1e9) {
+                                                   bool have_seed = false, double seed_in = 0.0, double min_in = 1e9,
+                                                   const ScaleSched *Z = nullptr) {
     const int lane = threadIdx.x & 31;
     const double D = tv.D;
     const double INF = __longlong_as_double(0x7ff0000000000000LL);
@@ -354,7 +389,8 @@ __device__ __forceinline__ OuterResult solve_outer(const TrajView &tv, const Sha
     int mode;
     int tau_hi;        // this lane's step, high word
     unsigned sbit;     // this lane's offset sign bit
-    if (__any_sync(FULL, min_dis >= 1e9)) {
+    // SCALED: the reference evaluates f(x0) at iter == 0 with the scaled shape, which is not the rigid seed minimum
+    if (SCALED || __any_sync(FULL, min_dis >= 1e9)) {
         // nothing below the initial 1e9 (degenerate input): the reference evaluates f(x0) at iter == 0
         mode = M_F0;
         tau_hi = 0; sbit = 0;   // offset +0.0: the sample is x itself
@@ -369,7 +405,7 @@ __device__ __forceinline__ OuterResult solve_outer(const TrajView &tv, const Sha
     while (running) {
         const double off = __hiloint2double(tau_hi ^ (int)sbit, (mode == M_F0) ? 0 : tau_lo);
         const double tq = smaxd(smind(x + off, hi_l), lo_l);
-        const double fq = eval_sdf<SHAPE, XFORM>(tv, S, px, py, tq, hint);
+        const double fq = eval_sdf<SHAPE, XFORM, SCALED>(tv, S, px, py, tq, hint, Z);
         const unsigned m_dec = __ballot_sync(FULL, (fq - fx) < 0);  // candidates that decrease f
         int jacc = -1, src = 0;
         bool failed = false, step_end = true;
@@ -450,14 +486,14 @@ __device__ __forceinline__ OuterResult solve_outer(const TrajView &tv, const Sha
 
 // getGradPrelAtTimeStamp (sw_manager.hpp:779-795) -> getonlyGrad1: central FD, dx = 1e-6 in the body frame
 // (Shape.hpp:35-53), or the Polygon's analytic override (Shape.hpp:1508-1534). 4 lanes do the 4 evaluations.
-template <int SHAPE, bool XFORM>
+template <int SHAPE, bool XFORM, bool SCALED = false>
 __device__ __forceinline__ void grad_prel(const TrajView &tv, const ShapeParams &S, double px, double py, double t,
-                                          double &gx, double &gy) {
+                                          double &gx, double &gy, const ScaleSched *Z = nullptr) {
     const int lane = threadIdx.x & 31;
     double x, y, yaw, sy, cy, rx, ry;
     traj_pos(tv, t, x, y, yaw);
     dev::sincos_portable(yaw, sy, cy);
-    rel_from_pose(px, py, x, y, cy, sy, rx, ry);
+    rel_at<SCALED>(Z, t, px, py, x, y, cy, sy, rx, ry);
     if (SHAPE == SH_POLYGON) {
         dev::PolyHit H = dev::polygon_scan(S, rx, ry);
         double vx = rx - H.cx, vy = ry - H.cy;
@@ -514,9 +550,13 @@ struct Contribution {
     double gdT, pena;
     bool active;
 };
+// SCALED: sdf_grad = -L' (-(St^-1)^T rotate g) with St = getScale(t*) at the absolute t* (:827, :1050); the yaw term keeps
+// the reference's form without St^-1 (:1062; exact only at St = I) and gdT has no dS/dt term (at fixed t*, S does not
+// depend on the durations).
+template <bool SCALED = false>
 __device__ __forceinline__ Contribution point_contribution(const TrajView &tv, const CostParams &cp, double px,
                                                            double py, double sdf, double tstar, double gx,
-                                                           double gy) {
+                                                           double gy, const ScaleSched *Z = nullptr) {
     Contribution C;
     double tl = tstar;
     int i = locate_piece(tv, tl);
@@ -552,8 +592,16 @@ __device__ __forceinline__ Contribution point_contribution(const TrajView &tv, c
     C.pena = 0.0;
     C.active = false;
     if (sdf_cost > 0) {
-        double rg0 = -(cy * gx + (-sy) * gy);
-        double rg1 = -(sy * gx + cy * gy);
+        double rg0, rg1;
+        if constexpr (SCALED) {
+            double ix, iy;
+            scale_inv(*Z, tstar, ix, iy);
+            rg0 = -((ix * cy) * gx + (-(ix * sy)) * gy);
+            rg1 = -((iy * sy) * gx + (iy * cy) * gy);
+        } else {
+            rg0 = -(cy * gx + (-sy) * gy);
+            rg1 = -(sy * gx + cy * gy);
+        }
         double sg0 = -sdf_out_grad * rg0, sg1 = -sdf_out_grad * rg1;
         double d0 = px - pos[0], d1 = py - pos[1];
         double w0 = -sy * d0 + cy * d1;
@@ -652,13 +700,13 @@ __device__ __forceinline__ void thread_choice_t_init(const TrajView &tv, const S
 }
 
 // getGradPrelAtTimeStamp (sw_manager.hpp:779-795) -> getonlyGrad1 (Shape.hpp:35-53), one point per thread
-template <int SHAPE, bool XFORM>
+template <int SHAPE, bool XFORM, bool SCALED = false>
 __device__ __forceinline__ void thread_grad_prel(const TrajView &tv, const ShapeParams &S, double px, double py, double t,
-                                                 double &gx, double &gy) {
+                                                 double &gx, double &gy, const ScaleSched *Z = nullptr) {
     double x, y, yaw, sy, cy, rx, ry;
     traj_pos(tv, t, x, y, yaw);
     dev::sincos_portable(yaw, sy, cy);
-    rel_from_pose(px, py, x, y, cy, sy, rx, ry);
+    rel_at<SCALED>(Z, t, px, py, x, y, cy, sy, rx, ry);
     if (SHAPE == SH_POLYGON) {
         dev::PolyHit H = dev::polygon_scan(S, rx, ry);
         double vx = rx - H.cx, vy = ry - H.cy;
@@ -710,9 +758,10 @@ __device__ __forceinline__ void thread_grad_prel(const TrajView &tv, const Shape
 // decreases f, the sign comes from the finite difference — bit-identical results (GPU parity tests, strict build).
 // In: lane i (< nb) holds point i of the batch (px, py, choiceTInit seed and minimum).  Out: res[2 i] = sdf, res[2 i + 1] = t*.
 // ------------------------------------------------------------------------------------------------
-template <int SHAPE, bool XFORM>
+template <int SHAPE, bool XFORM, bool SCALED = false>
 __device__ __forceinline__ void descent_engine(const TrajView &tv, const ShapeParams &S, int nb, double mpx, double mpy,
-                                               double mseed, double mmin, double *res, unsigned &evals) {
+                                               double mseed, double mmin, double *res, unsigned &evals,
+                                               const ScaleSched *Z = nullptr) {
     enum { E_F0 = 0, E_R1 = 1, E_RN = 2 };
     const int lane = threadIdx.x & 31, q = lane & 7, qbase = lane & 24;
     const double D = tv.D;
@@ -744,7 +793,7 @@ __device__ __forceinline__ void descent_engine(const TrajView &tv, const ShapePa
                     t_min = smaxd(0.0, nsd - 3.4);      // :856-857
                     t_max = smind(nsd + 3.4, D);
                     iter = 0; pred = 1; sgn = 1; jbase = 0; hint = 0;
-                    mode = (nmn >= 1e9) ? E_F0 : E_R1;
+                    mode = (SCALED || nmn >= 1e9) ? E_F0 : E_R1;  // SCALED: f(x0) of the scaled shape
                 }
             }
         }
@@ -765,7 +814,7 @@ __device__ __forceinline__ void descent_engine(const TrajView &tv, const ShapePa
         const double hi_l = slope ? ((q == 0) ? INF : D) : t_max;
         const double tc = smaxd(smind(x + off, hi_l), lo_l);
         const double tq = (cand || slope) ? tc : x;
-        const double fq = eval_sdf<SHAPE, XFORM>(tv, S, px, py, tq, hint);
+        const double fq = eval_sdf<SHAPE, XFORM, SCALED>(tv, S, px, py, tq, hint, Z);
 
         // ---- collectives (all lanes), then each quarter's decision, again without branches ----
         const unsigned m8 = (__ballot_sync(FULL, (fq - fx) < 0) >> qbase) & 0xffu;
@@ -816,9 +865,9 @@ __device__ __forceinline__ void descent_engine(const TrajView &tv, const ShapePa
 // wk[4 (32 w + i)], valid for i < nbw[w]; served in the order i-major, w-minor through the shared cursor): a group that
 // finishes its point takes the next one of the whole CTA, so the warps of a CTA finish together whatever the lengths of
 // their own descents.  Which group solves a point does not change its result; the reductions stay per warp, fixed order.
-template <int SHAPE, bool XFORM>
+template <int SHAPE, bool XFORM, bool SCALED = false>
 __device__ __forceinline__ void descent_engine2(const TrajView &tv, const ShapeParams &S, double *wk, const int *nbw, int *cursor,
-                                                int limit, unsigned &evals) {
+                                                int limit, unsigned &evals, const ScaleSched *Z = nullptr) {
     enum { E_F0 = 0, E_R1 = 1, E_RN = 2 };
     const int lane = threadIdx.x & 31, q = lane & 3, gbase = lane & 28;
     const double D = tv.D;
@@ -849,7 +898,7 @@ __device__ __forceinline__ void descent_engine2(const TrajView &tv, const ShapeP
                     t_min = smaxd(0.0, nsd - 3.4);
                     t_max = smind(nsd + 3.4, D);
                     iter = 0; pred = 1; sgn = 1; jbase = 0; hintA = 0; hintB = 0;
-                    mode = (nmn >= 1e9) ? E_F0 : E_R1;
+                    mode = (SCALED || nmn >= 1e9) ? E_F0 : E_R1;  // SCALED: f(x0) of the scaled shape
                 }
             }
         }
@@ -872,8 +921,8 @@ __device__ __forceinline__ void descent_engine2(const TrajView &tv, const ShapeP
         const double loA = slopeA ? ((q == 0) ? 0.0 : -INF) : t_min, hiA = slopeA ? ((q == 0) ? INF : D) : t_max;
         const double tcA = smaxd(smind(x + offA, hiA), loA), tcB = smaxd(smind(x + offB, t_max), t_min);
         const double tA = (candA || slopeA) ? tcA : x, tB = candB ? tcB : x;
-        const double fA = eval_sdf<SHAPE, XFORM>(tv, S, px, py, tA, hintA);
-        const double fB = eval_sdf<SHAPE, XFORM>(tv, S, px, py, tB, hintB);
+        const double fA = eval_sdf<SHAPE, XFORM, SCALED>(tv, S, px, py, tA, hintA, Z);
+        const double fB = eval_sdf<SHAPE, XFORM, SCALED>(tv, S, px, py, tB, hintB, Z);
 
         const unsigned balA = __ballot_sync(FULL, (fA - fx) < 0), balB = __ballot_sync(FULL, (fB - fx) < 0);
         const unsigned m8 = ((balA >> gbase) & 0xfu) | (((balB >> gbase) & 0xfu) << 4);
@@ -952,8 +1001,10 @@ __device__ __forceinline__ void tma_load_blob(double *smem_blob, const double *g
 // ------------------------------------------------------------------------------------------------
 // k_pose_table: (x, y, cos yaw, sin yaw) at the layer-1 lattice times, written into the blob in place.
 // The lattice and its poses are shared by every query point (choiceTInit layer 1 always scans 0..D in 0.15 s
-// steps), so they are computed once per evaluation instead of once per point.
+// steps), so they are computed once per evaluation instead of once per point.  Rigid for a deformable robot too: the
+// layer-1 scan does not read the scale.
 // ------------------------------------------------------------------------------------------------
+#ifndef SVSDF_SCALED_UNIT
 __global__ void k_pose_table(double *blob) {
     TrajView tv = make_view(blob);
     int k = blockIdx.x * blockDim.x + threadIdx.x;
@@ -965,6 +1016,7 @@ __global__ void k_pose_table(double *blob) {
     double *ps = blob + L.off_pose + k;
     ps[0] = x; ps[L.K1pad] = y; ps[2 * L.K1pad] = cy; ps[3 * L.K1pad] = sy;
 }
+#endif
 
 // ------------------------------------------------------------------------------------------------
 // K1: outer solve for every point (+ penalty, chain rule and CTA reduction for outside points)
@@ -982,10 +1034,10 @@ __global__ void k_pose_table(double *blob) {
 #ifndef SVSDF_GSIP_MIN_CTAS
 #define SVSDF_GSIP_MIN_CTAS 3
 #endif
-// BATCHED selects the schedule at compile time (two kernels: each carries only its own evaluation sites)
-template <int SHAPE, bool XFORM, bool BATCHED>
-__global__ void __launch_bounds__(kWarpsPerBlock * 32, (SHAPE == SH_MESH) ? SVSDF_MESH_MIN_CTAS : SVSDF_OUTER_MIN_CTAS)
-    k_outer(const __grid_constant__ KernelArgs A, const __grid_constant__ ShapeParams S) {
+// BATCHED selects the schedule at compile time (two kernels: each carries only its own evaluation sites).
+// SCALED: deformable robot with the schedule *Z (k_outer_scaled); the rigid k_outer passes nullptr and never reads it.
+template <int SHAPE, bool XFORM, bool BATCHED, bool SCALED>
+__device__ __forceinline__ void outer_body(const KernelArgs &A, const ShapeParams &S, const ScaleSched *Z) {
     extern __shared__ __align__(16) double smem[];
     __shared__ __align__(8) uint64_t bar;
     __shared__ int s_nb[kWarpsPerBlock];
@@ -1036,11 +1088,11 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, (SHAPE == SH_MESH) ? SVSD
             if (lane == 0) s_nb[warp] = nb;
             if (threadIdx.x == 0) s_cursor = 0;
             __syncthreads();   // every warp has the same number of batches (nB is a multiple of the warp count)
-            descent_engine2<SHAPE, XFORM>(tv, S, res - 128 * warp, s_nb, &s_cursor, kWarpsPerBlock * 32, ev2);
+            descent_engine2<SHAPE, XFORM, SCALED>(tv, S, res - 128 * warp, s_nb, &s_cursor, kWarpsPerBlock * 32, ev2, Z);
             __syncthreads();
             if (my_valid) { m_sdf = res[4 * lane]; m_ts = res[4 * lane + 1]; }
 #else
-            descent_engine<SHAPE, XFORM>(tv, S, nb, mpx, mpy, m_seed, m_min, res, ev2);
+            descent_engine<SHAPE, XFORM, SCALED>(tv, S, nb, mpx, mpy, m_seed, m_min, res, ev2, Z);
             if (my_valid) { m_sdf = res[2 * lane]; m_ts = res[2 * lane + 1]; }
 #endif
             my_evals += (unsigned long long)__reduce_add_sync(FULL, (unsigned)ev + ev2);
@@ -1049,16 +1101,16 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, (SHAPE == SH_MESH) ? SVSD
 #pragma unroll 1
             for (int i = 0; i < nb; ++i) {
                 const double px = __shfl_sync(FULL, mpx, i), py = __shfl_sync(FULL, mpy, i);
-                const OuterResult R = solve_outer<SHAPE, XFORM>(tv, S, px, py);
+                const OuterResult R = solve_outer<SHAPE, XFORM, SCALED>(tv, S, px, py, false, 0.0, 1e9, Z);
                 my_evals += (unsigned long long)R.evals;
                 if (lane == i) { m_sdf = R.sdf; m_ts = R.tstar; }
                 double gx, gy;
-                grad_prel<SHAPE, XFORM>(tv, S, px, py, R.tstar, gx, gy);
+                grad_prel<SHAPE, XFORM, SCALED>(tv, S, px, py, R.tstar, gx, gy, Z);
                 if (lane == i) { m_gx = gx; m_gy = gy; }
             }
         }
         my_evals += 4ull * (unsigned long long)nb;
-        if (BATCHED && batched && my_valid) thread_grad_prel<SHAPE, XFORM>(tv, S, mpx, mpy, m_ts, m_gx, m_gy);
+        if (BATCHED && batched && my_valid) thread_grad_prel<SHAPE, XFORM, SCALED>(tv, S, mpx, mpy, m_ts, m_gx, m_gy, Z);
         // ---- per-lane epilogue: outputs, interior flag, penalty + chain rule (one point per lane) ----
         const bool inside = my_valid && A.want_gsip && !(m_sdf > 0);  // getTrueSDFofSweptVolume: `if (argmin_dis > 0) return`
         if (my_valid) {
@@ -1072,7 +1124,7 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, (SHAPE == SH_MESH) ? SVSD
         if (A.want_reduce) {
             Contribution C;
             C.active = false;
-            if (my_valid && !inside) C = point_contribution(tv, A.cp, mpx, mpy, m_sdf, m_ts, m_gx, m_gy);
+            if (my_valid && !inside) C = point_contribution<SCALED>(tv, A.cp, mpx, mpy, m_sdf, m_ts, m_gx, m_gy, Z);
             // accumulate the active lanes' contributions in batch order (deterministic)
             unsigned m = __ballot_sync(FULL, C.active);
             while (m) {
@@ -1109,6 +1161,16 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, (SHAPE == SH_MESH) ? SVSD
             A.partials[(int64_t)blockIdx.x * nacc + e] = s;
         }
     }
+}
+template <int SHAPE, bool XFORM, bool BATCHED>
+__global__ void __launch_bounds__(kWarpsPerBlock * 32, (SHAPE == SH_MESH) ? SVSDF_MESH_MIN_CTAS : SVSDF_OUTER_MIN_CTAS)
+    k_outer(const __grid_constant__ KernelArgs A, const __grid_constant__ ShapeParams S) {
+    outer_body<SHAPE, XFORM, BATCHED, false>(A, S, nullptr);
+}
+template <int SHAPE, bool XFORM, bool BATCHED>
+__global__ void __launch_bounds__(kWarpsPerBlock * 32, (SHAPE == SH_MESH) ? SVSDF_MESH_MIN_CTAS : SVSDF_OUTER_MIN_CTAS)
+    k_outer_scaled(const __grid_constant__ KernelArgs A, const __grid_constant__ ShapeParams S, const __grid_constant__ ScaleSched Z) {
+    outer_body<SHAPE, XFORM, BATCHED, true>(A, S, &Z);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1174,9 +1236,9 @@ __global__ void __launch_bounds__(1024) k_compact(const unsigned char *flag, int
 // running a full outer solve on its sample.
 // dynamic smem: [ blob ]
 // ------------------------------------------------------------------------------------------------
-template <int SHAPE, bool XFORM, int WARPS>
-__global__ void __launch_bounds__(WARPS * 32, (WARPS == kWarpsPerBlock && SHAPE != SH_MESH) ? SVSDF_GSIP_MIN_CTAS : 1)
-    k_gsip(const __grid_constant__ KernelArgs A, const __grid_constant__ ShapeParams S) {
+// SCALED: the ring samples run scaled descents (getSDFofSweptVolume<useScale>); the velocity fallback and the ring do not change.
+template <int SHAPE, bool XFORM, int WARPS, bool SCALED>
+__device__ __forceinline__ void gsip_body(const KernelArgs &A, const ShapeParams &S, const ScaleSched *Z) {
     extern __shared__ __align__(16) double smem[];
     __shared__ __align__(8) uint64_t bar;
     __shared__ double s_theta[24], s_val[24], s_ts[24];
@@ -1229,7 +1291,7 @@ __global__ void __launch_bounds__(WARPS * 32, (WARPS == kWarpsPerBlock && SHAPE 
                 double sn, cs;
                 dev::sincos_portable(th, sn, cs);
                 double yx = px + 1.0 * r * cs, yy = py + 1.0 * r * sn;  // CircleCoord2D::getPosition (:36-39)
-                OuterResult R = solve_outer<SHAPE, XFORM>(tv, S, yx, yy);
+                OuterResult R = solve_outer<SHAPE, XFORM, SCALED>(tv, S, yx, yy, false, 0.0, 1e9, Z);
                 my_evals += (unsigned long long)R.evals;
                 if (lane == 0) { s_val[k] = R.sdf; s_ts[k] = R.tstar; }
             }
@@ -1271,7 +1333,7 @@ __global__ void __launch_bounds__(WARPS * 32, (WARPS == kWarpsPerBlock && SHAPE 
             if (A.out_rounds) A.out_rounds[pt] = rounds;
         }
         if (A.want_reduce && warp == 0) {
-            Contribution C = point_contribution(tv, A.cp, px, py, sdf, real_t_star, gx, gy);
+            Contribution C = point_contribution<SCALED>(tv, A.cp, px, py, sdf, real_t_star, gx, gy, Z);
             double *o = A.gsip_contrib + 20 * (int64_t)slot;
             if (lane < 18) {
                 int d = lane / 6, q = lane - 6 * d;
@@ -1288,6 +1350,16 @@ __global__ void __launch_bounds__(WARPS * 32, (WARPS == kWarpsPerBlock && SHAPE 
     }
     if (A.eval_counter && lane == 0) atomicAdd(A.eval_counter, my_evals);
 }
+template <int SHAPE, bool XFORM, int WARPS>
+__global__ void __launch_bounds__(WARPS * 32, (WARPS == kWarpsPerBlock && SHAPE != SH_MESH) ? SVSDF_GSIP_MIN_CTAS : 1)
+    k_gsip(const __grid_constant__ KernelArgs A, const __grid_constant__ ShapeParams S) {
+    gsip_body<SHAPE, XFORM, WARPS, false>(A, S, nullptr);
+}
+template <int SHAPE, bool XFORM, int WARPS>
+__global__ void __launch_bounds__(WARPS * 32, (WARPS == kWarpsPerBlock && SHAPE != SH_MESH) ? SVSDF_GSIP_MIN_CTAS : 1)
+    k_gsip_scaled(const __grid_constant__ KernelArgs A, const __grid_constant__ ShapeParams S, const __grid_constant__ ScaleSched Z) {
+    gsip_body<SHAPE, XFORM, WARPS, true>(A, S, &Z);
+}
 
 // ------------------------------------------------------------------------------------------------
 // k_finalize: fixed-order sum of the K1 CTA partials and the K2 per-point contributions.  One warp per accumulator
@@ -1295,7 +1367,9 @@ __global__ void __launch_bounds__(WARPS * 32, (WARPS == kWarpsPerBlock && SHAPE 
 // result is bit-reproducible.  The last CTA to finish (ticket counter) writes the output record:
 // out: [0] cost, [1 .. 18N] gradC in Eigen column-major order (d*6N + 6i + q), [1+18N .. 1+19N) gradT with the
 // reference's rule gradT(j) += gdT for all j < piece (back_end_optimizer.hpp:859-862), [1+19N] n_inside.
+// (k_finalize and the utility kernels below live in the rigid units only: the scaled units share them.)
 // ------------------------------------------------------------------------------------------------
+#ifndef SVSDF_SCALED_UNIT
 __device__ __forceinline__ double warp_sum_fixed(double v) {
 #pragma unroll
     for (int off = 16; off > 0; off >>= 1) v += __shfl_down_sync(FULL, v, off);
@@ -1417,10 +1491,18 @@ __global__ void __launch_bounds__(256) k_fp64_peak(double *out, int iters) {
     }
     out[(int64_t)blockIdx.x * blockDim.x + threadIdx.x] = a0 + a1 + a2 + a3 + a4 + a5 + a6 + a7;
 }
+#endif  // SVSDF_SCALED_UNIT
 
 // ------------------------------------------------------------------------------------------------
-// Host-side launchers (shape dispatch)
+// Host-side launchers (shape dispatch).  The scaled translation units (SVSDF_SCALED_UNIT) instantiate only the deformable-
+// robot kernels k_outer_scaled / k_gsip_scaled; the rigid units only k_outer / k_gsip.
 // ------------------------------------------------------------------------------------------------
+#ifdef SVSDF_SCALED_UNIT
+constexpr bool kScaledUnit = true;
+#else
+constexpr bool kScaledUnit = false;
+#endif
+
 struct LaunchCfg {
     int grid_outer, grid_gsip;
     size_t smem_outer, smem_gsip;
@@ -1429,8 +1511,24 @@ struct LaunchCfg {
     bool gsip_wide;           // use the 22-warp k_gsip variant
 };
 
-template <int SHAPE, bool XFORM>
-static cudaError_t launch_shape(const KernelArgs &A, const ShapeParams &S, const LaunchCfg &cfg, int N) {
+// k[0] sparse k_outer, k[1] batched k_outer, k[2] 8-warp k_gsip, k[3] 22-warp k_gsip
+template <int SHAPE, bool XFORM, bool SCALED>
+static void cost_kernels(const void *k[4]) {
+    if constexpr (SCALED) {
+        k[0] = (const void *)k_outer_scaled<SHAPE, XFORM, false>;
+        k[1] = (const void *)k_outer_scaled<SHAPE, XFORM, true>;
+        k[2] = (const void *)k_gsip_scaled<SHAPE, XFORM, kWarpsPerBlock>;
+        k[3] = (const void *)k_gsip_scaled<SHAPE, XFORM, kGsipWarps>;
+    } else {
+        k[0] = (const void *)k_outer<SHAPE, XFORM, false>;
+        k[1] = (const void *)k_outer<SHAPE, XFORM, true>;
+        k[2] = (const void *)k_gsip<SHAPE, XFORM, kWarpsPerBlock>;
+        k[3] = (const void *)k_gsip<SHAPE, XFORM, kGsipWarps>;
+    }
+}
+
+template <int SHAPE, bool XFORM, bool SCALED>
+static cudaError_t launch_shape(const KernelArgs &A, const ShapeParams &S, const ScaleSched *Z, const LaunchCfg &cfg, int N) {
     cudaError_t e;
     // the attribute is per device (a process may hold contexts on several GPUs): one flag per device ordinal
     static bool attr_set_dev[64] = {};
@@ -1438,26 +1536,34 @@ static cudaError_t launch_shape(const KernelArgs &A, const ShapeParams &S, const
     cudaGetDevice(&dev_ord);
     bool &attr_set = attr_set_dev[dev_ord & 63];
     if (!attr_set) {
-        e = cudaFuncSetAttribute(k_outer<SHAPE, XFORM, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-        if (e != cudaSuccess) return e;
-        e = cudaFuncSetAttribute(k_outer<SHAPE, XFORM, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-        if (e != cudaSuccess) return e;
-        e = cudaFuncSetAttribute(k_gsip<SHAPE, XFORM, kWarpsPerBlock>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-        if (e != cudaSuccess) return e;
-        e = cudaFuncSetAttribute(k_gsip<SHAPE, XFORM, kGsipWarps>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-        if (e != cudaSuccess) return e;
+        const void *k[4];
+        cost_kernels<SHAPE, XFORM, SCALED>(k);
+        for (int i = 0; i < 4; ++i) {
+            e = cudaFuncSetAttribute(k[i], cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+            if (e != cudaSuccess) return e;
+        }
         attr_set = true;
     }
-    if (A.batched) k_outer<SHAPE, XFORM, true><<<cfg.grid_outer, kWarpsPerBlock * 32, cfg.smem_outer, cfg.stream>>>(A, S);
-    else k_outer<SHAPE, XFORM, false><<<cfg.grid_outer, kWarpsPerBlock * 32, cfg.smem_outer, cfg.stream>>>(A, S);
+    if constexpr (SCALED) {
+        if (A.batched) k_outer_scaled<SHAPE, XFORM, true><<<cfg.grid_outer, kWarpsPerBlock * 32, cfg.smem_outer, cfg.stream>>>(A, S, *Z);
+        else k_outer_scaled<SHAPE, XFORM, false><<<cfg.grid_outer, kWarpsPerBlock * 32, cfg.smem_outer, cfg.stream>>>(A, S, *Z);
+    } else {
+        if (A.batched) k_outer<SHAPE, XFORM, true><<<cfg.grid_outer, kWarpsPerBlock * 32, cfg.smem_outer, cfg.stream>>>(A, S);
+        else k_outer<SHAPE, XFORM, false><<<cfg.grid_outer, kWarpsPerBlock * 32, cfg.smem_outer, cfg.stream>>>(A, S);
+    }
     e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     if (cfg.after_outer) cudaEventRecord(cfg.after_outer, cfg.stream);
     if (A.want_gsip) {
         k_compact<<<1, 1024, 0, cfg.stream>>>(A.inside_flag, A.P, A.inside_list, A.n_inside);
         // few inside points: one warp per ring sample (latency); many: 8-warp CTAs, two per SM (throughput)
-        if (cfg.gsip_wide) k_gsip<SHAPE, XFORM, kGsipWarps><<<cfg.grid_gsip, kGsipWarps * 32, cfg.smem_gsip, cfg.stream>>>(A, S);
-        else k_gsip<SHAPE, XFORM, kWarpsPerBlock><<<cfg.grid_gsip, kWarpsPerBlock * 32, cfg.smem_gsip, cfg.stream>>>(A, S);
+        if constexpr (SCALED) {
+            if (cfg.gsip_wide) k_gsip_scaled<SHAPE, XFORM, kGsipWarps><<<cfg.grid_gsip, kGsipWarps * 32, cfg.smem_gsip, cfg.stream>>>(A, S, *Z);
+            else k_gsip_scaled<SHAPE, XFORM, kWarpsPerBlock><<<cfg.grid_gsip, kWarpsPerBlock * 32, cfg.smem_gsip, cfg.stream>>>(A, S, *Z);
+        } else {
+            if (cfg.gsip_wide) k_gsip<SHAPE, XFORM, kGsipWarps><<<cfg.grid_gsip, kGsipWarps * 32, cfg.smem_gsip, cfg.stream>>>(A, S);
+            else k_gsip<SHAPE, XFORM, kWarpsPerBlock><<<cfg.grid_gsip, kWarpsPerBlock * 32, cfg.smem_gsip, cfg.stream>>>(A, S);
+        }
         e = cudaGetLastError();
         if (e != cudaSuccess) return e;
     }
@@ -1466,10 +1572,10 @@ static cudaError_t launch_shape(const KernelArgs &A, const ShapeParams &S, const
 }
 
 template <bool XFORM>
-static cudaError_t dispatch(const KernelArgs &A, const ShapeParams &S, const LaunchCfg &cfg, int N) {
+static cudaError_t dispatch(const KernelArgs &A, const ShapeParams &S, const ScaleSched *Z, const LaunchCfg &cfg, int N) {
     switch (S.id) {
 #define SVSDF_CASE(ID) \
-    case ID: return launch_shape<ID, XFORM>(A, S, cfg, N);
+    case ID: return launch_shape<ID, XFORM, kScaledUnit>(A, S, Z, cfg, N);
         SVSDF_CASE(SH_STAR)
         SVSDF_CASE(SH_HORSESHOE)
         SVSDF_CASE(SH_PIE)
@@ -1488,24 +1594,24 @@ static cudaError_t dispatch(const KernelArgs &A, const ShapeParams &S, const Lau
         SVSDF_CASE(SH_UNEVENCAPSULE)
         SVSDF_CASE(SH_CIRCLE)
 #undef SVSDF_CASE
-        case SH_POLYGON: return launch_shape<SH_POLYGON, false>(A, S, cfg, N);
-        case SH_MESH: return launch_shape<SH_MESH, false>(A, S, cfg, N);
+        case SH_POLYGON: return launch_shape<SH_POLYGON, false, kScaledUnit>(A, S, Z, cfg, N);
+        case SH_MESH: return launch_shape<SH_MESH, false, kScaledUnit>(A, S, Z, cfg, N);
         default: return cudaErrorInvalidValue;
     }
 }
 
 template <int SHAPE, bool XFORM>
 static cudaError_t occ_shape(size_t smem_outer, size_t smem_gsip, int *occ_outer, int *occ_gsip) {
-    cudaError_t e = cudaFuncSetAttribute(k_outer<SHAPE, XFORM, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(k_outer<SHAPE, XFORM, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(k_gsip<SHAPE, XFORM, kWarpsPerBlock>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    if (e != cudaSuccess) return e;
+    const void *k[4];
+    cost_kernels<SHAPE, XFORM, kScaledUnit>(k);
+    for (int i = 0; i < 3; ++i) {
+        cudaError_t e = cudaFuncSetAttribute(k[i], cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+        if (e != cudaSuccess) return e;
+    }
     // the two schedules are compiled to the same register cap (launch bounds); the batched kernel sizes the full wave
-    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ_outer, k_outer<SHAPE, XFORM, true>, kWarpsPerBlock * 32, smem_outer);
+    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ_outer, k[1], kWarpsPerBlock * 32, smem_outer);
     if (e != cudaSuccess) return e;
-    return cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ_gsip, k_gsip<SHAPE, XFORM, kWarpsPerBlock>, kWarpsPerBlock * 32, smem_gsip);
+    return cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ_gsip, k[2], kWarpsPerBlock * 32, smem_gsip);
 }
 
 // Resident CTAs per SM of k_outer / k_gsip for this shape and trajectory size: the host sizes the grids as
@@ -1541,13 +1647,8 @@ cudaError_t query_occupancy(const ShapeParams &S, int N, int blob_doubles, int *
     }
 }
 
-cudaError_t launch_pose_table(double *blob, int K1, cudaStream_t stream) {
-    k_pose_table<<<(K1 + 127) / 128, 128, 0, stream>>>(blob);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_cost_kernels(const KernelArgs &A, const ShapeParams &S, int N, int grid_outer, int grid_gsip,
-                                cudaStream_t stream, cudaEvent_t after_outer, int gsip_wide) {
+static cudaError_t launch_cost_impl(const KernelArgs &A, const ShapeParams &S, const ScaleSched *Z, int N, int grid_outer,
+                                    int grid_gsip, cudaStream_t stream, cudaEvent_t after_outer, int gsip_wide) {
     LaunchCfg cfg;
     cfg.after_outer = after_outer;
     cfg.gsip_wide = gsip_wide != 0;
@@ -1556,7 +1657,23 @@ cudaError_t launch_cost_kernels(const KernelArgs &A, const ShapeParams &S, int N
     cfg.smem_outer = outer_smem_doubles(A.blob_doubles, N) * sizeof(double);
     cfg.smem_gsip = (size_t)A.blob_doubles * sizeof(double);
     cfg.stream = stream;
-    return S.has_xform ? dispatch<true>(A, S, cfg, N) : dispatch<false>(A, S, cfg, N);
+    return S.has_xform ? dispatch<true>(A, S, Z, cfg, N) : dispatch<false>(A, S, Z, cfg, N);
+}
+
+#ifdef SVSDF_SCALED_UNIT
+cudaError_t launch_cost_kernels(const KernelArgs &A, const ShapeParams &S, const ScaleSched &Z, int N, int grid_outer, int grid_gsip,
+                                cudaStream_t stream, cudaEvent_t after_outer, int gsip_wide) {
+    return launch_cost_impl(A, S, &Z, N, grid_outer, grid_gsip, stream, after_outer, gsip_wide);
+}
+#else
+cudaError_t launch_pose_table(double *blob, int K1, cudaStream_t stream) {
+    k_pose_table<<<(K1 + 127) / 128, 128, 0, stream>>>(blob);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_cost_kernels(const KernelArgs &A, const ShapeParams &S, int N, int grid_outer, int grid_gsip,
+                                cudaStream_t stream, cudaEvent_t after_outer, int gsip_wide) {
+    return launch_cost_impl(A, S, nullptr, N, grid_outer, grid_gsip, stream, after_outer, gsip_wide);
 }
 
 cudaError_t launch_finalize(const double *partials, int n_blocks, int N, const int *n_inside,
@@ -1620,8 +1737,7 @@ cudaError_t launch_fp64_peak(double *out, int grid, int iters, cudaStream_t stre
     return cudaGetLastError();
 }
 
-// occupancy query used by the host to size the grids (CTAs per SM for k_outer of this shape is not needed to be
-// exact: we size for 2 resident CTAs per SM and let the hardware queue the rest)
+#endif  // SVSDF_SCALED_UNIT
 
 }  // namespace SVSDF_NS
 }  // namespace svsdf

@@ -24,6 +24,18 @@ namespace svsdf {
 SVSDF_DECLARE_LAUNCHERS(fast)
 SVSDF_DECLARE_LAUNCHERS(strict)
 #undef SVSDF_DECLARE_LAUNCHERS
+// deformable robots (svsdf_kernels_scaled_fast.cu / svsdf_kernels_scaled_strict.cu): the same cost kernels with the
+// schedule Z as an extra kernel parameter
+#define SVSDF_DECLARE_SCALED_LAUNCHERS(NS)                                                                       \
+    namespace NS {                                                                                               \
+    cudaError_t query_occupancy(const ShapeParams &S, int N, int blob_doubles, int *occ_outer, int *occ_gsip);   \
+    cudaError_t launch_cost_kernels(const KernelArgs &A, const ShapeParams &S, const ScaleSched &Z, int N,       \
+                                    int grid_outer, int grid_gsip, cudaStream_t stream, cudaEvent_t after_outer, \
+                                    int gsip_wide);                                                              \
+    }
+SVSDF_DECLARE_SCALED_LAUNCHERS(fast_scaled)
+SVSDF_DECLARE_SCALED_LAUNCHERS(strict_scaled)
+#undef SVSDF_DECLARE_SCALED_LAUNCHERS
 cudaError_t launch_extract_count(const ExtractArgs &E, int *block_counts, int n_blocks, int64_t *n_total,
                                  cudaStream_t stream);
 cudaError_t launch_extract_write(const ExtractArgs &E, const int *block_offsets, int n_blocks, double *out_xy,

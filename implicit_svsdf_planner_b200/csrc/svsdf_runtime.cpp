@@ -90,6 +90,10 @@ struct svsdf_ctx {
     int traj_N = 0;
     double traj_D = 0.0;
     int occ_N = -1, occ_blob = -1, occ_outer = 2, occ_gsip = 2;  // cached occupancy query
+    int occ_scaled = -1;          // which kernels (rigid 0 / scaled 1) the cached occupancy belongs to
+    // deformable robot (svsdf_set_scale): the scaled kernels run with this schedule
+    bool scaled = false;
+    ScaleSched sched{};
     int64_t last_n_inside = -1;  // interior points seen by the previous cost evaluation (picks the k_gsip variant)
     // reduction
     double *d_partials = nullptr;
@@ -360,16 +364,60 @@ int upload_traj(svsdf_ctx *ctx, int N, const double *T, const double *coeffs, bo
 }
 
 int refresh_occupancy(svsdf_ctx *ctx) {
-    if (ctx->occ_N == ctx->traj_N && ctx->occ_blob == ctx->layout.total) return SVSDF_OK;
+    const int sc = ctx->scaled ? 1 : 0;
+    if (ctx->occ_N == ctx->traj_N && ctx->occ_blob == ctx->layout.total && ctx->occ_scaled == sc) return SVSDF_OK;
     int oo = 0, og = 0;
-    cudaError_t e = ctx->strict ? strict::query_occupancy(ctx->shape, ctx->traj_N, ctx->layout.total, &oo, &og)
-                                : fast::query_occupancy(ctx->shape, ctx->traj_N, ctx->layout.total, &oo, &og);
+    const int N = ctx->traj_N, nb = ctx->layout.total;
+    cudaError_t e;
+    if (sc) e = ctx->strict ? strict_scaled::query_occupancy(ctx->shape, N, nb, &oo, &og)
+                            : fast_scaled::query_occupancy(ctx->shape, N, nb, &oo, &og);
+    else e = ctx->strict ? strict::query_occupancy(ctx->shape, N, nb, &oo, &og) : fast::query_occupancy(ctx->shape, N, nb, &oo, &og);
     CK(e);
     ctx->occ_outer = oo > 0 ? oo : 1;
     ctx->occ_gsip = og > 0 ? og : 1;
     ctx->occ_N = ctx->traj_N;
     ctx->occ_blob = ctx->layout.total;
+    ctx->occ_scaled = sc;
     return SVSDF_OK;
+}
+
+// The fdlibm sin of csrc/svsdf_sincos.cuh (Cody–Waite reduction, k_sin.c / k_cos.c polynomials with FMA) on the host,
+// for |x| < 1e6 (svsdf_set_scale keeps the schedule's arguments there): svsdf_scale_matrix returns the kernels' bits.
+double sin_portable_host(double x) {
+    const double v = std::fma(x, 0x1.45f306dc9c883p-1, 6755399441055744.0);
+    int64_t vb;
+    std::memcpy(&vb, &v, sizeof(vb));
+    const int q = (int)(uint32_t)(vb & 0xffffffffLL);
+    const double fn = v - 6755399441055744.0;
+    double r = std::fma(fn, -0x1.921fb54442d18p+0, x);
+    r = std::fma(fn, -0x1.1a62633145c07p-54, r);
+    r = std::fma(fn, 0x1.f1976b7ed8fbcp-110, r);
+    const double z = r * r;
+    double ps = std::fma(z, 1.58969099521155010221e-10, -2.50507602534068634195e-08);
+    ps = std::fma(z, ps, 2.75573137070700676789e-06);
+    ps = std::fma(z, ps, -1.98412698298579493134e-04);
+    ps = std::fma(z, ps, 8.33333333332248946124e-03);
+    ps = std::fma(z, ps, -1.66666666666666324348e-01);
+    const double sr = std::fma(r * z, ps, r);
+    double pc = std::fma(z, -1.13596475577881948265e-11, 2.08757232129817482790e-09);
+    pc = std::fma(z, pc, -2.75573143513906633035e-07);
+    pc = std::fma(z, pc, 2.48015872894767294178e-05);
+    pc = std::fma(z, pc, -1.38888888888741095749e-03);
+    pc = std::fma(z, pc, 4.16666666666666019037e-02);
+    const double cr = std::fma(z * z, pc, std::fma(z, -0.5, 1.0));
+    const double ss = (q & 1) ? cr : sr;
+    return (q & 2) ? -ss : ss;
+}
+
+bool scale_valid(const svsdf_scale &z) {
+    for (int d = 0; d < 2; ++d) {
+        const double v[4] = {z.a[d], z.b[d], z.w[d], z.phi[d]};
+        for (double x : v)
+            if (!std::isfinite(x)) return false;
+        if (!(z.a[d] - std::fabs(z.b[d]) > 0.0)) return false;  // S(t) stays invertible: |sin| <= 1, rounding is monotone
+        if (!(std::fabs(z.w[d]) * kMaxDuration + std::fabs(z.phi[d]) < 1e6)) return false;
+    }
+    return true;
 }
 
 int grid_for(const svsdf_ctx *ctx, int64_t P) {
@@ -445,10 +493,14 @@ int run_kernels(svsdf_ctx *ctx, const double *d_points, int64_t P, bool reduce, 
         ctx->err = "svsdf: trajectory blob does not fit in shared memory";
         return SVSDF_ERR_INVALID;
     }
-    cudaError_t e = ctx->strict ? strict::launch_cost_kernels(A, ctx->shape, N, grid, grid_gsip, ctx->stream,
-                                                              ctx->mark_kernels ? ctx->evk[2] : nullptr, gsip_wide)
-                                : fast::launch_cost_kernels(A, ctx->shape, N, grid, grid_gsip, ctx->stream,
-                                                            ctx->mark_kernels ? ctx->evk[2] : nullptr, gsip_wide);
+    cudaEvent_t mark = ctx->mark_kernels ? ctx->evk[2] : nullptr;
+    cudaError_t e;
+    if (ctx->scaled)
+        e = ctx->strict ? strict_scaled::launch_cost_kernels(A, ctx->shape, ctx->sched, N, grid, grid_gsip, ctx->stream, mark, gsip_wide)
+                        : fast_scaled::launch_cost_kernels(A, ctx->shape, ctx->sched, N, grid, grid_gsip, ctx->stream, mark, gsip_wide);
+    else
+        e = ctx->strict ? strict::launch_cost_kernels(A, ctx->shape, N, grid, grid_gsip, ctx->stream, mark, gsip_wide)
+                        : fast::launch_cost_kernels(A, ctx->shape, N, grid, grid_gsip, ctx->stream, mark, gsip_wide);
     CK(e);
     ctx->launches += gsip ? 3 : 1;
     if (ctx->mark_kernels) CK(cudaEventRecord(ctx->evk[3], ctx->stream));
@@ -1388,6 +1440,43 @@ int svsdf_device_ptr_points(svsdf_ctx *ctx, const double **dev_xy) {
         ctx->pts_inflight = false;
     }
     *dev_xy = ctx->d_points;
+    return SVSDF_OK;
+}
+
+int svsdf_set_scale(svsdf_ctx *ctx, const svsdf_scale *scale) {
+    if (!ctx) return SVSDF_ERR_INVALID;
+    if (!scale) {
+        ctx->scaled = false;
+        return SVSDF_OK;
+    }
+    if (!scale_valid(*scale)) {
+        ctx->err = "svsdf_set_scale: schedule must be finite with a_d - |b_d| > 0 and |w_d| * 300 + |phi_d| < 1e6";
+        return SVSDF_ERR_INVALID;
+    }
+    for (int d = 0; d < 2; ++d) {
+        ctx->sched.a[d] = scale->a[d];
+        ctx->sched.b[d] = scale->b[d];
+        ctx->sched.w[d] = scale->w[d];
+        ctx->sched.phi[d] = scale->phi[d];
+    }
+    ctx->scaled = true;
+    return SVSDF_OK;
+}
+
+int svsdf_scale_matrix(const svsdf_scale *scale, double t, double S_out[9], double Sinv_out[9]) {
+    if (!scale || !scale_valid(*scale) || !std::isfinite(t)) return SVSDF_ERR_INVALID;
+    // the arithmetic of scale_inv (svsdf_kernels.cuh) and Eigen 3.3's size-3 inverse of diag(sx, sy, 1)
+    const double sx = scale->a[0] + sin_portable_host(scale->w[0] * t + scale->phi[0]) * scale->b[0];
+    const double sy = scale->a[1] + sin_portable_host(scale->w[1] * t + scale->phi[1]) * scale->b[1];
+    const double inv = 1.0 / (sy * sx);
+    if (S_out) {
+        for (int k = 0; k < 9; ++k) S_out[k] = 0.0;
+        S_out[0] = sx; S_out[4] = sy; S_out[8] = 1.0;
+    }
+    if (Sinv_out) {
+        for (int k = 0; k < 9; ++k) Sinv_out[k] = 0.0;
+        Sinv_out[0] = sy * inv; Sinv_out[4] = sx * inv; Sinv_out[8] = (sx * sy) * inv;
+    }
     return SVSDF_OK;
 }
 

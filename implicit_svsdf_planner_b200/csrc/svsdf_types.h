@@ -78,6 +78,12 @@ struct ShapeParams {
     const float *fwn_trif;
 };
 
+// Deformable robot (svsdf_set_scale; the reference's getScale hook, sw_manager.hpp:495-503): per axis d = x, y
+// s_d(t) = a_d + sin(w_d t + phi_d) b_d, s_z = 1.  Passed by value to the scaled kernels only.
+struct ScaleSched {
+    double a[2], b[2], w[2], phi[2];
+};
+
 // Trajectory blob: one contiguous, 16-byte aligned buffer that the kernels pull into shared memory with a
 // single TMA bulk copy (cp.async.bulk.shared::cluster.global).  All offsets are in doubles.
 //   [0]  header (4 doubles: N, K1, D, reserved)

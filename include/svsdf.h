@@ -108,6 +108,22 @@ int svsdf_set_points_device(svsdf_ctx *ctx, const double *dev_xy, int64_t P);
 /* R2: updateTraj.  T: N durations; coeffs: MINCO `b`, 6N x 3 column-major. */
 int svsdf_set_traj(svsdf_ctx *ctx, int N, const double *T, const double *coeffs);
 
+/* Deformable robots: the reference's `useScale` switch and its `getScale(t)` hook (sw_manager.hpp:17, :495-503) as a
+ * schedule.  Per axis d = x, y: s_d(t) = a_d + sin(w_d t + phi_d) b_d; s_z = 1.  The reference's commented example is
+ * a = (0.8, 0.8), b = (0.6, 0.4), w = (1.5, 1.8), phi = (-1.0, 0.0).  Valid: every value finite, a_d - |b_d| > 0 (S stays
+ * invertible) and |w_d| * 300 + |phi_d| < 1e6 (the sin argument stays in the range of the fast reduction). */
+typedef struct svsdf_scale {
+    double a[2], b[2], w[2], phi[2];
+} svsdf_scale;
+/* NULL: rigid robot (the default).  A schedule turns on the scaled descent, FD gradient and chain rule for every later
+ * query, cost and evaluation on this context; the seed scan (choiceTInit) stays rigid as in the reference.  The
+ * schedule is copied.  Returns SVSDF_ERR_INVALID (and keeps the previous setting) for an invalid schedule. */
+int svsdf_set_scale(svsdf_ctx *ctx, const svsdf_scale *scale);
+/* S(t) and St.inverse() as 3x3 column-major matrices, with the arithmetic of the kernels: the pinned sin, Eigen 3.3's
+ * size-3 inverse (1/det with det = sy sx; Sinv = diag(sy/det', sx/det', (sx sy)/det') where 1/det' is rounded once).
+ * Either output may be NULL.  No context and no GPU needed. */
+int svsdf_scale_matrix(const svsdf_scale *scale, double t, double S_out[9], double Sinv_out[9]);
+
 /* R2: per-point swept-volume SDF query on the trajectory given by (N, T, coeffs).
  * pts: P x 3 (x, y, z) host doubles (z ignored).  Outputs (host, may be NULL): sdf[P], tstar[P], grad3[3P]
  * (body-frame FD gradient for sdf > 0; world-frame unit direction for the interior branch, exactly what the

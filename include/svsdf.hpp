@@ -127,6 +127,17 @@ class SweptVolumeManager {
         N_ = N; T_.assign(T, T + N); c_.assign(coeffs, coeffs + 18 * (size_t)N);
         return svsdf_set_traj(ctx_->h, N, T, coeffs);
     }
+    // useScale / getScale (:17, :495-503): a deformable robot with the schedule `scale` (nullptr: rigid, the default).
+    int setScale(const svsdf_scale *scale) {
+        has_scale_ = scale != nullptr;
+        if (scale) scale_ = *scale;
+        return svsdf_set_scale(ctx_->h, scale);
+    }
+    // getScale(t): S(t), 3x3 column-major (the identity for a rigid robot)
+    void getScale(double t, double S[9]) const {
+        if (!has_scale_ || svsdf_scale_matrix(&scale_, t, S, nullptr) != SVSDF_OK)
+            for (int k = 0; k < 9; ++k) S[k] = (k % 4 == 0) ? 1.0 : 0.0;
+    }
     // getTrueSDFofSweptVolume<true>(pos_eva, time_seed_f, grad_prel, set_ts) (:916-1018); set_ts is ignored like the reference's
     // call sites pass false (the scan always runs).
     double getTrueSDFofSweptVolume(const double pos_eva[3], double &time_seed_f, double grad_prel[3], bool /*set_ts*/ = false) {
@@ -172,6 +183,8 @@ class SweptVolumeManager {
     std::shared_ptr<detail::Ctx> ctx_;
     int N_ = 0;
     std::vector<double> T_, c_;
+    bool has_scale_ = false;
+    svsdf_scale scale_{};
 
    public:
     std::unique_ptr<shape::BasicShape> current_robot_shape;
