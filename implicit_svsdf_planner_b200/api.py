@@ -111,6 +111,7 @@ EXPORTED_SYMBOLS = [
     "svsdf_lmbm_default_params", "svsdf_lmbm_open", "svsdf_lmbm_close", "svsdf_lmbm_last_error", "svsdf_lmbm_minimize", "svsdf_set_lmbm_library", "svsdf_read_obj", "svsdf_free", "svsdf_mesh_fwn_host",
     "svsdf_front_init", "svsdf_front_get_kernels", "svsdf_front_cspace", "svsdf_front_check_kernel_value", "svsdf_front_expand", "svsdf_front_astar",
     "svsdf_front_astar_device", "svsdf_set_scale", "svsdf_scale_matrix",
+    "svsdf_cost_grad_multi", "svsdf_optimize_lockstep", "svsdf_lockstep_rounds",
 ]
 
 
@@ -187,6 +188,10 @@ def lib():
     L.svsdf_device_ptr_points.argtypes = [vp, C.POINTER(vp)]
     L.svsdf_set_scale.argtypes = [vp, C.POINTER(Scale)]
     L.svsdf_scale_matrix.argtypes = [C.POINTER(Scale), C.c_double, dp, dp]
+    L.svsdf_cost_grad_multi.argtypes = [vp, C.c_int, C.POINTER(MultiProblem)]
+    L.svsdf_optimize_lockstep.argtypes = [vp, C.POINTER(LockstepProblem), C.c_int, C.POINTER(LbfgsParams), C.c_int, C.POINTER(OptStats),
+                                          C.POINTER(C.c_int)]
+    L.svsdf_lockstep_rounds.argtypes = [vp, C.POINTER(C.c_int64)]
     _lib = L
     return L
 
@@ -309,6 +314,18 @@ class Problem(C.Structure):
 
 
 NEXT_T = C.CFUNCTYPE(C.c_int, C.c_void_p)
+
+
+class MultiProblem(C.Structure):
+    """svsdf_multi_problem (include/svsdf.h)."""
+    _fields_ = [("N", C.c_int), ("T", dp), ("coeffs", dp), ("points", dp), ("P", C.c_int64), ("stride", C.c_int),
+                ("cost_io", dp), ("gradT_io", dp), ("gradC_io", dp), ("n_inside_out", C.POINTER(C.c_int64))]
+
+
+class LockstepProblem(C.Structure):
+    """svsdf_lockstep_problem (include/svsdf.h)."""
+    _fields_ = [("N", C.c_int), ("initS", dp), ("finalS", dp), ("opt_x", dp), ("points", dp), ("P", C.c_int64), ("stride", C.c_int),
+                ("T_out", dp), ("coeffs_out", dp), ("f0_out", dp)]
 
 
 def optimize_batch(ctxs, problems, N, params=None, next_index=None):
@@ -574,6 +591,58 @@ class Context:
         stats = dict(final_cost=st.final_cost, iterations=st.iterations, evaluations=st.evaluations, status=st.status,
                      seconds=st.seconds, gpu_seconds=st.gpu_seconds)
         return rc, x, T, b, stats
+
+    def cost_grad_multi(self, problems):
+        """svsdf_cost_grad_multi: one evaluation of every problem in one set of launches.  problems: list of (T [N], coeffs_colmajor
+        [18 N], points [P, >= 2]).  Returns a list of (cost, gradT [N], gradC [18 N], n_inside), each the bits of set_points + cost_grad."""
+        n = len(problems)
+        arr = (MultiProblem * max(n, 1))()
+        keep, res = [], []
+        for k, (T, co, pts) in enumerate(problems):
+            T, co = _f64(T).reshape(-1), _f64(co).reshape(-1)
+            pts = _f64(pts).reshape(len(pts), -1) if len(pts) else np.zeros((0, 2))
+            N = T.shape[0]
+            cost, gT, gC, ni = np.zeros(1), np.zeros(N), np.zeros(18 * N), np.zeros(1, dtype=np.int64)
+            a = arr[k]
+            a.N, a.T, a.coeffs, a.points, a.P, a.stride = N, _p(T), _p(co), _p(pts) if pts.shape[0] else None, pts.shape[0], pts.shape[1]
+            a.cost_io, a.gradT_io, a.gradC_io, a.n_inside_out = _p(cost), _p(gT), _p(gC), ni.ctypes.data_as(C.POINTER(C.c_int64))
+            keep += [T, co, pts]
+            res.append((cost, gT, gC, ni))
+        self._ck(lib().svsdf_cost_grad_multi(self.h, n, arr), "svsdf_cost_grad_multi")
+        return [(float(c[0]), gT, gC, int(ni[0])) for c, gT, gC, ni in res]
+
+    def optimize_lockstep(self, problems, params: LbfgsParams | None = None, max_in_flight: int = 0):
+        """svsdf_optimize_lockstep: problems = list of dicts with init_s, final_s (3x3), x0, N and points [P, >= 2].  Returns
+        (results, rounds): per problem a dict (status, x, T, coeffs, cost_at_start, and the stats of optimize) equal to optimize's bits."""
+        n = len(problems)
+        arr = (LockstepProblem * max(n, 1))()
+        keep, outs = [], []
+        for k, pr in enumerate(problems):
+            N = int(pr["N"])
+            i_s, f_s = _colmajor33(pr["init_s"]), _colmajor33(pr["final_s"])
+            x = _f64(pr["x0"]).copy()
+            pts = _f64(pr["points"])
+            pts = pts.reshape(pts.shape[0], -1) if pts.shape[0] else np.zeros((0, 2))
+            T, b, f0 = np.empty(N), np.empty(18 * N), np.full(1, np.nan)
+            a = arr[k]
+            a.N, a.initS, a.finalS, a.opt_x = N, _p(i_s), _p(f_s), _p(x)
+            a.points, a.P, a.stride = (_p(pts) if pts.shape[0] else None), pts.shape[0], pts.shape[1]
+            a.T_out, a.coeffs_out, a.f0_out = _p(T), _p(b), _p(f0)
+            keep += [i_s, f_s, pts]
+            outs.append((x, T, b, f0))
+        stats = (OptStats * max(n, 1))()
+        status = np.zeros(max(n, 1), dtype=np.int32)
+        self._ck(lib().svsdf_optimize_lockstep(self.h, arr, n, C.byref(params) if params is not None else None, int(max_in_flight), stats,
+                                               status.ctypes.data_as(C.POINTER(C.c_int))), "svsdf_optimize_lockstep")
+        rounds = C.c_int64()
+        lib().svsdf_lockstep_rounds(self.h, C.byref(rounds))
+        res = []
+        for k, (x, T, b, f0) in enumerate(outs):
+            s = stats[k]
+            res.append(dict(status=int(status[k]), x=x, T=T, coeffs=b, cost_at_start=float(f0[0]), final_cost=s.final_cost,
+                            iterations=s.iterations, evaluations=s.evaluations, solver_status=s.status, seconds=s.seconds,
+                            gpu_seconds=s.gpu_seconds))
+        return res, rounds.value
 
     def shape_sdf(self, rel):
         rel = _f64(rel).reshape(-1, 3)

@@ -29,6 +29,11 @@ UNITS = [
     # deformable robots (svsdf_set_scale): the scaled k_outer / k_gsip instantiations, fast and strict
     ("svsdf_kernels_scaled_fast.cu", "svsdf_kernels_scaled_fast.o", []),
     ("svsdf_kernels_scaled_strict.cu", "svsdf_kernels_scaled_strict.o", ["-fmad=false"]),
+    # svsdf_cost_grad_multi: n problems per set of launches (rigid and scaled, fast and strict)
+    ("svsdf_kernels_multi_fast.cu", "svsdf_kernels_multi_fast.o", []),
+    ("svsdf_kernels_multi_strict.cu", "svsdf_kernels_multi_strict.o", ["-fmad=false"]),
+    ("svsdf_kernels_multi_scaled_fast.cu", "svsdf_kernels_multi_scaled_fast.o", []),
+    ("svsdf_kernels_multi_scaled_strict.cu", "svsdf_kernels_multi_scaled_strict.o", ["-fmad=false"]),
     ("svsdf_extract.cu", "svsdf_extract.o", ["-fmad=false"]),  # cell centres must round like the host formula
     ("svsdf_frontend.cu", "svsdf_frontend.o", ["-fmad=false"]),  # shape kernels: same rounding as the strict functors
     # host threads for the batch A* bookkeeping; no a*b+c contraction in the float winding-number builder (host/fwn_bvh.hpp)
@@ -36,6 +41,7 @@ UNITS = [
 ]
 HEADERS = [
     "svsdf_kernels.cuh",
+    "svsdf_kernels_multi.cuh",
     "svsdf_shapes.cuh",
     "svsdf_sincos.cuh",
     "svsdf_types.h",
@@ -46,6 +52,7 @@ HEADERS = [
     "host/astar_flat.hpp",
     "host/fwn_bvh.hpp",
     "host/mid_end.hpp",
+    "host/rendezvous.hpp",
     "../../include/svsdf.h",
 ]
 

@@ -1004,10 +1004,9 @@ __device__ __forceinline__ void tma_load_blob(double *smem_blob, const double *g
 // steps), so they are computed once per evaluation instead of once per point.  Rigid for a deformable robot too: the
 // layer-1 scan does not read the scale.
 // ------------------------------------------------------------------------------------------------
-#ifndef SVSDF_SCALED_UNIT
-__global__ void k_pose_table(double *blob) {
+// (shared with k_pose_table_multi, svsdf_kernels_multi.cuh)
+__device__ __forceinline__ void pose_table_entry(double *blob, int k) {
     TrajView tv = make_view(blob);
-    int k = blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= tv.K1) return;
     double x, y, yaw, sy, cy;
     traj_pos(tv, tv.lat[k], x, y, yaw);
@@ -1016,6 +1015,8 @@ __global__ void k_pose_table(double *blob) {
     double *ps = blob + L.off_pose + k;
     ps[0] = x; ps[L.K1pad] = y; ps[2 * L.K1pad] = cy; ps[3 * L.K1pad] = sy;
 }
+#if !defined(SVSDF_SCALED_UNIT) && !defined(SVSDF_MULTI_UNIT)
+__global__ void k_pose_table(double *blob) { pose_table_entry(blob, blockIdx.x * blockDim.x + threadIdx.x); }
 #endif
 
 // ------------------------------------------------------------------------------------------------
@@ -1036,8 +1037,10 @@ __global__ void k_pose_table(double *blob) {
 #endif
 // BATCHED selects the schedule at compile time (two kernels: each carries only its own evaluation sites).
 // SCALED: deformable robot with the schedule *Z (k_outer_scaled); the rigid k_outer passes nullptr and never reads it.
+// vblock / vgrid: this CTA's index and the grid it belongs to — blockIdx.x / gridDim.x for k_outer; for k_outer_multi the
+// problem's virtual grid, so that every problem keeps the decomposition (and the partial sums) of its single-problem call.
 template <int SHAPE, bool XFORM, bool BATCHED, bool SCALED>
-__device__ __forceinline__ void outer_body(const KernelArgs &A, const ShapeParams &S, const ScaleSched *Z) {
+__device__ __forceinline__ void outer_body(const KernelArgs &A, const ShapeParams &S, const ScaleSched *Z, int vblock, int vgrid) {
     extern __shared__ __align__(16) double smem[];
     __shared__ __align__(8) uint64_t bar;
     __shared__ int s_nb[kWarpsPerBlock];
@@ -1052,8 +1055,8 @@ __device__ __forceinline__ void outer_body(const KernelArgs &A, const ShapeParam
         for (int e = lane; e < nacc; e += 32) acc[e] = 0.0;
     __syncwarp();
 
-    const int64_t wstride = (int64_t)gridDim.x * kWarpsPerBlock;
-    const int64_t first = (int64_t)blockIdx.x * kWarpsPerBlock + warp;
+    const int64_t wstride = (int64_t)vgrid * kWarpsPerBlock;
+    const int64_t first = (int64_t)vblock * kWarpsPerBlock + warp;
     unsigned long long my_evals = 0;
     double *res = smem + A.blob_doubles + kWarpsPerBlock * nacc + warp * 128;  // per-warp work area of the descent engine
     // The warp walks its points in batches of up to 32 (lane i <-> i-th point of the batch).
@@ -1158,26 +1161,27 @@ __device__ __forceinline__ void outer_body(const KernelArgs &A, const ShapeParam
             double s = 0.0;
 #pragma unroll
             for (int w = 0; w < kWarpsPerBlock; ++w) s += acc0[w * nacc + e];
-            A.partials[(int64_t)blockIdx.x * nacc + e] = s;
+            A.partials[(int64_t)vblock * nacc + e] = s;
         }
     }
 }
 template <int SHAPE, bool XFORM, bool BATCHED>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32, (SHAPE == SH_MESH) ? SVSDF_MESH_MIN_CTAS : SVSDF_OUTER_MIN_CTAS)
     k_outer(const __grid_constant__ KernelArgs A, const __grid_constant__ ShapeParams S) {
-    outer_body<SHAPE, XFORM, BATCHED, false>(A, S, nullptr);
+    outer_body<SHAPE, XFORM, BATCHED, false>(A, S, nullptr, blockIdx.x, gridDim.x);
 }
 template <int SHAPE, bool XFORM, bool BATCHED>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32, (SHAPE == SH_MESH) ? SVSDF_MESH_MIN_CTAS : SVSDF_OUTER_MIN_CTAS)
     k_outer_scaled(const __grid_constant__ KernelArgs A, const __grid_constant__ ShapeParams S, const __grid_constant__ ScaleSched Z) {
-    outer_body<SHAPE, XFORM, BATCHED, true>(A, S, &Z);
+    outer_body<SHAPE, XFORM, BATCHED, true>(A, S, &Z, blockIdx.x, gridDim.x);
 }
 
 // ------------------------------------------------------------------------------------------------
 // k_compact: ordered compaction of the inside flags (single CTA, 1024 threads) -> inside_list, n_inside.
 // Flags are 0/1 bytes; every thread owns a contiguous run of 16-byte words (coalesced uint4 loads, popcount).
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(1024) k_compact(const unsigned char *flag, int64_t P, int *list, int *n_out) {
+// (the body is shared with k_compact_multi, one CTA per problem; flag must be 16-byte aligned)
+__device__ __forceinline__ void compact_body(const unsigned char *flag, int64_t P, int *list, int *n_out) {
     __shared__ int wsum[32];
     __shared__ int total;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -1229,6 +1233,11 @@ __global__ void __launch_bounds__(1024) k_compact(const unsigned char *flag, int
     }
     if (tid == 0) *n_out = total;
 }
+#ifndef SVSDF_MULTI_UNIT
+__global__ void __launch_bounds__(1024) k_compact(const unsigned char *flag, int64_t P, int *list, int *n_out) {
+    compact_body(flag, P, list, n_out);
+}
+#endif
 
 // ------------------------------------------------------------------------------------------------
 // K2: interior branch of getTrueSDFofSweptVolume<true> (sw_manager.hpp:926-1017, SampleSet2D :41-124).
@@ -1237,23 +1246,40 @@ __global__ void __launch_bounds__(1024) k_compact(const unsigned char *flag, int
 // dynamic smem: [ blob ]
 // ------------------------------------------------------------------------------------------------
 // SCALED: the ring samples run scaled descents (getSDFofSweptVolume<useScale>); the velocity fallback and the ring do not change.
-template <int SHAPE, bool XFORM, int WARPS, bool SCALED>
-__device__ __forceinline__ void gsip_body(const KernelArgs &A, const ShapeParams &S, const ScaleSched *Z) {
+// The slots of the interior branch come from a VIEW: GsipSingle below (k_gsip: one blob, loaded once, slot s = inside point
+// A.inside_list[s]); k_gsip_multi's view (svsdf_kernels_multi.cuh) maps a slot of the concatenated lists to its problem and reloads the
+// CTA's blob when the problem changes.  The body is the same for both.
+struct GsipSingle {
+    const KernelArgs &A;
+    __device__ __forceinline__ void start(double *sblob, uint64_t *bar) const { tma_load_blob(sblob, A.blob, A.blob_doubles, bar); }
+    __device__ __forceinline__ int count() const { return *A.n_inside; }
+    // point index of the slot and the arrays it indexes; true when the blob in shared memory was replaced (never here)
+    __device__ __forceinline__ bool at(int slot, double *, uint64_t *, int &pt, const double *&pts, const double *&tstar) const {
+        pt = A.inside_list[slot];
+        pts = A.points_xy;
+        tstar = A.inside_tstar;
+        return false;
+    }
+};
+template <int SHAPE, bool XFORM, int WARPS, bool SCALED, class View>
+__device__ __forceinline__ void gsip_body(const KernelArgs &A, const ShapeParams &S, const ScaleSched *Z, const View &view) {
     extern __shared__ __align__(16) double smem[];
     __shared__ __align__(8) uint64_t bar;
     __shared__ double s_theta[24], s_val[24], s_ts[24];
     double *sblob = smem;
-    tma_load_blob(sblob, A.blob, A.blob_doubles, &bar);
-    const TrajView tv = make_view(sblob);
+    view.start(sblob, &bar);
+    TrajView tv = make_view(sblob);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const double PI = 3.14159265358979323846;  // Shape.hpp:31
-    const int n_in = *A.n_inside;
+    const int n_in = view.count();
     unsigned long long my_evals = 0;
 
     for (int slot = blockIdx.x; slot < n_in; slot += gridDim.x) {
-        const int pt = A.inside_list[slot];
-        const double px = __ldg(A.points_xy + 2 * (int64_t)pt), py = __ldg(A.points_xy + 2 * (int64_t)pt + 1);
-        const double ts0 = A.inside_tstar[pt];
+        int pt;
+        const double *pts, *in_tstar;
+        if (view.at(slot, sblob, &bar, pt, pts, in_tstar)) tv = make_view(sblob);
+        const double px = __ldg(pts + 2 * (int64_t)pt), py = __ldg(pts + 2 * (int64_t)pt + 1);
+        const double ts0 = in_tstar[pt];
         // velocity at t* with the reference's fallback scan (:928-954); all threads redundantly
         double vx, vy, vw;
         traj_vel(tv, ts0, vx, vy, vw);
@@ -1353,12 +1379,12 @@ __device__ __forceinline__ void gsip_body(const KernelArgs &A, const ShapeParams
 template <int SHAPE, bool XFORM, int WARPS>
 __global__ void __launch_bounds__(WARPS * 32, (WARPS == kWarpsPerBlock && SHAPE != SH_MESH) ? SVSDF_GSIP_MIN_CTAS : 1)
     k_gsip(const __grid_constant__ KernelArgs A, const __grid_constant__ ShapeParams S) {
-    gsip_body<SHAPE, XFORM, WARPS, false>(A, S, nullptr);
+    gsip_body<SHAPE, XFORM, WARPS, false>(A, S, nullptr, GsipSingle{A});
 }
 template <int SHAPE, bool XFORM, int WARPS>
 __global__ void __launch_bounds__(WARPS * 32, (WARPS == kWarpsPerBlock && SHAPE != SH_MESH) ? SVSDF_GSIP_MIN_CTAS : 1)
     k_gsip_scaled(const __grid_constant__ KernelArgs A, const __grid_constant__ ShapeParams S, const __grid_constant__ ScaleSched Z) {
-    gsip_body<SHAPE, XFORM, WARPS, true>(A, S, &Z);
+    gsip_body<SHAPE, XFORM, WARPS, true>(A, S, &Z, GsipSingle{A});
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1369,20 +1395,19 @@ __global__ void __launch_bounds__(WARPS * 32, (WARPS == kWarpsPerBlock && SHAPE 
 // reference's rule gradT(j) += gdT for all j < piece (back_end_optimizer.hpp:859-862), [1+19N] n_inside.
 // (k_finalize and the utility kernels below live in the rigid units only: the scaled units share them.)
 // ------------------------------------------------------------------------------------------------
-#ifndef SVSDF_SCALED_UNIT
 __device__ __forceinline__ double warp_sum_fixed(double v) {
 #pragma unroll
     for (int off = 16; off > 0; off >>= 1) v += __shfl_down_sync(FULL, v, off);
     return __shfl_sync(FULL, v, 0);
 }
 
-__global__ void __launch_bounds__(256) k_finalize(const double *partials, int n_blocks, int N, const int *n_inside,
-                                                  const double *gsip_contrib, const int *gsip_piece, double *tot,
-                                                  unsigned int *ticket, double *out) {
+// bx / nbx: this CTA's index among the nbx CTAs that finalize one record (blockIdx.x / gridDim.x for k_finalize; k_finalize_multi
+// runs one such group per problem)
+__device__ __forceinline__ void finalize_body(const double *partials, int n_blocks, int N, int n_in, const double *gsip_contrib,
+                                              const int *gsip_piece, double *tot, unsigned int *ticket, double *out, int bx, int nbx) {
     const int nacc = 19 * N + 1;
-    const int n_in = n_inside ? *n_inside : 0;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int e = blockIdx.x * 8 + warp;
+    const int e = bx * 8 + warp;
     if (e < nacc) {
         double s = 0.0;
         for (int b = lane; b < n_blocks; b += 32) s += partials[(int64_t)b * nacc + e];
@@ -1406,7 +1431,7 @@ __global__ void __launch_bounds__(256) k_finalize(const double *partials, int n_
     __shared__ bool last;
     __threadfence();
     __syncthreads();
-    if (threadIdx.x == 0) last = (atomicAdd(ticket, 1u) == gridDim.x - 1);
+    if (threadIdx.x == 0) last = (atomicAdd(ticket, 1u) == (unsigned)nbx - 1);
     __syncthreads();
     if (!last) return;
     __threadfence();
@@ -1428,6 +1453,13 @@ __global__ void __launch_bounds__(256) k_finalize(const double *partials, int n_
         out[1 + 19 * N] = (double)n_in;
         *ticket = 0u;  // re-arm for the next evaluation
     }
+}
+
+#if !defined(SVSDF_SCALED_UNIT) && !defined(SVSDF_MULTI_UNIT)
+__global__ void __launch_bounds__(256) k_finalize(const double *partials, int n_blocks, int N, const int *n_inside,
+                                                  const double *gsip_contrib, const int *gsip_piece, double *tot,
+                                                  unsigned int *ticket, double *out) {
+    finalize_body(partials, n_blocks, N, n_inside ? *n_inside : 0, gsip_contrib, gsip_piece, tot, ticket, out, blockIdx.x, gridDim.x);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1502,6 +1534,8 @@ constexpr bool kScaledUnit = true;
 #else
 constexpr bool kScaledUnit = false;
 #endif
+// the multi-problem units (svsdf_kernels_multi*.cu) bring their own launchers (svsdf_kernels_multi.cuh)
+#ifndef SVSDF_MULTI_UNIT
 
 struct LaunchCfg {
     int grid_outer, grid_gsip;
@@ -1738,6 +1772,7 @@ cudaError_t launch_fp64_peak(double *out, int grid, int iters, cudaStream_t stre
 }
 
 #endif  // SVSDF_SCALED_UNIT
+#endif  // SVSDF_MULTI_UNIT
 
 }  // namespace SVSDF_NS
 }  // namespace svsdf

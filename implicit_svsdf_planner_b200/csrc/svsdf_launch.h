@@ -36,6 +36,30 @@ SVSDF_DECLARE_LAUNCHERS(strict)
 SVSDF_DECLARE_SCALED_LAUNCHERS(fast_scaled)
 SVSDF_DECLARE_SCALED_LAUNCHERS(strict_scaled)
 #undef SVSDF_DECLARE_SCALED_LAUNCHERS
+// svsdf_cost_grad_multi (svsdf_kernels_multi.cuh).  launch_multi: what = 0 sparse / 1 batched k_outer_multi, 2 k_gsip_multi (grid <= 0:
+// one full wave of the chosen variant); Z is read by the scaled units only.  The rigid units also run the pose table, the
+// compaction and the finalize of every multi launch.
+#define SVSDF_DECLARE_MULTI_LAUNCHERS(NS)                                                                         \
+    namespace NS {                                                                                               \
+    cudaError_t launch_multi(int what, const KernelArgs &A, const MultiArgs &M, const ShapeParams &S,            \
+                             const ScaleSched *Z, int grid, size_t smem, int gsip_wide, int sm_count,            \
+                             cudaStream_t st);                                                                   \
+    }
+SVSDF_DECLARE_MULTI_LAUNCHERS(fast_multi)
+SVSDF_DECLARE_MULTI_LAUNCHERS(strict_multi)
+SVSDF_DECLARE_MULTI_LAUNCHERS(fast_multi_scaled)
+SVSDF_DECLARE_MULTI_LAUNCHERS(strict_multi_scaled)
+#undef SVSDF_DECLARE_MULTI_LAUNCHERS
+#define SVSDF_DECLARE_MULTI_RIGID(NS)                                                                            \
+    namespace NS {                                                                                               \
+    cudaError_t launch_pose_multi(double *blobs, const MultiArgs &M, int max_K1, cudaStream_t st);               \
+    cudaError_t launch_compact_multi(const unsigned char *flag, int *list, const MultiArgs &M, cudaStream_t st); \
+    cudaError_t launch_finalize_multi(const double *partials, const double *gsip_contrib, const int *gsip_piece, \
+                                      const MultiArgs &M, int max_N, cudaStream_t st);                           \
+    }
+SVSDF_DECLARE_MULTI_RIGID(fast_multi)
+SVSDF_DECLARE_MULTI_RIGID(strict_multi)
+#undef SVSDF_DECLARE_MULTI_RIGID
 cudaError_t launch_extract_count(const ExtractArgs &E, int *block_counts, int n_blocks, int64_t *n_total,
                                  cudaStream_t stream);
 cudaError_t launch_extract_write(const ExtractArgs &E, const int *block_offsets, int n_blocks, double *out_xy,

@@ -15,11 +15,15 @@
 #include <algorithm>
 #include <cmath>
 #include <dlfcn.h>
+#include <functional>
 #include <unistd.h>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <map>
+#include <pthread.h>
 #include <string>
+#include <tuple>
 #include <vector>
 
 #include "../../include/svsdf.h"
@@ -28,10 +32,58 @@
 #include "host/mid_end.hpp"
 #include "host/lbfgs.hpp"
 #include "host/minco.hpp"
+#include "host/rendezvous.hpp"
 #include "svsdf_launch.h"
 #include "svsdf_types.h"
 
 using namespace svsdf;
+
+// The host half of one back-end evaluation (back_end_optimizer.hpp:353-398), shared by svsdf_evaluate and the lock-step back end
+// (svsdf_optimize_lockstep).  forward(): tau -> T and MINCO (coefficients, energy and its partial gradients), before the device
+// evaluation; backward(): adds the device record, propagates through MINCO and adds rho * sum(T).
+struct HostEval {
+    host::MincoS3NU minco;
+    int N = 0;
+    std::vector<double> times, gradByTimes, partialGradByTimes, partialGradByCoeffs, gradByPoints;
+    double energy = 0.0;
+
+    void setup(const double *initS, const double *finalS, int n_pieces) {
+        N = n_pieces;
+        minco.setConditions(initS, finalS, N);
+        times.assign(N, 0.0);
+        gradByTimes.assign(N, 0.0);
+        partialGradByTimes.assign(N, 0.0);
+        partialGradByCoeffs.assign((size_t)18 * N, 0.0);
+        gradByPoints.assign((size_t)3 * (N - 1), 0.0);
+    }
+    // forwardT / forwardP (back_end_optimizer.hpp:353-354)
+    void forward(const double *x) {
+        for (int i = 0; i < N; ++i) times[i] = host::forwardT(x[i]);
+        minco.setParameters(x + N, times.data());
+        energy = minco.getEnergy();
+        minco.getEnergyPartialGradByCoeffs(partialGradByCoeffs.data());
+        minco.getEnergyPartialGradByTimes(partialGradByTimes.data());
+    }
+    // o: the device record [cost, gradC (18N), gradT (N), n_inside] of the trajectory forward() built
+    double backward(const double *o, const double *x, double rho, double *g, double *pos_out, double *other_out) {
+        double cost = energy;
+        const double energy_cost = cost;
+        cost += o[0];
+        for (int e = 0; e < 18 * N; ++e) partialGradByCoeffs[e] += o[1 + e];
+        for (int i = 0; i < N; ++i) partialGradByTimes[i] += o[1 + 18 * N + i];
+        const double pos_cost = cost - energy_cost;
+        minco.propogateGrad(partialGradByCoeffs.data(), partialGradByTimes.data(), gradByPoints.data(), gradByTimes.data());
+        double tsum = 0.0;
+        for (int i = 0; i < N; ++i) tsum += times[i];
+        cost += rho * tsum;
+        for (int i = 0; i < N; ++i) gradByTimes[i] += rho;
+        *pos_out = pos_cost;
+        *other_out = cost - pos_cost;
+        for (int i = 0; i < N; ++i) g[i] = host::backwardGradT(x[i], gradByTimes[i]);
+        for (int i = 0; i < 3 * (N - 1); ++i) g[N + i] = gradByPoints[i];
+        return cost;
+    }
+};
 
 struct svsdf_ctx {
     svsdf_config cfg;
@@ -132,10 +184,8 @@ struct svsdf_ctx {
     int64_t *d_n_total = nullptr;
 
     // optimiser state (R3/R4)
-    host::MincoS3NU minco;
-    int pieceN = 0;
+    HostEval he;
     bool have_boundary = false;
-    std::vector<double> times, gradByTimes, partialGradByTimes, partialGradByCoeffs, gradByPoints;
     double cost_pos = 0, cost_other = 0, cost_total = 0;
     int n_evaluate = 0;
     double gpu_ms_total = 0.0;
@@ -153,6 +203,19 @@ struct svsdf_ctx {
     // test hook of the device A*, read ONCE at svsdf_create: SVSDF_FORCE_GRID_ASTAR = n > 0 sets k_astar_search's grid (1 = one
     // CTA runs every search on the same slot); -1 = not set
     int force_grid_astar = -1;
+    // svsdf_cost_grad_multi / svsdf_optimize_lockstep: packed inputs (one pinned stage mirrored by one device block, one copy in),
+    // grow-only scratch, pinned outputs (one copy out)
+    unsigned char *h_multi_in = nullptr, *d_multi_in = nullptr;
+    size_t cap_multi_in = 0;
+    unsigned char *d_multi_scratch = nullptr;
+    size_t cap_multi_scratch = 0;
+    double *h_multi_out = nullptr;
+    size_t cap_multi_out = 0;
+    unsigned int *d_multi_tickets = nullptr;  // [0] k_compact_multi's, [1 + k] problem k's k_finalize_multi ticket; zero between calls
+    int cap_multi_tickets = 0;
+    int64_t multi_last_inside = -1;  // inside points of the previous multi evaluation (picks the k_gsip_multi variant)
+    std::map<std::tuple<int, int, int>, int> occ_cache;  // (N, blob doubles, scaled) -> resident single-problem k_outer CTAs per SM
+    int64_t lockstep_rounds = 0;  // rounds of the last svsdf_optimize_lockstep
 };
 
 namespace {
@@ -304,28 +367,59 @@ int pose_table(svsdf_ctx *ctx) {
     return SVSDF_OK;
 }
 
-int upload_traj(svsdf_ctx *ctx, int N, const double *T, const double *coeffs, bool launch_pose = true) {
+// updateTraj's checks (sw_manager.hpp:376-385) and the blob layout of one trajectory; on failure the message is in *err
+int traj_layout(int N, const double *T, const double *coeffs, BlobLayout &L, double &D, const char **err) {
     if (N < 1 || N > kMaxPieces || !T || !coeffs) {
-        ctx->err = "svsdf: N out of range (1..64) or null trajectory";
+        *err = "svsdf: N out of range (1..64) or null trajectory";
         return SVSDF_ERR_INVALID;
     }
-    double D = 0.0;  // Trajectory::getTotalDuration (trajectory.hpp:410-419)
+    D = 0.0;  // Trajectory::getTotalDuration (trajectory.hpp:410-419)
     for (int i = 0; i < N; ++i) {
         if (!(T[i] > 0.0) || !std::isfinite(T[i])) {
-            ctx->err = "svsdf: non-positive or non-finite piece duration";
+            *err = "svsdf: non-positive or non-finite piece duration";
             return SVSDF_ERR_INVALID;
         }
         D += T[i];
     }
     if (!(D < kMaxDuration)) {
         // The reference silently keeps the previous duration in this case (sw_manager.hpp:380); we refuse.
-        ctx->err = "svsdf: total duration >= 300 s is not supported (reference updateTraj ignores it)";
+        *err = "svsdf: total duration >= 300 s is not supported (reference updateTraj ignores it)";
         return SVSDF_ERR_INVALID;
     }
     // layer-1 lattice: for (t = 0; t <= D; t += 0.15)
     int K1 = 0;
     for (double t = 0.0; t <= D; t += 0.15) K1++;
-    BlobLayout L = blob_layout(N, K1);
+    L = blob_layout(N, K1);
+    return SVSDF_OK;
+}
+
+// the host part of the blob (everything before the pose rows, which k_pose_table fills)
+void fill_blob(double *h, const BlobLayout &L, const double *T, const double *coeffs, double D) {
+    const int N = L.N;
+    std::memset(h, 0, (size_t)L.off_pose * sizeof(double));
+    h[0] = (double)N;
+    h[1] = (double)L.K1;
+    h[2] = D;
+    for (int i = 0; i < N; ++i) h[L.off_T + i] = T[i];
+    // coefficients: MINCO b (col-major 6N x 3) -> [piece][dim][power]  (minco.hpp:515-528 builds the same
+    // per-piece matrices, stored there highest power first)
+    for (int i = 0; i < N; ++i)
+        for (int d = 0; d < 3; ++d)
+            for (int k = 0; k < 6; ++k) h[L.off_c + 18 * i + 6 * d + k] = coeffs[(size_t)d * 6 * N + 6 * i + k];
+    {
+        int k = 0;
+        for (double t = 0.0; t <= D; t += 0.15) h[L.off_lat + k++] = t;
+    }
+}
+
+int upload_traj(svsdf_ctx *ctx, int N, const double *T, const double *coeffs, bool launch_pose = true) {
+    BlobLayout L;
+    double D = 0.0;
+    const char *msg = nullptr;
+    if (traj_layout(N, T, coeffs, L, D, &msg) != SVSDF_OK) {
+        ctx->err = msg;
+        return SVSDF_ERR_INVALID;
+    }
     if (L.total > ctx->cap_hblob) {
         if (ctx->h_blob) cudaFreeHost(ctx->h_blob);
         ctx->h_blob = nullptr;
@@ -341,20 +435,7 @@ int upload_traj(svsdf_ctx *ctx, int N, const double *T, const double *coeffs, bo
         ctx->cap_blob = L.total + 1024;
     }
     double *h = ctx->h_blob;
-    std::memset(h, 0, (size_t)L.off_pose * sizeof(double));
-    h[0] = (double)N;
-    h[1] = (double)K1;
-    h[2] = D;
-    for (int i = 0; i < N; ++i) h[L.off_T + i] = T[i];
-    // coefficients: MINCO b (col-major 6N x 3) -> [piece][dim][power]  (minco.hpp:515-528 builds the same
-    // per-piece matrices, stored there highest power first)
-    for (int i = 0; i < N; ++i)
-        for (int d = 0; d < 3; ++d)
-            for (int k = 0; k < 6; ++k) h[L.off_c + 18 * i + 6 * d + k] = coeffs[(size_t)d * 6 * N + 6 * i + k];
-    {
-        int k = 0;
-        for (double t = 0.0; t <= D; t += 0.15) h[L.off_lat + k++] = t;
-    }
+    fill_blob(h, L, T, coeffs, D);
     CK(cudaMemcpyAsync(ctx->d_blob, h, (size_t)L.off_pose * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
     ctx->layout = L;
     ctx->traj_N = N;
@@ -540,44 +621,250 @@ int cost_grad_raw(svsdf_ctx *ctx, int N, const double *T, const double *coeffs) 
 }
 
 double evaluate_impl(svsdf_ctx *ctx, const double *x, double *g, int n) {
-    const int N = ctx->pieceN;
+    const int N = ctx->he.N;
     if (!ctx->have_boundary || n != N + 3 * (N - 1)) {
         ctx->err = "svsdf_evaluate: boundary conditions not set or wrong n";
         ctx->last_status = SVSDF_ERR_NOT_READY;
         return NAN;
     }
     ctx->n_evaluate++;
-    // forwardT / forwardP (back_end_optimizer.hpp:353-354)
-    for (int i = 0; i < N; ++i) ctx->times[i] = host::forwardT(x[i]);
-    const double *q = x + N;
-    ctx->minco.setParameters(q, ctx->times.data());
-    double cost = ctx->minco.getEnergy();
-    ctx->minco.getEnergyPartialGradByCoeffs(ctx->partialGradByCoeffs.data());
-    ctx->minco.getEnergyPartialGradByTimes(ctx->partialGradByTimes.data());
-    const double energy_cost = cost;
-    int rc = cost_grad_raw(ctx, N, ctx->times.data(), ctx->minco.getCoeffs());
+    ctx->he.forward(x);
+    int rc = cost_grad_raw(ctx, N, ctx->he.times.data(), ctx->he.minco.getCoeffs());
     if (rc) {
         ctx->last_status = rc;
         return NAN;
     }
-    const double *o = ctx->h_out;
-    cost += o[0];
-    for (int e = 0; e < 18 * N; ++e) ctx->partialGradByCoeffs[e] += o[1 + e];
-    for (int i = 0; i < N; ++i) ctx->partialGradByTimes[i] += o[1 + 18 * N + i];
-    const double pos_cost = cost - energy_cost;
-    ctx->minco.propogateGrad(ctx->partialGradByCoeffs.data(), ctx->partialGradByTimes.data(),
-                             ctx->gradByPoints.data(), ctx->gradByTimes.data());
-    double tsum = 0.0;
-    for (int i = 0; i < N; ++i) tsum += ctx->times[i];
-    cost += ctx->rho * tsum;
-    for (int i = 0; i < N; ++i) ctx->gradByTimes[i] += ctx->rho;
-    ctx->cost_pos = pos_cost;
-    ctx->cost_other = cost - pos_cost;
+    const double cost = ctx->he.backward(ctx->h_out, x, ctx->rho, g, &ctx->cost_pos, &ctx->cost_other);
     ctx->cost_total = cost;
-    for (int i = 0; i < N; ++i) g[i] = host::backwardGradT(x[i], ctx->gradByTimes[i]);
-    for (int i = 0; i < 3 * (N - 1); ++i) g[N + i] = ctx->gradByPoints[i];
     ctx->last_status = SVSDF_OK;
     return cost;
+}
+
+// ---- n problems per set of launches (svsdf_cost_grad_multi, svsdf_optimize_lockstep) -------------------------------------------
+struct MultiItem {
+    int N = 0;
+    const double *T = nullptr, *coeffs = nullptr;
+    const double *pts = nullptr;  // P rows of `stride` doubles, x and y first
+    int64_t P = 0;
+    int stride = 2;
+    double *out = nullptr;        // host record [cost, gradC (18N), gradT (N), n_inside]
+    int rc = SVSDF_OK;
+};
+
+// Resident CTAs per SM of the SINGLE-problem k_outer for this trajectory size: problem k's virtual grid is the grid svsdf_cost_grad
+// would launch for it.
+int single_outer_occupancy(svsdf_ctx *ctx, int N, int blob, int *occ) {
+    const int sc = ctx->scaled ? 1 : 0;
+    const auto key = std::make_tuple(N, blob, sc);
+    auto it = ctx->occ_cache.find(key);
+    if (it != ctx->occ_cache.end()) { *occ = it->second; return SVSDF_OK; }
+    int oo = 0, og = 0;
+    cudaError_t e;
+    if (sc) e = ctx->strict ? strict_scaled::query_occupancy(ctx->shape, N, blob, &oo, &og) : fast_scaled::query_occupancy(ctx->shape, N, blob, &oo, &og);
+    else e = ctx->strict ? strict::query_occupancy(ctx->shape, N, blob, &oo, &og) : fast::query_occupancy(ctx->shape, N, blob, &oo, &og);
+    CK(e);
+    *occ = oo > 0 ? oo : 1;
+    ctx->occ_cache[key] = *occ;
+    return SVSDF_OK;
+}
+
+size_t align16(size_t b) { return (b + 15) & ~(size_t)15; }
+
+// Sizes a grow-only device buffer.
+template <class T>
+int grow_device(svsdf_ctx *ctx, T *&p, size_t &cap, size_t bytes) {
+    if (bytes <= cap) return SVSDF_OK;
+    cudaFree(p);
+    p = nullptr;
+    cap = 0;
+    const size_t c = bytes + bytes / 4 + 4096;
+    CK(cudaMalloc(&p, c));
+    cap = c;
+    return SVSDF_OK;
+}
+
+// One cost + gradient evaluation of every item with rc == SVSDF_OK, in one set of launches.  Items whose trajectory or points are
+// invalid get rc = SVSDF_ERR_INVALID and take no part; a CUDA error fails the call (and every item).  *ms: device time of the launches.
+int run_multi(svsdf_ctx *ctx, MultiItem *items, int n, float *ms) {
+    if (ms) *ms = 0.0f;
+    CK(cudaSetDevice(ctx->device));
+    std::vector<MultiProblem> pr;
+    std::vector<int> who, map_s, map_b;
+    std::vector<BlobLayout> lay;
+    std::vector<double> dur;
+    int64_t blob_tot = 0, pt_tot = 0, flag_tot = 0, part_tot = 0, out_tot = 0;
+    int max_K1 = 1, max_N = 1, max_blob = 2;
+    int smax_blob[2] = {0, 0}, smax_N[2] = {1, 1};  // per k_outer_multi launch (sparse, batched): the shared memory is sized by its largest
+    for (int k = 0; k < n; ++k) {
+        MultiItem &it = items[k];
+        if (it.rc != SVSDF_OK) continue;
+        BlobLayout L;
+        double D = 0.0;
+        const char *msg = nullptr;
+        if (it.P < 0 || it.P > 2000000000LL || it.stride < 2 || (it.P > 0 && !it.pts) || !it.out ||
+            traj_layout(it.N, it.T, it.coeffs, L, D, &msg) != SVSDF_OK) {
+            it.rc = SVSDF_ERR_INVALID;
+            continue;
+        }
+        int occ = 1;
+        int rc = single_outer_occupancy(ctx, it.N, L.total, &occ);
+        if (rc) return rc;
+        // grid_for with that occupancy, and the single call's test hooks
+        int64_t need = (it.P + kWarpsPerBlock - 1) / kWarpsPerBlock, cap = (int64_t)ctx->sm_count * occ;
+        if (need < 1) need = 1;
+        int G = (int)(need < cap ? need : cap);
+        if (ctx->force_grid_outer > 0) G = ctx->force_grid_outer;
+        int batched = (it.P >= (int64_t)16 * G * kWarpsPerBlock) ? 1 : 0;
+        if (ctx->force_batched >= 0) batched = ctx->force_batched;
+        MultiProblem m;
+        m.blob_off = blob_tot; m.pt_off = pt_tot; m.flag_off = flag_tot; m.part_off = part_tot; m.out_off = out_tot;
+        m.P = it.P; m.blob_doubles = L.total; m.N = it.N; m.K1 = L.K1; m.grid = G;
+        std::vector<int> &mp = batched ? map_b : map_s;
+        for (int v = 0; v < G; ++v) { mp.push_back((int)pr.size()); mp.push_back(v); }
+        pr.push_back(m);
+        who.push_back(k);
+        lay.push_back(L);
+        dur.push_back(D);
+        blob_tot += L.total;
+        pt_tot += it.P;
+        flag_tot += (it.P + 15) & ~(int64_t)15;
+        part_tot += (int64_t)G * (19 * it.N + 1);
+        out_tot += 19 * it.N + 2;
+        max_K1 = std::max(max_K1, L.K1);
+        max_N = std::max(max_N, it.N);
+        max_blob = std::max(max_blob, L.total);
+        smax_blob[batched] = std::max(smax_blob[batched], L.total);
+        smax_N[batched] = std::max(smax_N[batched], it.N);
+    }
+    const int m = (int)pr.size();
+    if (m == 0) return SVSDF_OK;
+    for (int b = 0; b < 2; ++b)
+        if (outer_smem_doubles(smax_blob[b], smax_N[b]) * sizeof(double) > 200 * 1024) {
+            ctx->err = "svsdf: trajectory blob does not fit in shared memory";
+            return SVSDF_ERR_INVALID;
+        }
+    // packed inputs: problem table | CTA maps (sparse, batched) | blobs | points (x, y)
+    const size_t o_prob = 0, o_ms = align16(o_prob + m * sizeof(MultiProblem)), o_mb = align16(o_ms + map_s.size() * sizeof(int)),
+                 o_blob = align16(o_mb + map_b.size() * sizeof(int)), o_pts = align16(o_blob + (size_t)blob_tot * 8),
+                 in_bytes = align16(o_pts + (size_t)pt_tot * 16);
+    if (in_bytes > ctx->cap_multi_in) {
+        if (ctx->h_multi_in) cudaFreeHost(ctx->h_multi_in);
+        cudaFree(ctx->d_multi_in);
+        ctx->h_multi_in = nullptr; ctx->d_multi_in = nullptr; ctx->cap_multi_in = 0;
+        const size_t c = in_bytes + in_bytes / 4 + 4096;
+        CK(cudaMallocHost(&ctx->h_multi_in, c));
+        CK(cudaMalloc(&ctx->d_multi_in, c));
+        ctx->cap_multi_in = c;
+    }
+    // the previous call's copy has completed (every call ends with a stream synchronise)
+    unsigned char *h = ctx->h_multi_in, *d = ctx->d_multi_in;
+    std::memcpy(h + o_prob, pr.data(), m * sizeof(MultiProblem));
+    if (!map_s.empty()) std::memcpy(h + o_ms, map_s.data(), map_s.size() * sizeof(int));
+    if (!map_b.empty()) std::memcpy(h + o_mb, map_b.data(), map_b.size() * sizeof(int));
+    for (int j = 0; j < m; ++j) {
+        const MultiItem &it = items[who[j]];
+        fill_blob(reinterpret_cast<double *>(h + o_blob) + pr[j].blob_off, lay[j], it.T, it.coeffs, dur[j]);
+        double *xy = reinterpret_cast<double *>(h + o_pts) + 2 * pr[j].pt_off;
+        if (it.stride == 2) {
+            if (it.P) std::memcpy(xy, it.pts, (size_t)it.P * 16);
+        } else {
+            for (int64_t i = 0; i < it.P; ++i) { xy[2 * i] = it.pts[i * it.stride]; xy[2 * i + 1] = it.pts[i * it.stride + 1]; }
+        }
+    }
+    // scratch: flags | inside t* | inside lists | contributions | pieces | partials | out | tot | counts | slot offsets
+    const size_t s_flag = 0, s_ts = align16(s_flag + (size_t)flag_tot + 16), s_list = align16(s_ts + (size_t)pt_tot * 8),
+                 s_con = align16(s_list + (size_t)pt_tot * 4), s_pc = align16(s_con + (size_t)pt_tot * 160),
+                 s_part = align16(s_pc + (size_t)pt_tot * 4), s_out = align16(s_part + (size_t)part_tot * 8),
+                 s_tot = align16(s_out + (size_t)out_tot * 8), s_cnt = align16(s_tot + (size_t)out_tot * 8), s_off = align16(s_cnt + (size_t)m * 4),
+                 s_bytes = align16(s_off + (size_t)(m + 1) * 4);
+    int rc = grow_device(ctx, ctx->d_multi_scratch, ctx->cap_multi_scratch, s_bytes);
+    if (rc) return rc;
+    if (m + 1 > ctx->cap_multi_tickets) {
+        cudaFree(ctx->d_multi_tickets);
+        ctx->d_multi_tickets = nullptr;
+        ctx->cap_multi_tickets = 0;
+        const int c = m + 1 + 1024;
+        CK(cudaMalloc(&ctx->d_multi_tickets, (size_t)c * sizeof(unsigned int)));
+        CK(cudaMemsetAsync(ctx->d_multi_tickets, 0, (size_t)c * sizeof(unsigned int), ctx->stream));
+        ctx->cap_multi_tickets = c;
+    }
+    if ((size_t)out_tot * 8 > ctx->cap_multi_out) {
+        if (ctx->h_multi_out) cudaFreeHost(ctx->h_multi_out);
+        ctx->h_multi_out = nullptr;
+        ctx->cap_multi_out = 0;
+        const size_t c = (size_t)out_tot * 8 + (size_t)out_tot * 2 + 4096;
+        CK(cudaMallocHost(&ctx->h_multi_out, c));
+        ctx->cap_multi_out = c;
+    }
+    unsigned char *sc = ctx->d_multi_scratch;
+    KernelArgs A;
+    std::memset(&A, 0, sizeof(A));
+    A.blob = reinterpret_cast<const double *>(d + o_blob);
+    A.points_xy = reinterpret_cast<const double *>(d + o_pts);
+    A.cp = ctx->cp;
+    A.partials = reinterpret_cast<double *>(sc + s_part);
+    A.want_reduce = 1;
+    A.want_gsip = 1;
+    A.inside_flag = sc + s_flag;
+    A.inside_tstar = reinterpret_cast<double *>(sc + s_ts);
+    A.inside_list = reinterpret_cast<int *>(sc + s_list);
+    A.gsip_contrib = reinterpret_cast<double *>(sc + s_con);
+    A.gsip_piece = reinterpret_cast<int *>(sc + s_pc);
+    A.eval_counter = ctx->count_evals ? ctx->d_eval_counter : nullptr;
+    MultiArgs M;
+    std::memset(&M, 0, sizeof(M));
+    M.n = m;
+    M.prob = reinterpret_cast<const MultiProblem *>(d + o_prob);
+    M.ins_count = reinterpret_cast<int *>(sc + s_cnt);
+    M.ins_off = reinterpret_cast<int *>(sc + s_off);
+    M.compact_ticket = ctx->d_multi_tickets;
+    M.tickets = ctx->d_multi_tickets + 1;
+    M.out = reinterpret_cast<double *>(sc + s_out);
+    M.tot = reinterpret_cast<double *>(sc + s_tot);
+    const ScaleSched *Z = ctx->scaled ? &ctx->sched : nullptr;
+    auto launch = [&](int what, int grid, size_t smem, int wide) -> cudaError_t {
+        if (ctx->scaled)
+            return ctx->strict ? strict_multi_scaled::launch_multi(what, A, M, ctx->shape, Z, grid, smem, wide, ctx->sm_count, ctx->stream)
+                               : fast_multi_scaled::launch_multi(what, A, M, ctx->shape, Z, grid, smem, wide, ctx->sm_count, ctx->stream);
+        return ctx->strict ? strict_multi::launch_multi(what, A, M, ctx->shape, Z, grid, smem, wide, ctx->sm_count, ctx->stream)
+                           : fast_multi::launch_multi(what, A, M, ctx->shape, Z, grid, smem, wide, ctx->sm_count, ctx->stream);
+    };
+    CK(cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, ctx->stream));
+    if (ms) CK(cudaEventRecord(ctx->ev0, ctx->stream));
+    double *d_blobs = reinterpret_cast<double *>(d + o_blob);
+    CK(ctx->strict ? strict_multi::launch_pose_multi(d_blobs, M, max_K1, ctx->stream) : fast_multi::launch_pose_multi(d_blobs, M, max_K1, ctx->stream));
+    int launches = 1;
+    for (int b = 0; b < 2; ++b) {
+        const std::vector<int> &mp = b ? map_b : map_s;
+        if (mp.empty()) continue;
+        M.cta_map = reinterpret_cast<const int *>(d + (b ? o_mb : o_ms));
+        CK(launch(b, (int)(mp.size() / 2), outer_smem_doubles(smax_blob[b], smax_N[b]) * sizeof(double), 0));
+        ++launches;
+    }
+    M.cta_map = nullptr;
+    CK(ctx->strict ? strict_multi::launch_compact_multi(A.inside_flag, A.inside_list, M, ctx->stream)
+                   : fast_multi::launch_compact_multi(A.inside_flag, A.inside_list, M, ctx->stream));
+    // few inside points in the previous round: 22-warp CTAs (the variant does not change the bits, tests/test_gpu_gsip.py)
+    int wide = (ctx->multi_last_inside >= 0 && ctx->multi_last_inside <= ctx->sm_count) ? 1 : 0;
+    if (ctx->force_gsip_wide >= 0) wide = ctx->force_gsip_wide ? 1 : 0;
+    CK(launch(2, ctx->force_grid_gsip > 0 ? ctx->force_grid_gsip : 0, (size_t)max_blob * sizeof(double), wide));
+    CK(ctx->strict ? strict_multi::launch_finalize_multi(A.partials, A.gsip_contrib, A.gsip_piece, M, max_N, ctx->stream)
+                   : fast_multi::launch_finalize_multi(A.partials, A.gsip_contrib, A.gsip_piece, M, max_N, ctx->stream));
+    launches += 3;
+    if (ms) CK(cudaEventRecord(ctx->ev1, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->h_multi_out, M.out, (size_t)out_tot * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    ctx->launches += launches;
+    if (ms) CK(cudaEventElapsedTime(ms, ctx->ev0, ctx->ev1));
+    int64_t inside = 0;
+    for (int j = 0; j < m; ++j) {
+        const int nout = 19 * pr[j].N + 2;
+        const double *o = ctx->h_multi_out + pr[j].out_off;
+        std::memcpy(items[who[j]].out, o, (size_t)nout * sizeof(double));
+        inside += (int64_t)o[nout - 1];
+    }
+    ctx->multi_last_inside = inside;
+    return SVSDF_OK;
 }
 
 }  // namespace
@@ -1329,6 +1616,9 @@ void svsdf_destroy(svsdf_ctx *ctx) {
     if (ctx->h_out) cudaFreeHost(ctx->h_out);
     if (ctx->h_stage) cudaFreeHost(ctx->h_stage);
     if (ctx->h_pts_stage) cudaFreeHost(ctx->h_pts_stage);
+    if (ctx->h_multi_in) cudaFreeHost(ctx->h_multi_in);
+    if (ctx->h_multi_out) cudaFreeHost(ctx->h_multi_out);
+    cudaFree(ctx->d_multi_in); cudaFree(ctx->d_multi_scratch); cudaFree(ctx->d_multi_tickets);
     if (ctx->ev_pts) cudaEventDestroy(ctx->ev_pts);
     if (ctx->lmbm) svsdf_lmbm_close(ctx->lmbm);
     if (ctx->ev0) cudaEventDestroy(ctx->ev0);
@@ -1583,13 +1873,7 @@ int svsdf_cost_grad_device(svsdf_ctx *ctx, int N, const double *T, const double 
 
 int svsdf_set_boundary(svsdf_ctx *ctx, const double *initS, const double *finalS, int N) {
     if (!ctx || !initS || !finalS || N < 2 || N > kMaxPieces) return SVSDF_ERR_INVALID;
-    ctx->pieceN = N;
-    ctx->minco.setConditions(initS, finalS, N);
-    ctx->times.assign(N, 0.0);
-    ctx->gradByTimes.assign(N, 0.0);
-    ctx->partialGradByTimes.assign(N, 0.0);
-    ctx->partialGradByCoeffs.assign((size_t)18 * N, 0.0);
-    ctx->gradByPoints.assign((size_t)3 * (N - 1), 0.0);
+    ctx->he.setup(initS, finalS, N);
     ctx->have_boundary = true;
     return SVSDF_OK;
 }
@@ -1609,8 +1893,8 @@ int svsdf_last_costs(const svsdf_ctx *ctx, double *out3) {
 
 int svsdf_get_traj(const svsdf_ctx *ctx, double *T_out, double *coeffs_out) {
     if (!ctx || !ctx->have_boundary) return SVSDF_ERR_NOT_READY;
-    if (T_out) std::memcpy(T_out, ctx->times.data(), sizeof(double) * ctx->pieceN);
-    if (coeffs_out) std::memcpy(coeffs_out, ctx->minco.getCoeffs(), sizeof(double) * 18 * ctx->pieceN);
+    if (T_out) std::memcpy(T_out, ctx->he.times.data(), sizeof(double) * ctx->he.N);
+    if (coeffs_out) std::memcpy(coeffs_out, ctx->he.minco.getCoeffs(), sizeof(double) * 18 * ctx->he.N);
     return SVSDF_OK;
 }
 
@@ -1683,10 +1967,10 @@ int svsdf_optimize(svsdf_ctx *ctx, const double *initS, const double *finalS, do
     ctx->time_kernels = false;
     // final trajectory from the returned iterate (optimize_traj_lmbm does the same on success and failure,
     // back_end_optimizer.cpp:44-94)
-    for (int i = 0; i < N; ++i) ctx->times[i] = host::forwardT(opt_x[i]);
-    ctx->minco.setParameters(opt_x + N, ctx->times.data());
-    if (T_out) std::memcpy(T_out, ctx->times.data(), sizeof(double) * N);
-    if (coeffs_out) std::memcpy(coeffs_out, ctx->minco.getCoeffs(), sizeof(double) * 18 * N);
+    for (int i = 0; i < N; ++i) ctx->he.times[i] = host::forwardT(opt_x[i]);
+    ctx->he.minco.setParameters(opt_x + N, ctx->he.times.data());
+    if (T_out) std::memcpy(T_out, ctx->he.times.data(), sizeof(double) * N);
+    if (coeffs_out) std::memcpy(coeffs_out, ctx->he.minco.getCoeffs(), sizeof(double) * 18 * N);
     if (stats) {
         stats->final_cost = R.f;
         stats->iterations = R.iterations;
@@ -1742,6 +2026,212 @@ int svsdf_cost_grad_batch(svsdf_ctx *const *ctxs, int n_ctx, int n_problems, int
         return svsdf_cost_grad(ctx, N, T + (size_t)k * N, coeffs + (size_t)k * 18 * N, cost_io + k, gradT_io + (size_t)k * N,
                                gradC_io + (size_t)k * 18 * N);
     });
+}
+
+int svsdf_cost_grad_multi(svsdf_ctx *ctx, int n, const svsdf_multi_problem *problems) {
+    if (!ctx) return SVSDF_ERR_INVALID;
+    if (n < 0 || n > kMaxMultiProblems || (n > 0 && !problems)) {
+        ctx->err = "svsdf_cost_grad_multi: needs 0 <= n <= 65535 and the problem array";
+        return SVSDF_ERR_INVALID;
+    }
+    std::vector<MultiItem> items(n);
+    std::vector<std::vector<double>> outs(n);
+    for (int k = 0; k < n; ++k) {
+        const svsdf_multi_problem &p = problems[k];
+        BlobLayout L;
+        double D;
+        const char *msg = "svsdf_cost_grad_multi: invalid points or null outputs";
+        if (!p.cost_io || !p.gradT_io || !p.gradC_io || p.P < 0 || p.P > 2000000000LL || p.stride < 2 || (p.P > 0 && !p.points) ||
+            traj_layout(p.N, p.T, p.coeffs, L, D, &msg) != SVSDF_OK) {
+            ctx->err = std::string("problem ") + std::to_string(k) + ": " + msg;
+            return SVSDF_ERR_INVALID;
+        }
+        outs[k].assign((size_t)19 * p.N + 2, 0.0);
+        MultiItem &it = items[k];
+        it.N = p.N; it.T = p.T; it.coeffs = p.coeffs; it.pts = p.points; it.P = p.P; it.stride = p.stride; it.out = outs[k].data();
+    }
+    if (n == 0) return SVSDF_OK;
+    int rc = run_multi(ctx, items.data(), n, nullptr);
+    if (rc) return rc;
+    for (int k = 0; k < n; ++k)
+        if (items[k].rc != SVSDF_OK) {  // cannot happen after the checks above; never hand back a record that was not computed
+            ctx->err = std::string("svsdf_cost_grad_multi: problem ") + std::to_string(k) + " was refused";
+            return items[k].rc;
+        }
+    bool finite = true;
+    for (int k = 0; k < n; ++k) {
+        const svsdf_multi_problem &p = problems[k];
+        const double *o = outs[k].data();
+        const int N = p.N;
+        *p.cost_io += o[0];
+        for (int e = 0; e < 18 * N; ++e) p.gradC_io[e] += o[1 + e];
+        for (int i = 0; i < N; ++i) p.gradT_io[i] += o[1 + 18 * N + i];
+        if (p.n_inside_out) *p.n_inside_out = (int64_t)o[1 + 19 * N];
+        finite = finite && std::isfinite(o[0]);
+    }
+    return finite ? SVSDF_OK : SVSDF_ERR_NONFINITE;
+}
+
+namespace {
+// One problem in flight of svsdf_optimize_lockstep: its thread, solver and host evaluation state.
+struct LockstepSlot {
+    svsdf_ctx *ctx = nullptr;
+    host::Rendezvous *rv = nullptr;
+    std::function<void(const std::vector<int> &)> *fire = nullptr;
+    int index = 0;
+    const svsdf_lockstep_problem *pr = nullptr;
+    HostEval he;
+    MultiItem item;
+    std::vector<double> out;
+    int last_status = SVSDF_OK;
+    int evals = 0;
+    double gpu_ms = 0.0;
+};
+
+static double lockstep_evaluate(void *inst, const double *x, double *g, const int n) {
+    LockstepSlot &s = *static_cast<LockstepSlot *>(inst);
+    const int N = s.he.N;
+    if (n != N + 3 * (N - 1)) {
+        s.last_status = SVSDF_ERR_NOT_READY;
+        return NAN;
+    }
+    s.he.forward(x);
+    s.item.T = s.he.times.data();
+    s.item.coeffs = s.he.minco.getCoeffs();
+    s.item.rc = SVSDF_OK;
+    s.rv->arrive(s.index, *s.fire);
+    if (s.item.rc != SVSDF_OK) {
+        s.last_status = s.item.rc;
+        return NAN;
+    }
+    double pos = 0.0, other = 0.0;
+    const double cost = s.he.backward(s.out.data(), x, s.ctx->rho, g, &pos, &other);
+    if (s.evals++ == 0 && s.pr->f0_out) *s.pr->f0_out = cost;
+    s.last_status = SVSDF_OK;
+    return cost;
+}
+}  // namespace
+
+int svsdf_optimize_lockstep(svsdf_ctx *ctx, const svsdf_lockstep_problem *problems, int n, const svsdf_lbfgs_params *params, int max_in_flight,
+                            svsdf_opt_stats *stats_out, int *status_out) {
+    if (!ctx) return SVSDF_ERR_INVALID;
+    if (ctx->lmbm) {
+        ctx->err = "svsdf_optimize_lockstep: runs the built-in L-BFGS only; this context has an LMBM library set";
+        return SVSDF_ERR_INVALID;
+    }
+    if (n < 0 || (n > 0 && !problems)) {
+        ctx->err = "svsdf_optimize_lockstep: needs n >= 0 and the problem array";
+        return SVSDF_ERR_INVALID;
+    }
+    for (int k = 0; k < n; ++k) {  // svsdf_optimize's checks, and valid query points
+        const svsdf_lockstep_problem &p = problems[k];
+        if (!p.initS || !p.finalS || !p.opt_x || p.N < 2 || p.N > kMaxPieces || p.P < 0 || p.P > 2000000000LL || p.stride < 2 ||
+            (p.P > 0 && !p.points)) {
+            ctx->err = std::string("svsdf_optimize_lockstep: problem ") + std::to_string(k) +
+                       ": needs initS, finalS, opt_x, 2 <= N <= 64, P >= 0, stride >= 2 and points when P > 0";
+            return SVSDF_ERR_INVALID;
+        }
+    }
+    ctx->lockstep_rounds = 0;
+    if (n == 0) return SVSDF_OK;
+    CK(cudaSetDevice(ctx->device));
+    const host::LbfgsParams hp = to_host_params(params);
+    const int M = std::min(n, max_in_flight > 0 ? max_in_flight : 1024);
+    if (M > kMaxMultiProblems) {
+        ctx->err = "svsdf_optimize_lockstep: max_in_flight above 65535";
+        return SVSDF_ERR_INVALID;
+    }
+    std::vector<LockstepSlot> slots(M);
+    host::Rendezvous rv(M);
+    int round_err = SVSDF_OK;
+    // the round: every waiting slot's trajectory and points through one multi evaluation
+    std::function<void(const std::vector<int> &)> fire = [&](const std::vector<int> &ready) {
+        std::vector<MultiItem> items;
+        items.reserve(ready.size());
+        for (int s : ready) items.push_back(slots[s].item);
+        float ms = 0.0f;
+        int rc = run_multi(ctx, items.data(), (int)items.size(), ctx->time_kernels ? &ms : nullptr);
+        for (size_t j = 0; j < ready.size(); ++j) {
+            LockstepSlot &s = slots[ready[j]];
+            s.item.rc = rc != SVSDF_OK ? rc : items[j].rc;
+            s.gpu_ms += ms;
+        }
+        if (rc != SVSDF_OK && round_err == SVSDF_OK) round_err = rc;
+    };
+    std::atomic<int> next{0};
+    auto solve = [&](LockstepSlot &s, int k) {
+        const svsdf_lockstep_problem &p = problems[k];
+        const int N = p.N, nv = N + 3 * (N - 1);
+        s.pr = &p;
+        s.he.setup(p.initS, p.finalS, N);
+        s.out.assign((size_t)19 * N + 2, 0.0);
+        s.item = MultiItem();
+        s.item.N = N; s.item.pts = p.points; s.item.P = p.P; s.item.stride = p.stride; s.item.out = s.out.data();
+        s.last_status = SVSDF_OK;
+        s.evals = 0;
+        s.gpu_ms = 0.0;
+        host::Lbfgs solver(hp);
+        const auto t0 = std::chrono::steady_clock::now();
+        const host::LbfgsResult R = solver.minimize(p.opt_x, nv, lockstep_evaluate, &s, nullptr, nullptr);
+        const auto t1 = std::chrono::steady_clock::now();
+        // final trajectory from the returned iterate, as svsdf_optimize
+        for (int i = 0; i < N; ++i) s.he.times[i] = host::forwardT(p.opt_x[i]);
+        s.he.minco.setParameters(p.opt_x + N, s.he.times.data());
+        if (p.T_out) std::memcpy(p.T_out, s.he.times.data(), sizeof(double) * N);
+        if (p.coeffs_out) std::memcpy(p.coeffs_out, s.he.minco.getCoeffs(), sizeof(double) * 18 * N);
+        if (stats_out) {
+            svsdf_opt_stats &st = stats_out[k];
+            st.final_cost = R.f; st.iterations = R.iterations; st.evaluations = R.evaluations; st.status = R.status;
+            st.seconds = std::chrono::duration<double>(t1 - t0).count();
+            st.gpu_seconds = s.gpu_ms * 1e-3;
+        }
+        int ret = R.status == 0 ? 1 : R.status;
+        if (s.last_status != SVSDF_OK) ret = s.last_status;
+        if (status_out) status_out[k] = ret;
+    };
+    // A thread takes problems from the counter until none is left (going on with the next problem keeps its place among the live
+    // problems), and departs once, at the end.
+    struct ThreadArg { LockstepSlot *s; decltype(solve) *solve; host::Rendezvous *rv; std::function<void(const std::vector<int> &)> *fire;
+                       std::atomic<int> *next; int n; };
+    std::vector<ThreadArg> args(M);
+    auto body = [](void *a) -> void * {
+        ThreadArg &t = *static_cast<ThreadArg *>(a);
+        for (int k = t.next->fetch_add(1); k < t.n; k = t.next->fetch_add(1)) (*t.solve)(*t.s, k);
+        t.rv->depart(*t.fire);
+        return nullptr;
+    };
+    ctx->time_kernels = true;
+    std::vector<pthread_t> th(M);
+    pthread_attr_t attr;
+    pthread_attr_init(&attr);
+    pthread_attr_setstacksize(&attr, (size_t)1 << 20);  // the solver and MINCO keep their arrays on the heap
+    int started = 0;
+    for (int s = 0; s < M; ++s) {
+        slots[s].ctx = ctx; slots[s].rv = &rv; slots[s].fire = &fire; slots[s].index = s;
+        args[s] = ThreadArg{&slots[s], &solve, &rv, &fire, &next, n};
+    }
+    for (int s = 0; s < M; ++s) {
+        if (pthread_create(&th[s], &attr, body, &args[s]) != 0) break;
+        ++started;
+    }
+    pthread_attr_destroy(&attr);
+    if (started < M) {
+        // fewer threads than slots (the system refused more): the missing slots leave without a problem — fewer problems in flight,
+        // the same results — and with no thread at all this thread runs slot 0
+        for (int s = std::max(started, 1); s < M; ++s) rv.depart(fire);
+        if (started == 0) body(&args[0]);
+    }
+    for (int s = 0; s < started; ++s) pthread_join(th[s], nullptr);
+    ctx->time_kernels = false;
+    ctx->lockstep_rounds = rv.rounds();
+    if (round_err != SVSDF_OK) return round_err;
+    return SVSDF_OK;
+}
+
+int svsdf_lockstep_rounds(const svsdf_ctx *ctx, int64_t *rounds) {
+    if (!ctx || !rounds) return SVSDF_ERR_INVALID;
+    *rounds = ctx->lockstep_rounds;
+    return SVSDF_OK;
 }
 
 int svsdf_minco_forward(const double *initS, const double *finalS, int N, const double *q, const double *T,

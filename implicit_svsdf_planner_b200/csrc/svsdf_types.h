@@ -150,6 +150,30 @@ struct KernelArgs {
     unsigned long long *eval_counter;  // optional: executed lane-evaluations (profiling builds)
 };
 
+// svsdf_cost_grad_multi (svsdf_kernels_multi.cuh): n problems in one set of launches.  The KernelArgs of a multi launch hold the
+// BASES of the packed buffers; MultiProblem says where problem k's pieces start.  Each problem keeps the decomposition of its
+// single-problem call: its virtual grid `grid` (grid_for with the single-problem k_outer's occupancy) and its `batched` schedule.
+constexpr int kMaxMultiProblems = 65535;  // problems per multi evaluation (k_finalize_multi's grid.y)
+struct MultiProblem {
+    int64_t blob_off;    // doubles into the packed blobs (even: every blob starts 16-byte aligned, as the TMA load needs)
+    int64_t pt_off;      // points into points_xy / inside_tstar / inside_list
+    int64_t flag_off;    // bytes into inside_flag (multiple of 16: k_compact's uint4 loads)
+    int64_t part_off;    // doubles into partials ([grid][19N + 1])
+    int64_t out_off;     // doubles into out / tot ([1 + 19N + 1])
+    int64_t P;
+    int blob_doubles, N, K1, grid;
+};
+struct MultiArgs {
+    int n;                       // problems
+    const MultiProblem *prob;    // [n]
+    const int *cta_map;          // [CTAs of the launch][2]: (problem, virtual CTA) of every physical k_outer_multi CTA
+    int *ins_count;              // [n] inside points per problem (k_compact_multi)
+    int *ins_off;                // [n + 1] exclusive prefix of ins_count: problem k owns inside slots [ins_off[k], ins_off[k + 1])
+    unsigned int *compact_ticket;  // k_compact_multi's last-CTA counter (zero between calls)
+    unsigned int *tickets;       // [n] k_finalize_multi's per-problem counters (zero between calls)
+    double *tot, *out;           // per problem at out_off
+};
+
 // K3 (svsdf_extract.cu): query-point extraction from the packed map kernel
 constexpr int kMaxWaypoints = 66;   // interior waypoints of <= 64 pieces (+ optional end points)
 constexpr int kMaxMapLayers = 64;   // z layers of a 3-D map (svsdf_set_map3d)

@@ -12,8 +12,10 @@ Host-side glue only (numpy); every arithmetic step is behind the C ABI.  The map
 oracle/k3_points.py by tests/test_oracle_k3.py, the chain itself by tests/test_gpu_plan.py on the reference's own star scene."""
 from __future__ import annotations
 
+import concurrent.futures as cf
 import dataclasses
 import math
+import time
 from typing import Optional
 
 import numpy as np
@@ -106,3 +108,99 @@ def generate_traj(ctx: "api.Context", cmap: CloudMap, start_xy, goal_xy, kernel_
 def ctx_evaluate(ctx, init_s, final_s, N, x):
     ctx.set_boundary(init_s, final_s, N)
     return ctx.evaluate(x)
+
+
+# status of svsdf_front_astar_device -> why a plan_batch problem has no path
+_ASTAR_REASON = {0: "start or goal outside the map", 2: "front end found no path", 3: "front end reached max_expansions",
+                 4: "path longer than max_path", -1: "front end internal guard"}
+
+
+def plan_batch(ctx: "api.Context", cmap: CloudMap, starts, goals, kernel_size: int = scenes.YAML["kernel_size"], kernel_yaw_num: int = 18,
+               front_end_safeh: float = 0.0, traj_parlength: float = 3.0, inittime: float = scenes.YAML["inittime"],
+               mid_cfg: Optional["api.MidConfig"] = None, lbfgs_params=None, max_path: int = 4096, max_in_flight: int = 0,
+               workers: Optional[int] = None, stats: Optional[dict] = None, back_end: bool = True) -> list:
+    """generate_traj for n start / goal pairs on one map: one device A* launch for all searches (svsdf_front_astar_device), per problem the
+    waypoints, the query points (extract_points3d, on the context) and the warm start (mid_get_ori_traj, on a thread pool: the mid end is
+    host code and ctypes releases the GIL), then ONE lock-step back end (svsdf_optimize_lockstep) for every problem whose mid end succeeded.
+    Returns one dict per problem with generate_traj's keys (except astar_rounds) and its bits, plus the query points (`points`);
+    a failed problem has ok=False and the reason (an exception of one problem's extraction or mid end fails that problem only).
+    stats (optional dict) receives the wall seconds of each stage, the back end's rounds and its kernel launches.  back_end=False stops
+    before the back end: the problems that would enter it are returned with its inputs (init_s, final_s, x0, points) instead."""
+    st = np.asarray(starts, dtype=np.float64).reshape(-1, 2)
+    go = np.asarray(goals, dtype=np.float64).reshape(-1, 2)
+    n = st.shape[0]
+    X, Y, Z = cmap.occ.shape
+    res = cmap.res
+    ctx.set_map3d(pack_map_kernel3d(cmap.occ, kernel_size), X, Y, Z, kernel_size, cmap.boundary_min, res)
+    ctx.front_init(kernel_size, kernel_yaw_num, res, front_end_safeh)
+    out: list = [None] * n
+    if n == 0:
+        return out
+    t0 = time.perf_counter()
+    paths, expansions, status, _ = ctx.front_astar_device(st, go, max_path)
+    t1 = time.perf_counter()
+    half = kernel_size * res / 3.0  # bdx / 3 (plan_manager.cpp:57-59, 165)
+    todo = []
+    for q in range(n):
+        path = paths[q]
+        if status[q] != 1 or path is None or len(path) < 3:
+            out[q] = dict(ok=False, reason=_ASTAR_REASON.get(int(status[q]), "front end found no path"), expansions=int(expansions[q]),
+                          astar_status=int(status[q]))
+            continue
+        idx, wps = waypoints_of_path(path, traj_parlength, res)
+        try:
+            n_points = ctx.extract_points3d(wps, [half, half, half])
+            pts = ctx.get_points()
+        except api.SvsdfError as e:
+            out[q] = dict(ok=False, reason=f"query points failed ({e})", N=len(wps) + 1, expansions=int(expansions[q]))
+            continue
+        init_s, final_s = np.zeros((3, 3)), np.zeros((3, 3))
+        init_s[:, 0], final_s[:, 0] = path[0], path[-1]  # plan_manager.cpp:143-147
+        todo.append(dict(q=q, path=path, wps=wps, N=len(wps) + 1, n_points=int(n_points), points=pts, init_s=init_s,
+                         final_s=final_s))
+
+    def mid(p):
+        N = p["N"]
+        rots = np.stack([rot_z(w[2]) for w in p["wps"]])
+        try:
+            return api.mid_get_ori_traj(p["init_s"], p["final_s"], p["wps"].T, np.full(N, inittime), rots, mid_cfg)
+        except api.SvsdfError as e:  # generate_traj lets this propagate; here it fails the one problem
+            return e
+
+    t2 = time.perf_counter()
+    with cf.ThreadPoolExecutor(max_workers=workers) as ex:
+        mids = list(ex.map(mid, todo))
+    t3 = time.perf_counter()
+    back = []
+    for p, m in zip(todo, mids):
+        q = p["q"]
+        if isinstance(m, Exception):
+            out[q] = dict(ok=False, reason=f"mid end failed ({m})", N=p["N"], n_points=p["n_points"])
+            continue
+        rc_mid, opt_x, T_mid, co_mid, cost_mid, it_mid = m
+        if rc_mid < 0:
+            out[q] = dict(ok=False, reason=f"mid end failed ({rc_mid})", N=p["N"], n_points=p["n_points"])
+            continue
+        p["mid"] = dict(status=int(rc_mid), cost=float(cost_mid), iterations=int(it_mid), T=T_mid)
+        p["x0"] = opt_x
+        back.append(p)
+    if not back_end:
+        for p in back:
+            out[p["q"]] = dict(ok=True, N=p["N"], n_points=p["n_points"], path=p["path"], waypoints=p["wps"], expansions=int(expansions[p["q"]]),
+                               mid=p["mid"], points=p["points"], init_s=p["init_s"], final_s=p["final_s"], x0=p["x0"])
+        back = []
+    params = lbfgs_params or api.default_lbfgs_params(mem_size=16, past=3, delta=1e-6, g_epsilon=0.0, max_iterations=0, min_step=1e-32)
+    launches0 = ctx.kernel_launches()
+    results, rounds = ctx.optimize_lockstep([dict(N=p["N"], init_s=p["init_s"], final_s=p["final_s"], x0=p["x0"], points=p["points"])
+                                             for p in back], params, max_in_flight)
+    t4 = time.perf_counter()
+    if stats is not None:
+        stats.update(front_s=t1 - t0, points_s=t2 - t1, mid_s=t3 - t2, back_s=t4 - t3, rounds=int(rounds),
+                     back_launches=ctx.kernel_launches() - launches0, back_problems=len(back))
+    for p, r in zip(back, results):
+        q = p["q"]
+        out[q] = dict(ok=r["status"] >= 0, status=r["status"], N=p["N"], n_points=p["n_points"], path=p["path"], waypoints=p["wps"],
+                      expansions=int(expansions[q]), mid=p["mid"], cost_at_warm_start=r["cost_at_start"], final_cost=float(r["final_cost"]),
+                      iterations=int(r["iterations"]), evaluations=int(r["evaluations"]), T=r["T"], coeffs=r["coeffs"], x=r["x"],
+                      seconds=float(r["seconds"]), points=p["points"])
+    return out

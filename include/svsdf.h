@@ -301,6 +301,52 @@ int svsdf_optimize_batch(svsdf_ctx *const *ctxs, int n_ctx, const svsdf_problem 
 int svsdf_cost_grad_batch(svsdf_ctx *const *ctxs, int n_ctx, int n_problems, int N, const double *const *pts, const int64_t *P,
                           int stride, const double *T, const double *coeffs, double *cost_io, double *gradT_io, double *gradC_io);
 
+/* ---- Many problems on ONE context: one set of launches per evaluation round ----------------------------------------------------
+ * svsdf_cost_grad_multi: the cost and gradient of n problems (each with its own N, T, coefficients and query points; the context's
+ * robot shape, pre-transform, penalty weights and scale schedule are shared) in one upload, one launch of each cost kernel (two k_outer
+ * launches when both point schedules occur) and one download.  Every problem gets the bits svsdf_set_points + svsdf_cost_grad give it
+ * on the same context, n_inside included: it keeps its own k_outer decomposition (the grid its single call would launch and the same
+ * sparse / batched schedule) and its own reduction order.  The dynamic shared memory of a k_outer launch is sized by its largest
+ * trajectory, so one long trajectory lowers the residency of the whole launch (speed only, not the bits).  0 <= n <= 65535; P = 0 is
+ * allowed (the cost is then 0).  An invalid problem (N outside 1..64, a bad duration, null outputs, P < 0, stride < 2, null points)
+ * refuses the whole call with SVSDF_ERR_INVALID before any work.  Returns SVSDF_ERR_NONFINITE, after accumulating every problem, when
+ * a cost is not finite. */
+typedef struct {
+    int N;
+    const double *T, *coeffs;                   /* [N] durations, [18 N] MINCO coefficients (column-major 6N x 3) */
+    const double *points;                       /* P rows of `stride` doubles (x, y first) */
+    int64_t P;
+    int stride;
+    double *cost_io, *gradT_io, *gradC_io;      /* accumulate like svsdf_cost_grad: [1], [N], [18 N] */
+    int64_t *n_inside_out;                      /* optional: interior points of the problem */
+} svsdf_multi_problem;
+int svsdf_cost_grad_multi(svsdf_ctx *ctx, int n, const svsdf_multi_problem *problems);
+
+/* svsdf_optimize_lockstep: n back ends on one context, in lock-step.  Up to max_in_flight problems (<= 0: min(n, 1024)) are in flight,
+ * each on its own host thread running the built-in L-BFGS (the solver of svsdf_optimize, unchanged); a thread that finishes takes the
+ * next problem.  Each evaluation does its host half (tau -> T, MINCO, energy; afterwards the adjoint and rho * sum(T)) on its thread and
+ * meets the others at a rendezvous: once every live problem is waiting, ONE svsdf_cost_grad_multi-style round evaluates all of them.
+ * Per problem, opt_x, T_out, coeffs_out, status_out (svsdf_optimize's return value) and stats_out (final cost, iterations,
+ * evaluations, status) equal svsdf_optimize on the same inputs bit for bit, whatever max_in_flight and the order in which problems are
+ * taken; stats seconds / gpu_seconds are the problem's wall time and the device time of the rounds it took part in.  f0_out (optional)
+ * receives the cost of the first evaluation, i.e. at the start point.  Inputs are checked like svsdf_optimize's (2 <= N <= 64, non-null
+ * initS / finalS / opt_x, P >= 0, stride >= 2, points when P > 0): one invalid problem refuses the call.  A context with an LMBM library
+ * (svsdf_set_lmbm_library) is refused with SVSDF_ERR_INVALID.  Returns SVSDF_OK, or the error of a failed round (every problem of that
+ * round then ends with it, as svsdf_optimize ends on a failed evaluation).  svsdf_lockstep_rounds: the rounds of the last call. */
+typedef struct {
+    int N;
+    const double *initS, *finalS;               /* 3x3 column-major */
+    double *opt_x;                              /* in: start, out: result; N + 3 (N - 1) entries */
+    const double *points;                       /* P rows of `stride` doubles */
+    int64_t P;
+    int stride;
+    double *T_out, *coeffs_out;                 /* optional: [N], [18 N] */
+    double *f0_out;                             /* optional: cost at the start point */
+} svsdf_lockstep_problem;
+int svsdf_optimize_lockstep(svsdf_ctx *ctx, const svsdf_lockstep_problem *problems, int n, const svsdf_lbfgs_params *params, int max_in_flight,
+                            svsdf_opt_stats *stats_out, int *status_out);
+int svsdf_lockstep_rounds(const svsdf_ctx *ctx, int64_t *rounds);
+
 /* ---- "next" row (SURVEY.md §8f rank 1): query-point construction on the device --------------------------------------
  * R8  PlannerManager::generateTraj point collection  plan_manager/src/plan_manager.cpp:156-175
  *     PCSmapManager::getPointsInAABBOutOfLastOne       map_manager/include/map_manager/PCSmap_manager.h:184-219
