@@ -95,6 +95,85 @@ class OptStats(C.Structure):
     ]
 
 
+class SweptParams(C.Structure):
+    """svsdf_swept_params (include/svsdf.h)."""
+    _fields_ = [("h", C.c_double), ("iso", C.c_double), ("has_box", C.c_int), ("box", C.c_double * 4), ("max_corners", C.c_int64),
+                ("want_field", C.c_int)]
+
+
+class SweptMesh(C.Structure):
+    """svsdf_swept_mesh (include/svsdf.h); the arrays belong to the library until svsdf_swept_free."""
+    _fields_ = [("i0", C.c_int64), ("j0", C.c_int64), ("nx", C.c_int), ("ny", C.c_int), ("n_vertices", C.c_int64),
+                ("n_segments", C.c_int64), ("n_triangles", C.c_int64), ("vertices", dp), ("segments", C.POINTER(C.c_int32)),
+                ("triangles", C.POINTER(C.c_int32)), ("field", dp), ("clipped", C.c_int), ("n_evaluated", C.c_int64)]
+
+
+class SweptContour:
+    """Result of Context.swept_contour: the level set f = iso of the swept-volume SDF on the lattice (fl(i h), fl(j h)).
+
+    i0, j0, nx, ny: the grid (corner (i0 + a, j0 + b) is field[b, a]); vertices [V, 2]; segments [S, 2] (inside on the left);
+    triangles [F, 3] (counter-clockwise fill of the inside); clipped; n_evaluated (corners of the narrow band); field [ny, nx]
+    (NaN where not evaluated) or None."""
+
+    def __init__(self, i0, j0, nx, ny, h, iso, vertices, segments, triangles, clipped, n_evaluated, field=None):
+        self.i0, self.j0, self.nx, self.ny, self.h, self.iso = int(i0), int(j0), int(nx), int(ny), float(h), float(iso)
+        self.vertices, self.segments, self.triangles = vertices, segments, triangles
+        self.clipped, self.n_evaluated, self.field = int(clipped), int(n_evaluated), field
+
+    def corners(self):
+        """(x [nx], y [ny]) of the grid lines: fl(i h), fl(j h)."""
+        return (np.arange(self.i0, self.i0 + self.nx, dtype=np.int64).astype(np.float64) * self.h,
+                np.arange(self.j0, self.j0 + self.ny, dtype=np.int64).astype(np.float64) * self.h)
+
+    def loops(self):
+        """The segments chained into polylines (vertex index arrays).  A closed loop repeats its first vertex at the end;
+        without clipping every polyline is closed."""
+        nxt = {}
+        for a, b in self.segments.tolist():
+            nxt[a] = b
+        has_pred = set(nxt.values())
+        out, seen = [], set()
+        starts = [a for a in nxt if a not in has_pred] + list(nxt)  # open chains first (clipped), then the loops
+        for s in starts:
+            if s in seen:
+                continue
+            chain = [s]
+            seen.add(s)
+            v = nxt.get(s)
+            while v is not None and v not in seen:
+                chain.append(v)
+                seen.add(v)
+                v = nxt.get(v)
+            if v == s:
+                chain.append(s)
+            out.append(np.array(chain, dtype=np.int64))
+        return out
+
+    def area(self):
+        """Signed area enclosed by the segments (shoelace; holes count negative)."""
+        if len(self.segments) == 0:
+            return 0.0
+        p, q = self.vertices[self.segments[:, 0]], self.vertices[self.segments[:, 1]]
+        return 0.5 * float(np.sum(p[:, 0] * q[:, 1] - q[:, 0] * p[:, 1]))
+
+
+def write_prism_obj(path, contour: "SweptContour", z0=0.0, z1=1.0):
+    """Writes the swept region as a closed prism to a Wavefront .obj: the fill at z0 (facing down) and z1 (facing up), and one wall
+    quad (two triangles, facing out) per segment.  Watertight when the contour is not clipped."""
+    V, S, F = contour.vertices, contour.segments, contour.triangles
+    n = len(V)
+    with open(path, "w") as fh:
+        for z in (z0, z1):
+            for x, y in V.tolist():
+                fh.write(f"v {x!r} {y!r} {float(z)!r}\n")
+        for a, b, c in F.tolist():
+            fh.write(f"f {a + 1} {c + 1} {b + 1}\n")
+            fh.write(f"f {a + n + 1} {b + n + 1} {c + n + 1}\n")
+        for a, b in S.tolist():
+            fh.write(f"f {a + 1} {b + 1} {b + n + 1}\n")
+            fh.write(f"f {a + 1} {b + n + 1} {a + n + 1}\n")
+
+
 PROGRESS_T = C.CFUNCTYPE(C.c_int, C.c_void_p, dp, C.c_int)
 EVAL_T = C.CFUNCTYPE(C.c_double, C.c_void_p, dp, dp, C.c_int)
 
@@ -111,7 +190,7 @@ EXPORTED_SYMBOLS = [
     "svsdf_lmbm_default_params", "svsdf_lmbm_open", "svsdf_lmbm_close", "svsdf_lmbm_last_error", "svsdf_lmbm_minimize", "svsdf_set_lmbm_library", "svsdf_read_obj", "svsdf_free", "svsdf_mesh_fwn_host",
     "svsdf_front_init", "svsdf_front_get_kernels", "svsdf_front_cspace", "svsdf_front_check_kernel_value", "svsdf_front_expand", "svsdf_front_astar",
     "svsdf_front_astar_device", "svsdf_set_scale", "svsdf_scale_matrix",
-    "svsdf_cost_grad_multi", "svsdf_optimize_lockstep", "svsdf_lockstep_rounds",
+    "svsdf_cost_grad_multi", "svsdf_optimize_lockstep", "svsdf_lockstep_rounds", "svsdf_swept_contour", "svsdf_swept_free",
 ]
 
 
@@ -192,6 +271,9 @@ def lib():
     L.svsdf_optimize_lockstep.argtypes = [vp, C.POINTER(LockstepProblem), C.c_int, C.POINTER(LbfgsParams), C.c_int, C.POINTER(OptStats),
                                           C.POINTER(C.c_int)]
     L.svsdf_lockstep_rounds.argtypes = [vp, C.POINTER(C.c_int64)]
+    L.svsdf_swept_contour.argtypes = [vp, C.c_int, dp, dp, C.POINTER(SweptParams), C.POINTER(SweptMesh)]
+    L.svsdf_swept_free.argtypes = [C.POINTER(SweptMesh)]
+    L.svsdf_swept_free.restype = None
     _lib = L
     return L
 
@@ -525,6 +607,30 @@ class Context:
         c = _f64(coeffs_colmajor).reshape(-1)
         self._ck(lib().svsdf_set_traj(self.h, T.shape[0], _p(T), _p(c)), "svsdf_set_traj")
 
+    def swept_contour(self, T, coeffs_colmajor, h, iso=0.0, box=None, want_field=False, max_corners=0) -> SweptContour:
+        """svsdf_swept_contour: the outline (segments) and fill (triangles) of {f <= iso} for the swept-volume SDF f of this
+        trajectory on the z = 0 plane, meshed on the GPU over the narrow band.  box: (xmin, ymin, xmax, ymax) or None (automatic,
+        never clipped)."""
+        T = _f64(T)
+        c = _f64(coeffs_colmajor).reshape(-1)
+        prm = SweptParams()
+        prm.h, prm.iso, prm.max_corners, prm.want_field = float(h), float(iso), int(max_corners), int(bool(want_field))
+        if box is not None:
+            prm.has_box = 1
+            prm.box = (C.c_double * 4)(*[float(v) for v in box])
+        m = SweptMesh()
+        L = lib()
+        self._ck(L.svsdf_swept_contour(self.h, T.shape[0], _p(T), _p(c), C.byref(prm), C.byref(m)), "svsdf_swept_contour")
+        try:
+            V, S, F = m.n_vertices, m.n_segments, m.n_triangles
+            verts = np.ctypeslib.as_array(m.vertices, shape=(V, 2)).copy() if V else np.empty((0, 2))
+            segs = np.ctypeslib.as_array(m.segments, shape=(S, 2)).copy() if S else np.empty((0, 2), dtype=np.int32)
+            tris = np.ctypeslib.as_array(m.triangles, shape=(F, 3)).copy() if F else np.empty((0, 3), dtype=np.int32)
+            field = np.ctypeslib.as_array(m.field, shape=(m.ny, m.nx)).copy() if m.field else None
+            return SweptContour(m.i0, m.j0, m.nx, m.ny, h, iso, verts, segs, tris, m.clipped, m.n_evaluated, field)
+        finally:
+            L.svsdf_swept_free(C.byref(m))
+
     def query(self, T, coeffs_colmajor, pts, outer_only=False):
         T = _f64(T)
         c = _f64(coeffs_colmajor).reshape(-1)
@@ -848,6 +954,13 @@ class SweptVolumeManager:
         if z is None:
             return np.eye(3)
         return scale_matrix(t, **z)[0]
+
+    def calculateSwept(self, h, iso=0.0):  # sw_manager.hpp:265-336, on the planner's own field (see include/svsdf.hpp)
+        """(U [n, 3], G [m, 3]): the filled swept region of the current trajectory as a flat triangle mesh at z = 0."""
+        r = self.ctx.swept_contour(self._T, self._coeffs, h, iso)
+        U = np.zeros((len(r.vertices), 3))
+        U[:, :2] = r.vertices
+        return U, r.triangles.astype(np.int32)
 
     def getonlySDF(self, pos_rel):  # Shape.hpp:266
         return self.ctx.shape_sdf(pos_rel)

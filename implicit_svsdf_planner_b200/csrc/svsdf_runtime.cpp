@@ -216,6 +216,9 @@ struct svsdf_ctx {
     int64_t multi_last_inside = -1;  // inside points of the previous multi evaluation (picks the k_gsip_multi variant)
     std::map<std::tuple<int, int, int>, int> occ_cache;  // (N, blob doubles, scaled) -> resident single-problem k_outer CTAs per SM
     int64_t lockstep_rounds = 0;  // rounds of the last svsdf_optimize_lockstep
+    // svsdf_swept_contour: grow-only device buffers (per corner, per needed corner, per CTA, outputs) and the samples' upload
+    unsigned char *d_sw_corner = nullptr, *d_sw_point = nullptr, *d_sw_small = nullptr, *d_sw_out = nullptr;
+    size_t cap_sw_corner = 0, cap_sw_point = 0, cap_sw_small = 0, cap_sw_out = 0;
 };
 
 namespace {
@@ -1619,6 +1622,7 @@ void svsdf_destroy(svsdf_ctx *ctx) {
     if (ctx->h_multi_in) cudaFreeHost(ctx->h_multi_in);
     if (ctx->h_multi_out) cudaFreeHost(ctx->h_multi_out);
     cudaFree(ctx->d_multi_in); cudaFree(ctx->d_multi_scratch); cudaFree(ctx->d_multi_tickets);
+    cudaFree(ctx->d_sw_corner); cudaFree(ctx->d_sw_point); cudaFree(ctx->d_sw_small); cudaFree(ctx->d_sw_out);
     if (ctx->ev_pts) cudaEventDestroy(ctx->ev_pts);
     if (ctx->lmbm) svsdf_lmbm_close(ctx->lmbm);
     if (ctx->ev0) cudaEventDestroy(ctx->ev0);
@@ -1834,6 +1838,238 @@ int svsdf_cost_grad(svsdf_ctx *ctx, int N, const double *T, const double *coeffs
     for (int i = 0; i < N; ++i) gradT_io[i] += o[1 + 18 * N + i];
     if (!std::isfinite(o[0])) return SVSDF_ERR_NONFINITE;
     return SVSDF_OK;
+}
+
+// ---- svsdf_swept_contour (kernels: svsdf_swept.cu; the band bound: DESIGN.md §7) ----------------------------------------------
+namespace {
+constexpr int64_t kSweptDefaultCorners = (int64_t)1 << 25;
+constexpr int64_t kSweptMaxCorners = (int64_t)1 << 28;  // vertex, segment and triangle indices stay in int32
+
+// Path samples for the band bound.  Piece i is cut into ceil(T_i / 0.15) equal parts of local time; a sample is the position at a
+// part's midpoint (the piece's own polynomial) and delta = half the part (plus a rounding allowance on the local time) times a bound
+// on |velocity| over the piece from the coefficients: |v_d| <= sum_k k |c_dk| Tmax^(k-1).  reach = (delta + s_eff rho) padded, where a
+// body-frame point beyond rho is provably > iso.  Sampling piece by piece needs no continuity between pieces.
+void swept_samples(const svsdf_ctx *ctx, int N, const double *T, const double *coeffs, double D, double rho, std::vector<double> &samp) {
+    double s_eff = 1.0;
+    if (ctx->scaled)
+        for (int d = 0; d < 2; ++d) s_eff = std::max(s_eff, ctx->sched.a[d] + std::fabs(ctx->sched.b[d]));
+    const double ext = 1e-9 * (1.0 + D);
+    samp.clear();
+    for (int i = 0; i < N; ++i) {
+        const double *cx = coeffs + 6 * i, *cy = coeffs + 6 * N + 6 * i;
+        const double tmax = T[i] * (1.0 + 1e-9) + ext;
+        double vx = 0.0, vy = 0.0, tk = 1.0;
+        for (int k = 1; k < 6; ++k) {
+            vx += k * std::fabs(cx[k]) * tk;
+            vy += k * std::fabs(cy[k]) * tk;
+            tk *= tmax;
+        }
+        const double vmax = std::sqrt(vx * vx + vy * vy);
+        const int m = std::max(1, (int)std::ceil(T[i] / 0.15));
+        const double part = T[i] / m;
+        for (int j = 0; j < m; ++j) {
+            const double tau = (j + 0.5) * part;
+            double x = 0.0, y = 0.0, tn = 1.0;
+            for (int k = 0; k < 6; ++k) {
+                x += cx[k] * tn;
+                y += cy[k] * tn;
+                tn *= tau;
+            }
+            const double delta = (0.5 * part + ext) * vmax;
+            const double reach = (delta + s_eff * rho) * (1.0 + 1e-9) + 1e-9 * (1.0 + std::fabs(x) + std::fabs(y) + s_eff * rho);
+            samp.push_back(x);
+            samp.push_back(y);
+            samp.push_back(reach);
+        }
+    }
+}
+
+// largest i with fl(i h) <= x / smallest i with fl(i h) >= x
+int64_t lattice_floor(double x, double h) {
+    int64_t i = (int64_t)std::floor(x / h);
+    while ((double)i * h > x) --i;
+    while ((double)(i + 1) * h <= x) ++i;
+    return i;
+}
+int64_t lattice_ceil(double x, double h) {
+    int64_t i = (int64_t)std::ceil(x / h);
+    while ((double)i * h < x) ++i;
+    while ((double)(i - 1) * h >= x) --i;
+    return i;
+}
+}  // namespace
+
+int svsdf_swept_contour(svsdf_ctx *ctx, int N, const double *T, const double *coeffs, const svsdf_swept_params *prm,
+                        svsdf_swept_mesh *out) {
+    if (!ctx || !prm || !out) return SVSDF_ERR_INVALID;
+    std::memset(out, 0, sizeof(*out));
+    auto invalid = [&](const char *msg) {
+        ctx->err = msg;
+        return SVSDF_ERR_INVALID;
+    };
+    const double h = prm->h, iso = prm->iso;
+    if (!(std::isfinite(h) && h > 0.0)) return invalid("svsdf_swept_contour: h must be finite and > 0");
+    if (!std::isfinite(iso)) return invalid("svsdf_swept_contour: iso must be finite");
+    const int64_t cap = prm->max_corners == 0 ? kSweptDefaultCorners : prm->max_corners;
+    if (cap < 4 || cap > kSweptMaxCorners) return invalid("svsdf_swept_contour: max_corners must be 0 or in 4 .. 2^28");
+    BlobLayout L;
+    double D = 0.0;
+    const char *msg = nullptr;
+    if (traj_layout(N, T, coeffs, L, D, &msg) != SVSDF_OK) return invalid(msg);
+    for (int64_t e = 0; e < 18 * (int64_t)N; ++e)
+        if (!std::isfinite(coeffs[e])) return invalid("svsdf_swept_contour: non-finite trajectory coefficient");
+    // rho: body-frame radius beyond which the shape functor is provably > iso (sdf >= (|q| - R) / prune_scale for |q| >= prune_rmin)
+    const ShapeParams &S = ctx->shape;
+    const bool bounded = S.rout < 1e299;
+    const double rho = bounded ? std::max(std::max(S.prune_rmin, S.rout + S.prune_scale * iso), 0.0) : INFINITY;
+    std::vector<double> samp;
+    swept_samples(ctx, N, T, coeffs, D, rho, samp);
+    const int n_samp = (int)(samp.size() / 3);
+    if (n_samp > kSweptMaxSamples) return invalid("svsdf_swept_contour: too many path samples");
+    double bx0, by0, bx1, by1;
+    if (prm->has_box) {
+        bx0 = prm->box[0]; by0 = prm->box[1]; bx1 = prm->box[2]; by1 = prm->box[3];
+        if (!(std::isfinite(bx0) && std::isfinite(by0) && std::isfinite(bx1) && std::isfinite(by1)))
+            return invalid("svsdf_swept_contour: non-finite box");
+        if (bx0 > bx1 || by0 > by1) return invalid("svsdf_swept_contour: inverted box");
+    } else {
+        if (!bounded) return invalid("svsdf_swept_contour: the shape has no far-field bound; give a box");
+        bx0 = by0 = INFINITY;
+        bx1 = by1 = -INFINITY;
+        for (int k = 0; k < n_samp; ++k) {
+            const double x = samp[3 * k], y = samp[3 * k + 1], r = samp[3 * k + 2];
+            bx0 = std::min(bx0, x - r); bx1 = std::max(bx1, x + r);
+            by0 = std::min(by0, y - r); by1 = std::max(by1, y + r);
+        }
+        // strictly beyond every reach, whatever the rounding of the subtractions above
+        const double pad = 1e-9 * (1.0 + std::max(std::max(std::fabs(bx0), std::fabs(bx1)), std::max(std::fabs(by0), std::fabs(by1))));
+        bx0 -= pad; by0 -= pad; bx1 += pad; by1 += pad;
+    }
+    const double lim = 0x1p50;
+    if (!(std::fabs(bx0) / h < lim && std::fabs(bx1) / h < lim && std::fabs(by0) / h < lim && std::fabs(by1) / h < lim))
+        return invalid("svsdf_swept_contour: box too large for the lattice of h");
+    const int64_t i0 = lattice_floor(bx0, h), j0 = lattice_floor(by0, h);
+    const int64_t i1 = std::max(lattice_ceil(bx1, h), i0 + 1), j1 = std::max(lattice_ceil(by1, h), j0 + 1);
+    const int64_t nx64 = i1 - i0 + 1, ny64 = j1 - j0 + 1;
+    if (nx64 > cap || ny64 > cap || nx64 * ny64 > cap) return invalid("svsdf_swept_contour: box has more corners than max_corners");
+    const int nx = (int)nx64, ny = (int)ny64;
+    const int64_t n = nx64 * ny64;
+    CK(cudaSetDevice(ctx->device));
+
+    SweptArgs A;
+    std::memset(&A, 0, sizeof(A));
+    A.i0 = i0; A.j0 = j0; A.nx = nx; A.ny = ny; A.h = h; A.iso = iso;
+    A.tiles_x = (nx + kSweptTile - 1) / kSweptTile;
+    A.tiles_y = (ny + kSweptTile - 1) / kSweptTile;
+    const int tiles = A.tiles_x * A.tiles_y;
+    const int nblk = (int)((n + kSweptBlock - 1) / kSweptBlock);
+    A.n_samp = n_samp;
+    // per corner: need (n bytes), field (n doubles), vertex ids (3 n ints)
+    const size_t off_field = align16((size_t)n), off_vid = off_field + align16((size_t)n * 8);
+    int rc = grow_device(ctx, ctx->d_sw_corner, ctx->cap_sw_corner, off_vid + (size_t)n * 12);
+    if (rc) return rc;
+    A.need = ctx->d_sw_corner;
+    A.field = reinterpret_cast<double *>(ctx->d_sw_corner + off_field);
+    A.vid = reinterpret_cast<int *>(ctx->d_sw_corner + off_vid);
+    // small: header [0] non-finite, [1] clipped, [2..6] channel totals, [7] needed corners; samples; tile counts; per-CTA counts
+    const size_t off_samp = 64, off_tile = off_samp + align16(samp.size() * 8), off_blk = off_tile + align16((size_t)(tiles + 1) * 4);
+    rc = grow_device(ctx, ctx->d_sw_small, ctx->cap_sw_small, off_blk + (size_t)5 * (nblk + 1) * 4);
+    if (rc) return rc;
+    int *d_hdr = reinterpret_cast<int *>(ctx->d_sw_small);
+    A.status = d_hdr;
+    A.samp = reinterpret_cast<double *>(ctx->d_sw_small + off_samp);
+    A.tile_off = reinterpret_cast<int *>(ctx->d_sw_small + off_tile);
+    A.blk = reinterpret_cast<int *>(ctx->d_sw_small + off_blk);
+    rc = ensure_stage(ctx, std::max<size_t>(64 + samp.size() * 8, 64));
+    if (rc) return rc;
+    std::memset(ctx->h_stage, 0, 64);
+    std::memcpy(reinterpret_cast<unsigned char *>(ctx->h_stage) + 64, samp.data(), samp.size() * 8);
+    CK(cudaMemcpyAsync(ctx->d_sw_small, ctx->h_stage, 64 + samp.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
+    cudaStream_t st = ctx->stream;
+    // classify the tiles and their corners, count and compact the needed corners
+    CK(launch_swept(0, A, st));
+    CK(launch_swept_scan(A.tile_off, tiles, 1, d_hdr + 7, st));
+    int hdr[8];
+    CK(cudaMemcpyAsync(ctx->h_stage, d_hdr, sizeof(hdr), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    std::memcpy(hdr, ctx->h_stage, sizeof(hdr));
+    const int64_t P = hdr[7];
+    ctx->launches += 2;
+    rc = grow_device(ctx, ctx->d_sw_point, ctx->cap_sw_point, (size_t)std::max<int64_t>(P, 1) * 28 + 32);
+    if (rc) return rc;
+    A.P = P;
+    A.pts = reinterpret_cast<double *>(ctx->d_sw_point);
+    A.val = reinterpret_cast<double *>(ctx->d_sw_point + (size_t)std::max<int64_t>(P, 1) * 16);
+    A.idx = reinterpret_cast<int *>(ctx->d_sw_point + (size_t)std::max<int64_t>(P, 1) * 24);
+    if (P > 0) {
+        // the outer solve of svsdf_query (outer_only = 1) on the mesher's own points: the same kernels, so the same bits per point
+        CK(launch_swept(1, A, st));
+        rc = upload_traj(ctx, N, T, coeffs);
+        if (rc) return rc;
+        rc = run_kernels(ctx, A.pts, P, false, false, const_cast<double *>(A.val), nullptr, nullptr, nullptr);
+        if (rc) return rc;
+        CK(launch_swept(2, A, st));
+        ctx->launches += 2;
+    }
+    // marching squares: counts, their prefix, then vertices, segments and triangles
+    CK(launch_swept(3, A, st));
+    CK(launch_swept_scan(A.blk, nblk, 5, d_hdr + 2, st));
+    CK(cudaMemcpyAsync(ctx->h_stage, d_hdr, sizeof(hdr), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    std::memcpy(hdr, ctx->h_stage, sizeof(hdr));
+    ctx->launches += 2;
+    if (hdr[0]) {
+        ctx->err = "svsdf_swept_contour: non-finite field value";
+        return SVSDF_ERR_NONFINITE;
+    }
+    const int64_t V = (int64_t)hdr[2] + hdr[3] + hdr[4], Sg = hdr[5], F = hdr[6];
+    const size_t b_verts = (size_t)V * 16, b_segs = (size_t)Sg * 8, b_tris = (size_t)F * 12;
+    const size_t o_segs = align16(b_verts), o_tris = o_segs + align16(b_segs), o_end = o_tris + align16(b_tris);
+    rc = grow_device(ctx, ctx->d_sw_out, ctx->cap_sw_out, o_end + 16);
+    if (rc) return rc;
+    A.verts = reinterpret_cast<double *>(ctx->d_sw_out);
+    A.segs = reinterpret_cast<int *>(ctx->d_sw_out + o_segs);
+    A.tris = reinterpret_cast<int *>(ctx->d_sw_out + o_tris);
+    CK(launch_swept(4, A, st));
+    CK(launch_swept(5, A, st));
+    ctx->launches += 2;
+    const size_t b_field = prm->want_field ? (size_t)n * 8 : 0;
+    rc = ensure_stage(ctx, o_end + b_field + 16);
+    if (rc) return rc;
+    unsigned char *hs = reinterpret_cast<unsigned char *>(ctx->h_stage);
+    if (o_end) CK(cudaMemcpyAsync(hs, ctx->d_sw_out, o_end, cudaMemcpyDeviceToHost, st));
+    if (b_field) CK(cudaMemcpyAsync(hs + o_end, A.field, b_field, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    out->i0 = i0; out->j0 = j0; out->nx = nx; out->ny = ny;
+    out->n_vertices = V; out->n_segments = Sg; out->n_triangles = F;
+    out->clipped = hdr[1] ? 1 : 0;
+    out->n_evaluated = P;
+    out->vertices = static_cast<double *>(std::malloc(b_verts + 16));
+    out->segments = static_cast<int32_t *>(std::malloc(b_segs + 16));
+    out->triangles = static_cast<int32_t *>(std::malloc(b_tris + 16));
+    out->field = b_field ? static_cast<double *>(std::malloc(b_field)) : nullptr;
+    if (!out->vertices || !out->segments || !out->triangles || (b_field && !out->field)) {
+        svsdf_swept_free(out);
+        ctx->err = "svsdf_swept_contour: out of host memory";
+        return SVSDF_ERR_INVALID;
+    }
+    std::memcpy(out->vertices, hs, b_verts);
+    std::memcpy(out->segments, hs + o_segs, b_segs);
+    std::memcpy(out->triangles, hs + o_tris, b_tris);
+    if (b_field) std::memcpy(out->field, hs + o_end, b_field);
+    return SVSDF_OK;
+}
+
+void svsdf_swept_free(svsdf_swept_mesh *mesh) {
+    if (!mesh) return;
+    std::free(mesh->vertices);
+    std::free(mesh->segments);
+    std::free(mesh->triangles);
+    std::free(mesh->field);
+    mesh->vertices = nullptr;
+    mesh->segments = nullptr;
+    mesh->triangles = nullptr;
+    mesh->field = nullptr;
 }
 
 int svsdf_cost_grad_device(svsdf_ctx *ctx, int N, const double *T, const double *coeffs, int repeats,

@@ -197,6 +197,31 @@ struct ExtractArgs {
     double keepout[2 * kMaxKeepout];
 };
 
+// svsdf_swept_contour (svsdf_swept.cu): the narrow-band marching-squares mesher
+constexpr int kSweptTile = 16;           // classification / compaction tile: 16 x 16 corners, one CTA of 256 threads
+constexpr int kSweptMaxSamples = 2112;   // path samples: at most ceil(T_i / 0.15) per piece, D < 300 s, N <= 64
+constexpr int kSweptBlock = 1024;        // corners per CTA of the marching-squares passes (256 threads x 4)
+struct SweptArgs {
+    int64_t i0, j0;
+    int nx, ny;
+    int tiles_x, tiles_y;
+    double h, iso;
+    int n_samp;
+    const double *samp;        // [n_samp][3]: sample x, y and its reach (a corner farther than reach from every sample is > iso)
+    unsigned char *need;       // [ny][nx] corner is evaluated
+    double *field;             // [ny][nx]
+    int *tile_off;             // [tiles + 1] needed corners per tile, then their exclusive prefix (k_sw_scan)
+    double *pts;               // [P][2] needed corners (tile-major, row-major in a tile)
+    int *idx;                  // [P] their field index
+    const double *val;         // [P] their values (the evaluation's output)
+    int64_t P;
+    int *blk;                  // [5][n_blocks + 1] per-CTA counts of the marching-squares channels, then their prefix
+    int *status;               // [0] non-finite value seen, [1] clipped
+    int *vid;                  // [ny][nx][3] vertex of the horizontal edge, the vertical edge and the corner
+    double *verts;             // [V][2]
+    int *segs, *tris;          // [S][2], [F][3]
+};
+
 // K5 (svsdf_frontend.cu): collision kernels of the A* front end
 constexpr int kMaxYawKernels = 64;
 constexpr int kMaxKernelSize = 32;  // kernel rows are held as 32-bit masks

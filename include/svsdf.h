@@ -124,6 +124,60 @@ int svsdf_set_scale(svsdf_ctx *ctx, const svsdf_scale *scale);
  * Either output may be NULL.  No context and no GPU needed. */
 int svsdf_scale_matrix(const svsdf_scale *scale, double t, double S_out[9], double Sinv_out[9]);
 
+/* ---- Swept-volume outline and mesh: the planner's own field contoured on the GPU ---------------------------------------------
+ * svsdf_swept_contour meshes the level set f(p) = iso of f = getSDFofSweptVolume<false,true> (exactly what svsdf_query(...,
+ * outer_only = 1) returns, bit for bit per point) on the z = 0 plane, for the trajectory (N, T, coeffs) as svsdf_query takes it and
+ * with the context's shape, pre-transform, scale schedule and build (strict / fast).  Where the planner's local search misses the
+ * global minimum, the outline shows what the planner sees.  No interior (GSIP) branch: inside the volume the outer solve's value
+ * (negative there) is what is interpolated.
+ *   Grid: corner (i, j) sits at (fl(i h), fl(j h)) (i, j int64, one rounded product, no origin), so grids of different boxes line up.
+ *     The box is snapped outwards to this lattice; corners i0 .. i0 + nx - 1, j0 .. j0 + ny - 1; field index (j - j0) nx + (i - i0).
+ *     Automatic box (has_box = 0): the trajectory's bounding box padded by the band bound below, so that every corner outside it is
+ *     provably > iso and the result is never clipped.  Unavailable (SVSDF_ERR_INVALID) when the shape has no far-field bound
+ *     (svsdf_shape_bound_radius >= 1e300).
+ *   Inside: f <= iso (the sdf <= 0 convention of the interior flag; iso = 0 is the boundary, iso = safety_hor where the penalty starts).
+ *   Vertices: one per crossing edge (exactly one end inside), shared by the cells that own the edge; with a the edge's lower-index
+ *     corner s = (iso - f_a) / (f_b - f_a), p = p_a + s (p_b - p_a) per coordinate, every operation rounded once (no contraction), so
+ *     the strict and fast builds give the same vertices from the same field.  Inside corners are vertices too.
+ *     Order: crossings of horizontal edges (row-major), then of vertical edges, then inside corners (row-major).
+ *   Saddles (two diagonal corners inside): m = ((f00 + f10) + (f01 + f11)) * 0.25; m <= iso connects the inside corners.
+ *   Segments (2 int32 each, vertex indices) have the inside on their left: outer loops run counter-clockwise, holes clockwise.
+ *   Triangles (3 int32, counter-clockwise) fill the inside: per cell each inside polygon (inside corners and crossing vertices walked
+ *     counter-clockwise from the lower-left corner) is fan-triangulated from its first vertex.  Segments and triangles come cell by
+ *     cell (row-major), within a cell in that walk order.
+ *   clipped = 1 when an inside corner lies on the box border (only a user box can do this).  Loops are closed, and the boundary of the
+ *     fill equals the segment set, exactly when clipped = 0.
+ * Narrow band: only corners of cells that can hold the contour are evaluated (n_evaluated of the box's nx ny).  A cell is skipped only
+ * when a bound proves its four corners > iso: f(p) >= min_t |p - x(t)| / s_max - R (R = the shape's far-field radius, s_max the largest
+ * scale factor) with x(t) covered by samples x_k and radii delta_k from the velocity coefficients (DESIGN.md §7).  The field of a
+ * skipped corner is NaN.  A fixed number of kernel launches per call (none of the evaluation's when no corner is needed); the
+ * context's resident points and everything svsdf_cost_grad depends on are left as they were.
+ * Errors: SVSDF_ERR_INVALID (nothing allocated) for a non-finite h or h <= 0, a non-finite iso, a non-finite or inverted box, a box over
+ * max_corners (0: 2^25; at most 2^28), or a bad trajectory; SVSDF_ERR_NONFINITE when an evaluated corner's value is not finite.
+ * The library allocates the output arrays; release them with svsdf_swept_free. */
+typedef struct {
+    double h;              /* grid spacing (> 0) */
+    double iso;            /* level */
+    int has_box;           /* 0: automatic box */
+    double box[4];         /* xmin, ymin, xmax, ymax (has_box = 1) */
+    int64_t max_corners;   /* cap on nx * ny; 0 = 2^25 */
+    int want_field;        /* 1: return the field (nx * ny doubles, NaN where not evaluated) */
+} svsdf_swept_params;
+typedef struct {
+    int64_t i0, j0;        /* lattice index of the box's lower-left corner */
+    int nx, ny;            /* corners per row / column */
+    int64_t n_vertices, n_segments, n_triangles;
+    double *vertices;      /* n_vertices x 2 (x, y) */
+    int32_t *segments;     /* n_segments x 2 */
+    int32_t *triangles;    /* n_triangles x 3 */
+    double *field;         /* ny x nx or NULL */
+    int clipped;
+    int64_t n_evaluated;   /* corners whose field was evaluated */
+} svsdf_swept_mesh;
+int svsdf_swept_contour(svsdf_ctx *ctx, int N, const double *T, const double *coeffs, const svsdf_swept_params *params,
+                        svsdf_swept_mesh *out);
+void svsdf_swept_free(svsdf_swept_mesh *mesh);
+
 /* R2: per-point swept-volume SDF query on the trajectory given by (N, T, coeffs).
  * pts: P x 3 (x, y, z) host doubles (z ignored).  Outputs (host, may be NULL): sdf[P], tstar[P], grad3[3P]
  * (body-frame FD gradient for sdf > 0; world-frame unit direction for the interior branch, exactly what the

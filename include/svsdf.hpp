@@ -151,6 +151,26 @@ class SweptVolumeManager {
         svsdf_query(ctx_->h, N_, T_.data(), c_.data(), 1, pos_eva, &sdf, &time_seed_f, grad_prel, nullptr, 1);
         return sdf;
     }
+    // calculateSwept (:265-336) on the planner's own field: the filled region {getSDFofSweptVolume <= iso} of the current trajectory
+    // (svsdf_swept_contour, automatic box) as a flat triangle mesh at z = 0: U n x 3 vertices, G m x 3 faces (row-major, 0-based).
+    // Unlike the reference's (igl::marching_cubes over its own continuation field, mesh robots only), this is 2-D marching squares
+    // of the field the planner optimises, for every shape; the outline is svsdf_swept_contour's segments.  Returns a svsdf_status.
+    int calculateSwept(double h, double iso, std::vector<double> &U, std::vector<int32_t> &G) {
+        svsdf_swept_params p{};
+        p.h = h;
+        p.iso = iso;
+        svsdf_swept_mesh m{};
+        const int rc = svsdf_swept_contour(ctx_->h, N_, T_.data(), c_.data(), &p, &m);
+        if (rc != SVSDF_OK) return rc;
+        U.assign((size_t)m.n_vertices * 3, 0.0);
+        for (int64_t i = 0; i < m.n_vertices; ++i) {
+            U[3 * i] = m.vertices[2 * i];
+            U[3 * i + 1] = m.vertices[2 * i + 1];
+        }
+        G.assign(m.triangles, m.triangles + 3 * m.n_triangles);
+        svsdf_swept_free(&m);
+        return SVSDF_OK;
+    }
     // batched query (P rows of 3 doubles): what a caller with many points should use
     int getTrueSDFofSweptVolume(int64_t P, const double *pos_eva, double *sdf, double *tstar, double *grad3, int *rounds = nullptr) {
         return svsdf_query(ctx_->h, N_, T_.data(), c_.data(), P, pos_eva, sdf, tstar, grad3, rounds, 0);
