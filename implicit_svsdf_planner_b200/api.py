@@ -15,6 +15,8 @@ There is no CPU fallback: if the CUDA library is missing or no H100 is visible, 
 from __future__ import annotations
 
 import ctypes as C
+import dataclasses
+import math
 import os
 
 import numpy as np
@@ -157,6 +159,35 @@ class SweptContour:
         return 0.5 * float(np.sum(p[:, 0] * q[:, 1] - q[:, 0] * p[:, 1]))
 
 
+class ClearanceOut(C.Structure):
+    """svsdf_clearance (include/svsdf.h); the arrays belong to the library until svsdf_clearance_free."""
+    _fields_ = [("n_occupied", C.c_int64), ("n_evaluated", C.c_int64), ("n_within", C.c_int64), ("n_colliding", C.c_int64),
+                ("min_sdf", C.c_double), ("argmin", C.c_int64), ("ij", C.POINTER(C.c_int32)), ("xy", dp), ("sdf", dp), ("tstar", dp)]
+
+
+@dataclasses.dataclass
+class Clearance:
+    """Result of Context.map_clearance: the occupied map cells whose swept-volume SDF value is <= d_max, in map order (i * Y + j).
+
+    ij [n, 2] cell indices, xy [n, 2] cell centres, sdf [n], tstar [n]; the summary is computed from that list (min_sdf = +inf and
+    argmin = -1 when it is empty).  n_occupied: occupied columns of the map; n_evaluated: columns evaluated (the band)."""
+    d_max: float
+    ij: np.ndarray
+    xy: np.ndarray
+    sdf: np.ndarray
+    tstar: np.ndarray
+    n_occupied: int
+    n_evaluated: int
+    n_within: int
+    n_colliding: int
+    min_sdf: float
+    argmin: int
+
+    @property
+    def collision_free(self) -> bool:
+        return self.min_sdf > 0.0
+
+
 def write_prism_obj(path, contour: "SweptContour", z0=0.0, z1=1.0):
     """Writes the swept region as a closed prism to a Wavefront .obj: the fill at z0 (facing down) and z1 (facing up), and one wall
     quad (two triangles, facing out) per segment.  Watertight when the contour is not clipped."""
@@ -191,6 +222,7 @@ EXPORTED_SYMBOLS = [
     "svsdf_front_init", "svsdf_front_get_kernels", "svsdf_front_cspace", "svsdf_front_check_kernel_value", "svsdf_front_expand", "svsdf_front_astar",
     "svsdf_front_astar_device", "svsdf_set_scale", "svsdf_scale_matrix",
     "svsdf_cost_grad_multi", "svsdf_optimize_lockstep", "svsdf_lockstep_rounds", "svsdf_swept_contour", "svsdf_swept_free",
+    "svsdf_map_clearance", "svsdf_clearance_free",
 ]
 
 
@@ -274,6 +306,9 @@ def lib():
     L.svsdf_swept_contour.argtypes = [vp, C.c_int, dp, dp, C.POINTER(SweptParams), C.POINTER(SweptMesh)]
     L.svsdf_swept_free.argtypes = [C.POINTER(SweptMesh)]
     L.svsdf_swept_free.restype = None
+    L.svsdf_map_clearance.argtypes = [vp, C.c_int, dp, dp, C.c_double, C.POINTER(ClearanceOut)]
+    L.svsdf_clearance_free.argtypes = [C.POINTER(ClearanceOut)]
+    L.svsdf_clearance_free.restype = None
     _lib = L
     return L
 
@@ -560,6 +595,7 @@ class Context:
             raise SvsdfError(f"svsdf_create failed with status {rc} (no usable sm_90 (H100) CUDA device? no CPU fallback)")
         self.h = h
         self.P = 0
+        self.safety_hor = float(safety_hor)  # the penalty's horizon: plan's certification lists the cells within it
 
     def close(self):
         if getattr(self, "h", None):
@@ -630,6 +666,26 @@ class Context:
             return SweptContour(m.i0, m.j0, m.nx, m.ny, h, iso, verts, segs, tris, m.clipped, m.n_evaluated, field)
         finally:
             L.svsdf_swept_free(C.byref(m))
+
+    def map_clearance(self, T, coeffs_colmajor, d_max=math.inf) -> Clearance:
+        """svsdf_map_clearance: the swept-volume SDF (svsdf_query's value, interior depth included) of this trajectory at the centre of
+        every occupied column of the context's map, listed where it is <= d_max (>= 0 or +inf), with the summary (min_sdf, argmin,
+        n_colliding ...).  Only the columns near the path are evaluated; the result is that of evaluating all of them."""
+        T = _f64(T)
+        c = _f64(coeffs_colmajor).reshape(-1)
+        m = ClearanceOut()
+        L = lib()
+        self._ck(L.svsdf_map_clearance(self.h, T.shape[0], _p(T), _p(c), float(d_max), C.byref(m)), "svsdf_map_clearance")
+        try:
+            n = m.n_within
+            ij = np.ctypeslib.as_array(m.ij, shape=(n, 2)).copy() if n else np.empty((0, 2), dtype=np.int32)
+            xy = np.ctypeslib.as_array(m.xy, shape=(n, 2)).copy() if n else np.empty((0, 2))
+            sdf = np.ctypeslib.as_array(m.sdf, shape=(n,)).copy() if n else np.empty(0)
+            ts = np.ctypeslib.as_array(m.tstar, shape=(n,)).copy() if n else np.empty(0)
+            return Clearance(float(d_max), ij, xy, sdf, ts, int(m.n_occupied), int(m.n_evaluated), int(n), int(m.n_colliding),
+                             float(m.min_sdf), int(m.argmin))
+        finally:
+            L.svsdf_clearance_free(C.byref(m))
 
     def query(self, T, coeffs_colmajor, pts, outer_only=False):
         T = _f64(T)
@@ -961,6 +1017,11 @@ class SweptVolumeManager:
         U = np.zeros((len(r.vertices), 3))
         U[:, :2] = r.vertices
         return U, r.triangles.astype(np.int32)
+
+    def getMinSVSDF(self, d_max=math.inf):  # plan_manager.hpp:45, declared there and never defined (see include/svsdf.hpp)
+        """Minimum of the swept-volume SDF of the current trajectory over the occupied cells of the context's map with value <= d_max
+        (+inf when there is none): > 0 means the trajectory is collision free against the whole map."""
+        return self.ctx.map_clearance(self._T, self._coeffs, d_max).min_sdf
 
     def getonlySDF(self, pos_rel):  # Shape.hpp:266
         return self.ctx.shape_sdf(pos_rel)

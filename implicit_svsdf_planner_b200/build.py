@@ -37,6 +37,7 @@ UNITS = [
     ("svsdf_extract.cu", "svsdf_extract.o", ["-fmad=false"]),  # cell centres must round like the host formula
     ("svsdf_frontend.cu", "svsdf_frontend.o", ["-fmad=false"]),  # shape kernels: same rounding as the strict functors
     ("svsdf_swept.cu", "svsdf_swept.o", ["-fmad=false"]),  # swept-volume mesher: vertices independent of the field's build
+    ("svsdf_clearance.cu", "svsdf_clearance.o", ["-fmad=false"]),  # map clearance: cell centres round like svsdf_extract's
     # host threads for the batch A* bookkeeping; no a*b+c contraction in the float winding-number builder (host/fwn_bvh.hpp)
     ("svsdf_runtime.cpp", "svsdf_runtime.o", ["-Xcompiler", "-fopenmp", "-Xcompiler", "-ffp-contract=off"]),
 ]

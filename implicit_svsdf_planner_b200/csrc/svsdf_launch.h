@@ -69,6 +69,9 @@ cudaError_t launch_extract_write(const ExtractArgs &E, const int *block_offsets,
 // (row stride n + 1, the total lands at [n] and at totals[ch]) in one CTA.
 cudaError_t launch_swept(int what, const SweptArgs &A, cudaStream_t st);
 cudaError_t launch_swept_scan(int *counts, int n, int channels, int *totals, cudaStream_t st);
+// svsdf_map_clearance (svsdf_clearance.cu).  what: 0 k_cl_count (band bits per word, band cells per CTA, occupied columns), 1 k_cl_write
+// (the band's cells and centres in map order, after launch_swept_scan of the per-CTA counts).
+cudaError_t launch_clearance(int what, const ClearanceArgs &A, cudaStream_t st);
 // K5 (svsdf_frontend.cu)
 cudaError_t launch_front_cells(const ShapeParams &S, const FrontParams &F, const double *yaws, unsigned char *cells, cudaStream_t st);
 cudaError_t launch_front_expand(const ShapeParams &S, const FrontParams &F, const SubSwParams &P, const unsigned char *map,

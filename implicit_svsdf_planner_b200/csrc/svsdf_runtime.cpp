@@ -219,6 +219,9 @@ struct svsdf_ctx {
     // svsdf_swept_contour: grow-only device buffers (per corner, per needed corner, per CTA, outputs) and the samples' upload
     unsigned char *d_sw_corner = nullptr, *d_sw_point = nullptr, *d_sw_small = nullptr, *d_sw_out = nullptr;
     size_t cap_sw_corner = 0, cap_sw_point = 0, cap_sw_small = 0, cap_sw_out = 0;
+    // svsdf_map_clearance: grow-only device buffers (header, samples and per-CTA counts; band bits per map word; band cells)
+    unsigned char *d_cl_small = nullptr, *d_cl_band = nullptr, *d_cl_point = nullptr;
+    size_t cap_cl_small = 0, cap_cl_band = 0, cap_cl_point = 0;
 };
 
 namespace {
@@ -1623,6 +1626,7 @@ void svsdf_destroy(svsdf_ctx *ctx) {
     if (ctx->h_multi_out) cudaFreeHost(ctx->h_multi_out);
     cudaFree(ctx->d_multi_in); cudaFree(ctx->d_multi_scratch); cudaFree(ctx->d_multi_tickets);
     cudaFree(ctx->d_sw_corner); cudaFree(ctx->d_sw_point); cudaFree(ctx->d_sw_small); cudaFree(ctx->d_sw_out);
+    cudaFree(ctx->d_cl_small); cudaFree(ctx->d_cl_band); cudaFree(ctx->d_cl_point);
     if (ctx->ev_pts) cudaEventDestroy(ctx->ev_pts);
     if (ctx->lmbm) svsdf_lmbm_close(ctx->lmbm);
     if (ctx->ev0) cudaEventDestroy(ctx->ev0);
@@ -2070,6 +2074,156 @@ void svsdf_swept_free(svsdf_swept_mesh *mesh) {
     mesh->segments = nullptr;
     mesh->triangles = nullptr;
     mesh->field = nullptr;
+}
+
+// ---- svsdf_map_clearance (kernels: svsdf_clearance.cu; why the band is exact: DESIGN.md §7) -----------------------------------------
+int svsdf_map_clearance(svsdf_ctx *ctx, int N, const double *T, const double *coeffs, double d_max, svsdf_clearance *out) {
+    if (!ctx || !out) return SVSDF_ERR_INVALID;
+    std::memset(out, 0, sizeof(*out));
+    out->min_sdf = INFINITY;
+    out->argmin = -1;
+    auto invalid = [&](const char *msg) {
+        ctx->err = msg;
+        return SVSDF_ERR_INVALID;
+    };
+    // the band proves only "outer value > d_max"; for d_max >= 0 that value is the whole answer (no interior branch), below 0 it is not
+    if (!(d_max >= 0.0)) return invalid("svsdf_map_clearance: d_max must be >= 0 or +INFINITY");
+    BlobLayout L;
+    double D = 0.0;
+    const char *msg = nullptr;
+    if (traj_layout(N, T, coeffs, L, D, &msg) != SVSDF_OK) return invalid(msg);
+    for (int64_t e = 0; e < 18 * (int64_t)N; ++e)
+        if (!std::isfinite(coeffs[e])) return invalid("svsdf_map_clearance: non-finite trajectory coefficient");
+    if (!ctx->d_map) {
+        ctx->err = "svsdf_map_clearance: map not set";
+        return SVSDF_ERR_NOT_READY;
+    }
+    if ((int64_t)ctx->map_X * ctx->map_Y > 2000000000LL) return invalid("svsdf_map_clearance: map has more than 2e9 columns");
+    // the band: rho and the samples of svsdf_swept_contour with iso = d_max
+    const ShapeParams &S = ctx->shape;
+    const bool all = !(S.rout < 1e299) || !std::isfinite(d_max);
+    std::vector<double> samp;
+    if (!all) {
+        const double rho = std::max(std::max(S.prune_rmin, S.rout + S.prune_scale * d_max), 0.0);
+        swept_samples(ctx, N, T, coeffs, D, rho, samp);
+        if ((int)(samp.size() / 3) > kSweptMaxSamples) return invalid("svsdf_map_clearance: too many path samples");
+    }
+    CK(cudaSetDevice(ctx->device));
+    ClearanceArgs A;
+    std::memset(&A, 0, sizeof(A));
+    A.map = ctx->d_map;
+    A.X = ctx->map_X; A.Y = ctx->map_Y; A.h = ctx->map_h; A.row_bytes = ctx->map_row_bytes; A.Z = ctx->map_Z;
+    A.layer = (int64_t)(A.X + 2 * A.h) * A.row_bytes;
+    A.ox = ctx->map_ox; A.oy = ctx->map_oy; A.res = ctx->map_res;
+    A.wy0 = A.h / 32;
+    A.nW = (A.h + A.Y - 1) / 32 - A.wy0 + 1;
+    A.n_items = (int64_t)A.X * A.nW;
+    A.all = all ? 1 : 0;
+    A.n_samp = (int)(samp.size() / 3);
+    const int nblk = (int)((A.n_items + 255) / 256);
+    // small: header [0] occupied columns (u64), [8] band cells (int); samples; per-CTA counts
+    const size_t off_samp = 64, off_blk = off_samp + align16(samp.size() * 8);
+    int rc = grow_device(ctx, ctx->d_cl_small, ctx->cap_cl_small, off_blk + (size_t)(nblk + 1) * 4);
+    if (rc) return rc;
+    rc = grow_device(ctx, ctx->d_cl_band, ctx->cap_cl_band, (size_t)A.n_items * 4);
+    if (rc) return rc;
+    A.n_occ = reinterpret_cast<unsigned long long *>(ctx->d_cl_small);
+    int *d_total = reinterpret_cast<int *>(ctx->d_cl_small + 8);
+    A.samp = reinterpret_cast<double *>(ctx->d_cl_small + off_samp);
+    A.blk = reinterpret_cast<int *>(ctx->d_cl_small + off_blk);
+    A.band = reinterpret_cast<unsigned *>(ctx->d_cl_band);
+    rc = ensure_stage(ctx, 64 + samp.size() * 8);
+    if (rc) return rc;
+    unsigned char *hs = reinterpret_cast<unsigned char *>(ctx->h_stage);
+    std::memset(hs, 0, 64);
+    if (!samp.empty()) std::memcpy(hs + 64, samp.data(), samp.size() * 8);
+    cudaStream_t st = ctx->stream;
+    CK(cudaMemcpyAsync(ctx->d_cl_small, hs, 64 + samp.size() * 8, cudaMemcpyHostToDevice, st));
+    CK(launch_clearance(0, A, st));
+    CK(launch_swept_scan(A.blk, nblk, 1, d_total, st));
+    CK(cudaMemcpyAsync(hs, ctx->d_cl_small, 16, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    ctx->launches += 2;
+    unsigned long long n_occ;
+    int P32;
+    std::memcpy(&n_occ, hs, 8);
+    std::memcpy(&P32, hs + 8, 4);
+    const int64_t P = P32;
+    // band cells: (i, j) int32 pairs, centres, values, t* — contiguous, so one download brings them all
+    const size_t o_pts = align16((size_t)P * 8), o_sdf = o_pts + (size_t)P * 16, o_ts = o_sdf + (size_t)P * 8, o_end = o_ts + (size_t)P * 8;
+    rc = grow_device(ctx, ctx->d_cl_point, ctx->cap_cl_point, o_end + 16);
+    if (rc) return rc;
+    A.ij = reinterpret_cast<int *>(ctx->d_cl_point);
+    A.pts = reinterpret_cast<double *>(ctx->d_cl_point + o_pts);
+    double *d_sdf = reinterpret_cast<double *>(ctx->d_cl_point + o_sdf), *d_ts = reinterpret_cast<double *>(ctx->d_cl_point + o_ts);
+    if (P > 0) {
+        CK(launch_clearance(1, A, st));
+        ctx->launches += 1;
+        // svsdf_query's path (outer solve, then the interior branch) on the band: the same kernels, so the same bits per point
+        rc = upload_traj(ctx, N, T, coeffs);
+        if (rc) return rc;
+        rc = run_kernels(ctx, A.pts, P, false, true, d_sdf, d_ts, nullptr, nullptr);
+        if (rc) return rc;
+        rc = ensure_stage(ctx, o_end);
+        if (rc) return rc;
+        hs = reinterpret_cast<unsigned char *>(ctx->h_stage);
+        CK(cudaMemcpyAsync(hs, ctx->d_cl_point, o_end, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+    }
+    const int32_t *h_ij = reinterpret_cast<const int32_t *>(hs);
+    const double *h_xy = reinterpret_cast<const double *>(hs + o_pts), *h_sdf = reinterpret_cast<const double *>(hs + o_sdf),
+                 *h_ts = reinterpret_cast<const double *>(hs + o_ts);
+    int64_t n_within = 0;
+    for (int64_t p = 0; p < P; ++p) {
+        if (!std::isfinite(h_sdf[p])) {
+            ctx->err = "svsdf_map_clearance: non-finite value";
+            return SVSDF_ERR_NONFINITE;
+        }
+        n_within += h_sdf[p] <= d_max;
+    }
+    out->ij = static_cast<int32_t *>(std::malloc((size_t)n_within * 8 + 16));
+    out->xy = static_cast<double *>(std::malloc((size_t)n_within * 16 + 16));
+    out->sdf = static_cast<double *>(std::malloc((size_t)n_within * 8 + 16));
+    out->tstar = static_cast<double *>(std::malloc((size_t)n_within * 8 + 16));
+    if (!out->ij || !out->xy || !out->sdf || !out->tstar) {
+        svsdf_clearance_free(out);
+        ctx->err = "svsdf_map_clearance: out of host memory";
+        return SVSDF_ERR_INVALID;
+    }
+    int64_t k = 0, n_coll = 0;
+    for (int64_t p = 0; p < P; ++p) {
+        const double v = h_sdf[p];
+        if (!(v <= d_max)) continue;
+        out->ij[2 * k] = h_ij[2 * p];
+        out->ij[2 * k + 1] = h_ij[2 * p + 1];
+        out->xy[2 * k] = h_xy[2 * p];
+        out->xy[2 * k + 1] = h_xy[2 * p + 1];
+        out->sdf[k] = v;
+        out->tstar[k] = h_ts[p];
+        n_coll += v <= 0.0;
+        if (v < out->min_sdf) {  // strict: the first in list order among ties
+            out->min_sdf = v;
+            out->argmin = k;
+        }
+        ++k;
+    }
+    out->n_occupied = (int64_t)n_occ;
+    out->n_evaluated = P;
+    out->n_within = n_within;
+    out->n_colliding = n_coll;
+    return SVSDF_OK;
+}
+
+void svsdf_clearance_free(svsdf_clearance *c) {
+    if (!c) return;
+    std::free(c->ij);
+    std::free(c->xy);
+    std::free(c->sdf);
+    std::free(c->tstar);
+    c->ij = nullptr;
+    c->xy = nullptr;
+    c->sdf = nullptr;
+    c->tstar = nullptr;
 }
 
 int svsdf_cost_grad_device(svsdf_ctx *ctx, int N, const double *T, const double *coeffs, int repeats,

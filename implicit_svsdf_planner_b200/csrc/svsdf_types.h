@@ -222,6 +222,25 @@ struct SweptArgs {
     int *segs, *tris;          // [S][2], [F][3]
 };
 
+// svsdf_map_clearance (svsdf_clearance.cu): the occupied map columns near a trajectory.  One item per 32-cell word of a map row (the
+// words that hold real cells, rows 0 .. X - 1), 256 items per CTA, row-major: the CTA order is the map order.
+struct ClearanceArgs {
+    const unsigned char *map;  // Z layers of (X + 2h) x row_bytes, MSB-first bits along y (svsdf_set_map / svsdf_set_map3d)
+    int X, Y, h, row_bytes, Z;
+    int64_t layer;             // bytes per layer
+    double ox, oy, res;        // boundary_xyzmin (x, y) and grid resolution
+    int wy0, nW;               // first word of a row that holds a real cell, words per row
+    int64_t n_items;           // X * nW
+    int all;                   // 1: every occupied column is in the band (d_max = +inf or a shape without a far-field bound)
+    int n_samp;
+    const double *samp;        // [n_samp][3]: sample x, y and its reach (a centre farther than reach from every sample is > d_max)
+    unsigned *band;            // [n_items] band bits of the word (k_cl_count)
+    int *blk;                  // [n_blocks + 1] band cells per CTA, then their exclusive prefix (k_sw_scan)
+    unsigned long long *n_occ; // occupied columns of the map
+    int *ij;                   // [P][2] band cells in map order: (i, j)
+    double *pts;               // [P][2] their centres
+};
+
 // K5 (svsdf_frontend.cu): collision kernels of the A* front end
 constexpr int kMaxYawKernels = 64;
 constexpr int kMaxKernelSize = 32;  // kernel rows are held as 32-bit masks

@@ -76,8 +76,9 @@ def rot_z(yaw: float) -> np.ndarray:
 
 def generate_traj(ctx: "api.Context", cmap: CloudMap, start_xy, goal_xy, kernel_size: int = scenes.YAML["kernel_size"], kernel_yaw_num: int = 18,
                   front_end_safeh: float = 0.0, traj_parlength: float = 3.0, inittime: float = scenes.YAML["inittime"],
-                  mid_cfg: Optional["api.MidConfig"] = None, lbfgs_params=None, max_path: int = 4096) -> dict:
-    """generatePath + generateTraj for one start / goal on the map `cmap` (the context's shape is the robot)."""
+                  mid_cfg: Optional["api.MidConfig"] = None, lbfgs_params=None, max_path: int = 4096, certify: bool = False) -> dict:
+    """generatePath + generateTraj for one start / goal on the map `cmap` (the context's shape is the robot).  certify=True adds
+    `clearance` (see certificate) to a result that reached the back end."""
     X, Y, Z = cmap.occ.shape
     res = cmap.res
     ctx.set_map3d(pack_map_kernel3d(cmap.occ, kernel_size), X, Y, Z, kernel_size, cmap.boundary_min, res)
@@ -99,10 +100,23 @@ def generate_traj(ctx: "api.Context", cmap: CloudMap, start_xy, goal_xy, kernel_
     params = lbfgs_params or api.default_lbfgs_params(mem_size=16, past=3, delta=1e-6, g_epsilon=0.0, max_iterations=0, min_step=1e-32)
     f0, _ = ctx_evaluate(ctx, init_s, final_s, N, opt_x)
     rc, x, T, b, st = ctx.optimize(init_s, final_s, opt_x, N, params)  # the query points are the context's resident set (extract_points3d)
-    return dict(ok=rc >= 0, status=int(rc), N=N, n_points=int(n_points), path=path, waypoints=wps, expansions=int(expansions[0]), astar_rounds=int(rounds),
-                mid=dict(status=int(rc_mid), cost=float(cost_mid), iterations=int(it_mid), T=T_mid), cost_at_warm_start=float(f0),
-                final_cost=float(st["final_cost"]), iterations=int(st["iterations"]), evaluations=int(st["evaluations"]), T=T, coeffs=b, x=x,
-                seconds=float(st["seconds"]))
+    out = dict(ok=rc >= 0, status=int(rc), N=N, n_points=int(n_points), path=path, waypoints=wps, expansions=int(expansions[0]), astar_rounds=int(rounds),
+               mid=dict(status=int(rc_mid), cost=float(cost_mid), iterations=int(it_mid), T=T_mid), cost_at_warm_start=float(f0),
+               final_cost=float(st["final_cost"]), iterations=int(st["iterations"]), evaluations=int(st["evaluations"]), T=T, coeffs=b, x=x,
+               seconds=float(st["seconds"]))
+    if certify:
+        out["clearance"] = certificate(ctx, T, b)
+    return out
+
+
+def certificate(ctx: "api.Context", T, coeffs) -> dict:
+    """The trajectory checked against every occupied cell of the context's map (svsdf_map_clearance, the reference's getMinSVSDF) with
+    d_max = the context's safety_hor: the least swept-volume SDF value over the cells within the penalty's horizon, where it is reached,
+    and collision_free = min_sdf > 0.  `ok` says only that the solver returned status >= 0; this says whether the robot misses the map."""
+    c = ctx.map_clearance(T, np.asarray(coeffs).reshape(-1), ctx.safety_hor)
+    k = c.argmin
+    return dict(min_sdf=c.min_sdf, argmin_xy=c.xy[k].copy() if k >= 0 else None, t_star=float(c.tstar[k]) if k >= 0 else None,
+                n_colliding=c.n_colliding, n_within=c.n_within, n_evaluated=c.n_evaluated, collision_free=bool(c.min_sdf > 0.0))
 
 
 def ctx_evaluate(ctx, init_s, final_s, N, x):
@@ -118,14 +132,16 @@ _ASTAR_REASON = {0: "start or goal outside the map", 2: "front end found no path
 def plan_batch(ctx: "api.Context", cmap: CloudMap, starts, goals, kernel_size: int = scenes.YAML["kernel_size"], kernel_yaw_num: int = 18,
                front_end_safeh: float = 0.0, traj_parlength: float = 3.0, inittime: float = scenes.YAML["inittime"],
                mid_cfg: Optional["api.MidConfig"] = None, lbfgs_params=None, max_path: int = 4096, max_in_flight: int = 0,
-               workers: Optional[int] = None, stats: Optional[dict] = None, back_end: bool = True) -> list:
+               workers: Optional[int] = None, stats: Optional[dict] = None, back_end: bool = True, certify: bool = False) -> list:
     """generate_traj for n start / goal pairs on one map: one device A* launch for all searches (svsdf_front_astar_device), per problem the
     waypoints, the query points (extract_points3d, on the context) and the warm start (mid_get_ori_traj, on a thread pool: the mid end is
     host code and ctypes releases the GIL), then ONE lock-step back end (svsdf_optimize_lockstep) for every problem whose mid end succeeded.
     Returns one dict per problem with generate_traj's keys (except astar_rounds) and its bits, plus the query points (`points`);
     a failed problem has ok=False and the reason (an exception of one problem's extraction or mid end fails that problem only).
     stats (optional dict) receives the wall seconds of each stage, the back end's rounds and its kernel launches.  back_end=False stops
-    before the back end: the problems that would enter it are returned with its inputs (init_s, final_s, x0, points) instead."""
+    before the back end: the problems that would enter it are returned with its inputs (init_s, final_s, x0, points) instead.
+    certify=True adds generate_traj's `clearance` to every problem that went through the back end (one svsdf_map_clearance per problem,
+    after the back end; stats then also holds its wall seconds, certify_s)."""
     st = np.asarray(starts, dtype=np.float64).reshape(-1, 2)
     go = np.asarray(goals, dtype=np.float64).reshape(-1, 2)
     n = st.shape[0]
@@ -203,4 +219,11 @@ def plan_batch(ctx: "api.Context", cmap: CloudMap, starts, goals, kernel_size: i
                       expansions=int(expansions[q]), mid=p["mid"], cost_at_warm_start=r["cost_at_start"], final_cost=float(r["final_cost"]),
                       iterations=int(r["iterations"]), evaluations=int(r["evaluations"]), T=r["T"], coeffs=r["coeffs"], x=r["x"],
                       seconds=float(r["seconds"]), points=p["points"])
+    if certify:
+        t5 = time.perf_counter()
+        for p in back:
+            r = out[p["q"]]
+            r["clearance"] = certificate(ctx, r["T"], r["coeffs"])
+        if stats is not None:
+            stats["certify_s"] = time.perf_counter() - t5
     return out

@@ -178,6 +178,41 @@ int svsdf_swept_contour(svsdf_ctx *ctx, int N, const double *T, const double *co
                         svsdf_swept_mesh *out);
 void svsdf_swept_free(svsdf_swept_mesh *mesh);
 
+/* ---- Map clearance: a trajectory checked against every occupied cell of the map ----------------------------------------------
+ * svsdf_map_clearance evaluates the swept-volume SDF of the trajectory (N, T, coeffs) at the centre of every occupied map column and lists
+ * the cells whose value is <= d_max.  It is the check the reference declares as PlannerManager::getMinSVSDF (plan_manager.hpp:45) and
+ * never defines: is the optimised trajectory collision free against the whole map, not only against the back end's query points?
+ *   Obstacles: the occupied cells of the context's map (svsdf_set_map, svsdf_set_map_device or svsdf_set_map3d).  A column (i, j) counts
+ *     once when any of its z layers is occupied (the back end zeroes z too, so every voxel it would penalise is covered).  Only cells
+ *     inside the map count: the map kernel's padding and the outside of the map are NOT obstacles here, unlike the reference's
+ *     isOccupied, which treats out-of-range indices as occupied (Gridmap3D.cpp:199-202).
+ *   Centre of cell (i, j): ((i + 0.5) res + ox, (j + 0.5) res + oy), rounded as svsdf_extract_points[3d] rounds it, bit for bit.
+ *   Value: exactly what svsdf_query(..., outer_only = 0) returns for that centre on this context (getTrueSDFofSweptVolume<true>: the
+ *     interior (GSIP) depth where the centre is inside), for every shape, pre-transform, scale schedule and build.
+ *   List: every occupied cell with value <= d_max, in ascending i * Y + j order; n_within, n_colliding, min_sdf and argmin are computed
+ *     from it (argmin: the first cell in list order among ties; +INFINITY and -1 for an empty list).
+ *   d_max: >= 0 or +INFINITY.  Only the cells near the path are evaluated (n_evaluated of n_occupied): a column is skipped only when the
+ *     band bound of svsdf_swept_contour with iso = d_max proves its outer value > d_max >= 0, and then that outer value is the answer.
+ *     d_max = +INFINITY, or a shape without a far-field bound, evaluates every occupied column.
+ * Errors (nothing allocated): SVSDF_ERR_INVALID for a NaN or negative d_max, a bad trajectory or non-finite coefficients;
+ * SVSDF_ERR_NOT_READY without a map; SVSDF_ERR_NONFINITE when an evaluated value is not finite.  A fixed number of kernel launches per
+ * call, whatever the map size (none of the evaluation's when no column is near the path); the context's resident points,
+ * last_n_inside and everything svsdf_cost_grad depends on keep their values.  Release the arrays with svsdf_clearance_free. */
+typedef struct {
+    int64_t n_occupied;   /* occupied map columns (cells (i, j) with any occupied z layer) */
+    int64_t n_evaluated;  /* columns whose value was computed (the band) */
+    int64_t n_within;     /* listed cells: value <= d_max */
+    int64_t n_colliding;  /* listed cells with value <= 0 */
+    double  min_sdf;      /* minimum over the listed cells; +INFINITY when none */
+    int64_t argmin;       /* index into the list (first in list order among ties); -1 when none */
+    int32_t *ij;          /* n_within x 2: cell index (i, j) */
+    double  *xy;          /* n_within x 2: cell centre */
+    double  *sdf;         /* n_within */
+    double  *tstar;       /* n_within */
+} svsdf_clearance;
+int svsdf_map_clearance(svsdf_ctx *ctx, int N, const double *T, const double *coeffs, double d_max, svsdf_clearance *out);
+void svsdf_clearance_free(svsdf_clearance *c);
+
 /* R2: per-point swept-volume SDF query on the trajectory given by (N, T, coeffs).
  * pts: P x 3 (x, y, z) host doubles (z ignored).  Outputs (host, may be NULL): sdf[P], tstar[P], grad3[3P]
  * (body-frame FD gradient for sdf > 0; world-frame unit direction for the interior branch, exactly what the

@@ -14,6 +14,7 @@
 // last_error() gives the text.  Construction throws std::runtime_error when no sm_90 (H100) GPU is usable (no CPU fallback).
 #pragma once
 #include <array>
+#include <cmath>
 #include <cstdint>
 #include <memory>
 #include <stdexcept>
@@ -170,6 +171,16 @@ class SweptVolumeManager {
         G.assign(m.triangles, m.triangles + 3 * m.n_triangles);
         svsdf_swept_free(&m);
         return SVSDF_OK;
+    }
+    // getMinSVSDF (plan_manager.hpp:45: declared by the reference, never defined): the minimum of getTrueSDFofSweptVolume over the
+    // occupied cells of the context's map with value <= d_max (svsdf_map_clearance), +INFINITY when there is none; > 0 means the current
+    // trajectory is collision free against the whole map.  NaN when the call fails (see svsdf_last_error).
+    double getMinSVSDF(double d_max = INFINITY) {
+        svsdf_clearance c{};
+        if (svsdf_map_clearance(ctx_->h, N_, T_.data(), c_.data(), d_max, &c) != SVSDF_OK) return NAN;
+        const double m = c.min_sdf;
+        svsdf_clearance_free(&c);
+        return m;
     }
     // batched query (P rows of 3 doubles): what a caller with many points should use
     int getTrueSDFofSweptVolume(int64_t P, const double *pos_eva, double *sdf, double *tstar, double *grad3, int *rounds = nullptr) {
