@@ -143,6 +143,20 @@ void orc_expand_nodes(const char *name, const double *poly_params, int ks, int K
         expand_node(S, SK, M, G, node_ij[2 * q], node_ij[2 * q + 1], node_yaw[q], ks, ok_out + 9 * q, child_yaw_out + 9 * q, parts_out + 9 * q);
 }
 
+// PCSmapManager::getPointsInAABB2D (points_in_aabb2d) around (cx, cy): writes up to cap points (x, y), returns how many there are
+int64_t orc_points_in_aabb(const uint8_t *occ, int X, int Y, double ox, double oy, double map_res, double cx, double cy, double hbx, double hby,
+                           double *xy, int64_t cap) {
+    FrontMap M;
+    M.build(occ, X, Y, 1);
+    MapGeom G;
+    G.ox = ox; G.oy = oy; G.res = map_res;
+    std::vector<double> pts;
+    points_in_aabb2d(M, G, cx, cy, hbx, hby, pts);
+    const int64_t np = (int64_t)pts.size() / 2;
+    std::memcpy(xy, pts.data(), (size_t)std::min(np, cap) * 2 * sizeof(double));
+    return np;
+}
+
 // AstarPathSearch for n start/goal pairs; path_out [n][max_path][3], len_out [n] (0 = no path), exp_out [n] expansions
 void orc_astar(const char *name, const double *poly_params, int ks, int K, double safeh, const uint8_t *occ, int X, int Y, double ox, double oy,
                double map_res, int n, const double *start_xy, const double *goal_xy, int max_path, double *path_out, int *len_out, int *exp_out) {

@@ -88,6 +88,9 @@ def lib(variant: str = "default"):
                                        C.c_double, C.c_int64, C.POINTER(C.c_int), dp, u8, dp, u8]
         L.orc_astar.argtypes = [C.c_char_p, dp, C.c_int, C.c_int, C.c_double, u8, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int, dp,
                                 dp, C.c_int, dp, C.POINTER(C.c_int), C.POINTER(C.c_int)]
+        L.orc_points_in_aabb.restype = C.c_int64
+        L.orc_points_in_aabb.argtypes = [u8, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double,
+                                         C.c_double, dp, C.c_int64]
         L.orc_max_threads.restype = C.c_int
         L.orc_num_procs.restype = C.c_int
         _libs[variant] = L
@@ -203,6 +206,17 @@ def expand_nodes(name, occ, node_ij, node_yaw, origin=(0.0, 0.0), map_res=1.0, k
     lib().orc_expand_nodes(name.encode(), _p(pp), kernel_size, kernel_count, float(map_res), safeh, _u8p(occ), X, Y, float(origin[0]),
                            float(origin[1]), float(map_res), n, ij.ctypes.data_as(C.POINTER(C.c_int)), _p(fy), _u8p(ok), _p(cy), _u8p(parts))
     return ok.astype(bool), cy, parts
+
+
+def points_in_aabb(occ, centre, half, origin=(0.0, 0.0), map_res=1.0):
+    """PCSmapManager::getPointsInAABB2D: the occupied cell centres [m, 2] in the box of half size `half` around `centre`."""
+    occ = np.ascontiguousarray(occ, dtype=np.uint8)
+    X, Y = occ.shape
+    cap = X * Y
+    xy = np.empty((max(cap, 1), 2))
+    m = lib().orc_points_in_aabb(_u8p(occ), X, Y, float(origin[0]), float(origin[1]), float(map_res), float(centre[0]), float(centre[1]),
+                                 float(half), float(half), _p(xy), cap)
+    return xy[:m].copy()
 
 
 def astar(name, occ, start_xy, goal_xy, origin=(0.0, 0.0), map_res=1.0, kernel_size=17, kernel_count=18, safeh=0.0, max_path=1024,

@@ -40,7 +40,8 @@ def main(ref: str) -> None:
         fh.write(text)
     with open(os.path.join(gen, "sw_macros.inc"), "a", encoding="utf-8") as fh:
         fh.write("// ---- ours: the deformable-robot build\n#undef useScale\n#define useScale true\n")
-    shutil.copyfile(os.path.join(HERE, "ref_path_shim.cpp"), os.path.join(OUT, "ref_path_shim.cpp"))
+    for f in ("ref_path_shim.cpp", "ref_shape_scaffold.inc"):  # the scaffold's `_ref/gen/` includes must resolve to the copy too
+        shutil.copyfile(os.path.join(HERE, f), os.path.join(OUT, f))
     print("ref_extract_scale: wrote", OUT)
 
 

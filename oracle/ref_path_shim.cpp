@@ -81,70 +81,7 @@ struct Config {
 #include <utils/trajectory.hpp>  // WHOLE reference header (Piece<D>, Trajectory<D>)
 #include <utils/minco.hpp>       // WHOLE reference header (BandedSystem, MINCO_S2NU/S3NU/S4NU)
 
-#include "_ref/gen/shape_macros.inc"  // PI, DEFINE_USEFUL_FUNCTION (Shape.hpp:31,34-78)
-
-namespace shape {
-#include "_ref/gen/shape_or_mask.inc"  // Shape.hpp:95
-
-class BasicShape {
-  private:
-    Config config;
-#include "_ref/gen/shape_base_kernels.inc"  // Shapekernel, ByteShapeKernel (Shape.hpp:100-218)
-    int kernel_count{-1};
-    int kernelsize{-1};
-    double kernelresu{-1};
-    bool initselfkerneldone{false};
-
-  public:
-    Eigen::Vector3d trans;
-    Eigen::Matrix3d Rotate;
-    double yaw;
-    Shapekernel *shape_kernels{nullptr};
-    ByteShapeKernel *byte_shape_kernels{nullptr};
-
-    // same virtual surface as Shape.hpp:266-270
-    virtual double getonlySDF(const Eigen::RowVector3d &) { return 0; }
-    virtual double getonlySDF(const Eigen::RowVector3d &, const Eigen::Matrix3d &) { return 0; }
-    virtual Eigen::Vector3d getonlyGrad1(const Eigen::RowVector3d &) { return Eigen::Vector3d::Zero(); }
-    virtual double getSDFwithGrad1(const Eigen::RowVector3d &, Eigen::Vector3d &) { return 0; }
-    virtual Eigen::Matrix3d getonlyGrad2(const Eigen::RowVector3d &) { return Eigen::Matrix3d::Zero(); }
-
-    BasicShape(const Config &conf) : config(conf) {
-        kernel_count = conf.kernel_yaw_num;  // Shape.hpp:273-275
-        kernelsize = conf.kernel_size;
-        kernelresu = conf.occupancy_resolution;
-        std::vector<double> para;
-        para = config.poly_params;
-        // (host-side set-up, runs once: keeps glibc's sin/cos in BOTH variants, as the product's host code does;
-        //  "portable" redirects only what the kernels evaluate per sample)
-#ifdef REF_LIBM_PORTABLE
-#pragma push_macro("sin")
-#pragma push_macro("cos")
-#undef sin
-#undef cos
-#endif
-#include "_ref/gen/shape_base_ctor_transform.inc"  // Shape.hpp:287-294 verbatim (mesh loading around it omitted)
-#ifdef REF_LIBM_PORTABLE
-#pragma pop_macro("sin")
-#pragma pop_macro("cos")
-#endif
-    }
-    void getTransform(Matrix3d &R, RowVector3d &trans_) {  // Shape.hpp:357-362
-        R = Rotate;
-        trans_ = trans.transpose();
-    }
-    virtual ~BasicShape() {
-        delete[] shape_kernels;
-        delete[] byte_shape_kernels;
-    }
-    int kernelCount() const { return kernel_count; }
-    int kernelSize() const { return kernelsize; }
-#include "_ref/gen/shape_base_initshape.inc"  // initShape (Shape.hpp:384-430)
-};
-
-#include "_ref/gen/shape_classes.inc"  // Circle, the 16 registry shapes, Polygon (Shape.hpp:432-1572)
-}  // namespace shape
-using namespace shape;  // sw_manager.hpp:21
+#include "ref_shape_scaffold.inc"  // BasicShape scaffolding + the verbatim shape classes (Shape.hpp)
 
 #include "_ref/gen/sw_macros.inc"     // TRAJ_ORDER, useScale, useNumer, pi (sw_manager.hpp:16-20)
 #include "_ref/gen/sw_sampleset.inc"  // CircleCoord2D, SampleSet2D (sw_manager.hpp:25-124)

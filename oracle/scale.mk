@@ -19,7 +19,7 @@ REF_SRC ?= /root/reference
 REF_INC ?= /root/reference/src/utils/include
 REF_PATH_FLAGS := -O3 -DNDEBUG -std=c++17 -fPIC -fopenmp -ffp-contract=off -w -Iref_shim -I$(REF_INC) -I.
 ref: _ref/libref_path_scaled_glibc.so _ref/libref_path_scaled_portable.so
-_ref/scaled/.stamp: ref_extract.py ref_extract_scale.py ref_path_shim.cpp
+_ref/scaled/.stamp: ref_extract.py ref_extract_scale.py ref_path_shim.cpp ref_shape_scaffold.inc
 	python3 ref_extract_scale.py --ref $(REF_SRC)
 	touch $@
 SCALED_DEPS := ref_path_scaled_shim.cpp ref_scale_hook.inc ref_shim/Eigen/Eigen portable_sincos.hpp _ref/scaled/.stamp

@@ -1,6 +1,9 @@
 """GPU parity tests of the A* front end's collision kernels (SURVEY.md §8f rank 3; csrc/svsdf_frontend.cu) through the C ABI:
 svsdf_front_init / _get_kernels (BasicShape::initShape), svsdf_front_cspace (kernelConv over the whole configuration space),
-svsdf_front_check_kernel_value (checkKernelValue).  Integer / byte work: everything is compared bit for bit with the oracle."""
+svsdf_front_check_kernel_value (checkKernelValue).  Integer / byte work: everything is compared bit for bit with the oracle.
+The oracle is itself held to the reference's own node test and search by tests/test_oracle_front_ref_pin.py, and
+tests/test_gpu_front_edges.py takes every entry point to the limits of its inputs (resolutions, box sizes, map shapes, yaw
+counts and father yaws) against both."""
 import numpy as np
 import pytest
 
