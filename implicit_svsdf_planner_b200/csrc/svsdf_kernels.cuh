@@ -1681,8 +1681,8 @@ cudaError_t query_occupancy(const ShapeParams &S, int N, int blob_doubles, int *
     }
 }
 
-static cudaError_t launch_cost_impl(const KernelArgs &A, const ShapeParams &S, const ScaleSched *Z, int N, int grid_outer,
-                                    int grid_gsip, cudaStream_t stream, cudaEvent_t after_outer, int gsip_wide) {
+cudaError_t launch_cost_kernels(const KernelArgs &A, const ShapeParams &S, const ScaleSched *Z, int N, int grid_outer, int grid_gsip,
+                                cudaStream_t stream, cudaEvent_t after_outer, int gsip_wide) {
     LaunchCfg cfg;
     cfg.after_outer = after_outer;
     cfg.gsip_wide = gsip_wide != 0;
@@ -1694,20 +1694,11 @@ static cudaError_t launch_cost_impl(const KernelArgs &A, const ShapeParams &S, c
     return S.has_xform ? dispatch<true>(A, S, Z, cfg, N) : dispatch<false>(A, S, Z, cfg, N);
 }
 
-#ifdef SVSDF_SCALED_UNIT
-cudaError_t launch_cost_kernels(const KernelArgs &A, const ShapeParams &S, const ScaleSched &Z, int N, int grid_outer, int grid_gsip,
-                                cudaStream_t stream, cudaEvent_t after_outer, int gsip_wide) {
-    return launch_cost_impl(A, S, &Z, N, grid_outer, grid_gsip, stream, after_outer, gsip_wide);
-}
-#else
+// the rigid units also bring the launchers every variant shares
+#ifndef SVSDF_SCALED_UNIT
 cudaError_t launch_pose_table(double *blob, int K1, cudaStream_t stream) {
     k_pose_table<<<(K1 + 127) / 128, 128, 0, stream>>>(blob);
     return cudaGetLastError();
-}
-
-cudaError_t launch_cost_kernels(const KernelArgs &A, const ShapeParams &S, int N, int grid_outer, int grid_gsip,
-                                cudaStream_t stream, cudaEvent_t after_outer, int gsip_wide) {
-    return launch_cost_impl(A, S, nullptr, N, grid_outer, grid_gsip, stream, after_outer, gsip_wide);
 }
 
 cudaError_t launch_finalize(const double *partials, int n_blocks, int N, const int *n_inside,

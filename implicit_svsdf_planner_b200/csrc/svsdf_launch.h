@@ -1,18 +1,37 @@
-// svsdf_launch.h — host-callable launchers exported by the two kernel translation units
-// (svsdf_kernels_fast.cu: FMA contraction on; svsdf_kernels_strict.cu: -fmad=false).
+// svsdf_launch.h — host-callable launchers exported by the kernel translation units (fast: FMA contraction on; strict:
+// -fmad=false).
 #pragma once
 #include <cuda_runtime.h>
 
 #include "svsdf_types.h"
 
 namespace svsdf {
-#define SVSDF_DECLARE_LAUNCHERS(NS)                                                                              \
+// Launchers of every kernel variant: the single-problem unit NS (svsdf_kernels_{fast,strict}.cu, and for deformable robots
+// svsdf_kernels_scaled_{fast,strict}.cu) and its multi-problem unit MULTI (svsdf_kernels_multi*.cu, svsdf_cost_grad_multi).  Z, the
+// scale schedule, is read by the scaled units only.  launch_multi: what = 0 sparse / 1 batched k_outer_multi, 2 k_gsip_multi (grid <= 0:
+// one full wave of the chosen variant).
+#define SVSDF_DECLARE_LAUNCHERS(NS, MULTI)                                                                        \
+    namespace NS {                                                                                               \
+    cudaError_t query_occupancy(const ShapeParams &S, int N, int blob_doubles, int *occ_outer, int *occ_gsip);   \
+    cudaError_t launch_cost_kernels(const KernelArgs &A, const ShapeParams &S, const ScaleSched *Z, int N,       \
+                                    int grid_outer, int grid_gsip, cudaStream_t stream, cudaEvent_t after_outer, \
+                                    int gsip_wide);                                                              \
+    }                                                                                                            \
+    namespace MULTI {                                                                                            \
+    cudaError_t launch_multi(int what, const KernelArgs &A, const MultiArgs &M, const ShapeParams &S,            \
+                             const ScaleSched *Z, int grid, size_t smem, int gsip_wide, int sm_count,            \
+                             cudaStream_t st);                                                                   \
+    }
+SVSDF_DECLARE_LAUNCHERS(fast, fast_multi)
+SVSDF_DECLARE_LAUNCHERS(strict, strict_multi)
+SVSDF_DECLARE_LAUNCHERS(fast_scaled, fast_multi_scaled)
+SVSDF_DECLARE_LAUNCHERS(strict_scaled, strict_multi_scaled)
+#undef SVSDF_DECLARE_LAUNCHERS
+// Only the rigid units define these; the scaled variants use them too.  The multi-problem ones run the pose table, the compaction and the
+// finalize of every multi launch.
+#define SVSDF_DECLARE_RIGID_LAUNCHERS(NS, MULTI)                                                                  \
     namespace NS {                                                                                               \
     cudaError_t launch_pose_table(double *blob, int K1, cudaStream_t stream);                                    \
-    cudaError_t query_occupancy(const ShapeParams &S, int N, int blob_doubles, int *occ_outer, int *occ_gsip);   \
-    cudaError_t launch_cost_kernels(const KernelArgs &A, const ShapeParams &S, int N, int grid_outer,            \
-                                    int grid_gsip, cudaStream_t stream, cudaEvent_t after_outer,                 \
-                                    int gsip_wide);                                                              \
     cudaError_t launch_finalize(const double *partials, int n_blocks, int N, const int *n_inside,                \
                                 const double *gsip_contrib, const int *gsip_piece, double *tot,                  \
                                 unsigned int *ticket, double *out, cudaStream_t stream);                         \
@@ -20,46 +39,16 @@ namespace svsdf {
                                   cudaStream_t stream);                                                          \
     cudaError_t launch_fp64_peak(double *out, int grid, int iters, cudaStream_t stream);                         \
     cudaError_t launch_sincos(const double *x, int64_t n, double *s, double *c, cudaStream_t stream);            \
-    }
-SVSDF_DECLARE_LAUNCHERS(fast)
-SVSDF_DECLARE_LAUNCHERS(strict)
-#undef SVSDF_DECLARE_LAUNCHERS
-// deformable robots (svsdf_kernels_scaled_fast.cu / svsdf_kernels_scaled_strict.cu): the same cost kernels with the
-// schedule Z as an extra kernel parameter
-#define SVSDF_DECLARE_SCALED_LAUNCHERS(NS)                                                                       \
-    namespace NS {                                                                                               \
-    cudaError_t query_occupancy(const ShapeParams &S, int N, int blob_doubles, int *occ_outer, int *occ_gsip);   \
-    cudaError_t launch_cost_kernels(const KernelArgs &A, const ShapeParams &S, const ScaleSched &Z, int N,       \
-                                    int grid_outer, int grid_gsip, cudaStream_t stream, cudaEvent_t after_outer, \
-                                    int gsip_wide);                                                              \
-    }
-SVSDF_DECLARE_SCALED_LAUNCHERS(fast_scaled)
-SVSDF_DECLARE_SCALED_LAUNCHERS(strict_scaled)
-#undef SVSDF_DECLARE_SCALED_LAUNCHERS
-// svsdf_cost_grad_multi (svsdf_kernels_multi.cuh).  launch_multi: what = 0 sparse / 1 batched k_outer_multi, 2 k_gsip_multi (grid <= 0:
-// one full wave of the chosen variant); Z is read by the scaled units only.  The rigid units also run the pose table, the
-// compaction and the finalize of every multi launch.
-#define SVSDF_DECLARE_MULTI_LAUNCHERS(NS)                                                                         \
-    namespace NS {                                                                                               \
-    cudaError_t launch_multi(int what, const KernelArgs &A, const MultiArgs &M, const ShapeParams &S,            \
-                             const ScaleSched *Z, int grid, size_t smem, int gsip_wide, int sm_count,            \
-                             cudaStream_t st);                                                                   \
-    }
-SVSDF_DECLARE_MULTI_LAUNCHERS(fast_multi)
-SVSDF_DECLARE_MULTI_LAUNCHERS(strict_multi)
-SVSDF_DECLARE_MULTI_LAUNCHERS(fast_multi_scaled)
-SVSDF_DECLARE_MULTI_LAUNCHERS(strict_multi_scaled)
-#undef SVSDF_DECLARE_MULTI_LAUNCHERS
-#define SVSDF_DECLARE_MULTI_RIGID(NS)                                                                            \
-    namespace NS {                                                                                               \
+    }                                                                                                            \
+    namespace MULTI {                                                                                            \
     cudaError_t launch_pose_multi(double *blobs, const MultiArgs &M, int max_K1, cudaStream_t st);               \
     cudaError_t launch_compact_multi(const unsigned char *flag, int *list, const MultiArgs &M, cudaStream_t st); \
     cudaError_t launch_finalize_multi(const double *partials, const double *gsip_contrib, const int *gsip_piece, \
                                       const MultiArgs &M, int max_N, cudaStream_t st);                           \
     }
-SVSDF_DECLARE_MULTI_RIGID(fast_multi)
-SVSDF_DECLARE_MULTI_RIGID(strict_multi)
-#undef SVSDF_DECLARE_MULTI_RIGID
+SVSDF_DECLARE_RIGID_LAUNCHERS(fast, fast_multi)
+SVSDF_DECLARE_RIGID_LAUNCHERS(strict, strict_multi)
+#undef SVSDF_DECLARE_RIGID_LAUNCHERS
 cudaError_t launch_extract_count(const ExtractArgs &E, int *block_counts, int n_blocks, int64_t *n_total,
                                  cudaStream_t stream);
 cudaError_t launch_extract_write(const ExtractArgs &E, const int *block_offsets, int n_blocks, double *out_xy,

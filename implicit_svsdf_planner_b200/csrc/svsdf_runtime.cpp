@@ -83,6 +83,71 @@ struct HostEval {
         for (int i = 0; i < 3 * (N - 1); ++i) g[N + i] = gradByPoints[i];
         return cost;
     }
+    // The final trajectory from the solver's returned iterate x (optimize_traj_lmbm does the same on success and failure,
+    // back_end_optimizer.cpp:44-94) and the run's statistics.
+    void finish(const double *x, const host::LbfgsResult &R, double seconds, double gpu_seconds, double *T_out, double *coeffs_out,
+                svsdf_opt_stats *stats) {
+        for (int i = 0; i < N; ++i) times[i] = host::forwardT(x[i]);
+        minco.setParameters(x + N, times.data());
+        if (T_out) std::memcpy(T_out, times.data(), sizeof(double) * N);
+        if (coeffs_out) std::memcpy(coeffs_out, minco.getCoeffs(), sizeof(double) * 18 * N);
+        if (stats) {
+            stats->final_cost = R.f;
+            stats->iterations = R.iterations;
+            stats->evaluations = R.evaluations;
+            stats->status = R.status;
+            stats->seconds = seconds;
+            stats->gpu_seconds = gpu_seconds;
+        }
+    }
+};
+
+// An owning block of device memory (or, PINNED, page-locked host memory) of T.  reserve(n) is grow-only and keeps no contents: when the
+// block holds fewer than n elements it is freed and n + n / 2 + 4096 are allocated (reserve_exact: n).  A reserved buffer is never null,
+// even for n = 0.
+template <class T, bool PINNED = false>
+class Buffer {
+  public:
+    Buffer() = default;
+    Buffer(Buffer &&o) noexcept : p_(o.p_), cap_(o.cap_) { o.p_ = nullptr; o.cap_ = 0; }
+    Buffer &operator=(Buffer &&o) noexcept {
+        std::swap(p_, o.p_);
+        std::swap(cap_, o.cap_);
+        return *this;
+    }
+    ~Buffer() { release(); }
+    cudaError_t reserve(size_t n) { return p_ && n <= cap_ ? cudaSuccess : allocate(n + n / 2 + 4096); }
+    cudaError_t reserve_exact(size_t n) { return p_ && n <= cap_ ? cudaSuccess : allocate(n); }
+    void release() {
+        if (p_) PINNED ? cudaFreeHost(p_) : cudaFree(p_);
+        p_ = nullptr;
+        cap_ = 0;
+    }
+    size_t capacity() const { return cap_; }
+    T *get() const { return p_; }
+    operator T *() const { return p_; }
+
+  private:
+    cudaError_t allocate(size_t n) {
+        release();
+        void *q = nullptr;
+        const cudaError_t e = PINNED ? cudaMallocHost(&q, n * sizeof(T)) : cudaMalloc(&q, n * sizeof(T));
+        if (e != cudaSuccess) return e;
+        p_ = static_cast<T *>(q);
+        cap_ = n;
+        return cudaSuccess;
+    }
+    T *p_ = nullptr;
+    size_t cap_ = 0;
+};
+template <class T>
+using DeviceBuffer = Buffer<T>;
+template <class T>
+using PinnedBuffer = Buffer<T, true>;
+
+// (resident single-problem k_outer, k_gsip CTAs per SM) of one trajectory size
+struct Occupancy {
+    int outer, gsip;
 };
 
 struct svsdf_ctx {
@@ -103,85 +168,74 @@ struct svsdf_ctx {
     int64_t launches = 0;
 
     // query points
-    double *d_mesh_tri = nullptr;  // SH_MESH: kMeshStride doubles per face
-    unsigned int *d_fwn_child = nullptr;  // SH_MESH: the winding-number hierarchy (host/fwn_bvh.hpp)
-    float *d_fwn_data = nullptr, *d_fwn_cbox = nullptr, *d_fwn_trif = nullptr;
+    DeviceBuffer<double> d_mesh_tri;  // SH_MESH: kMeshStride doubles per face
+    DeviceBuffer<unsigned int> d_fwn_child;  // SH_MESH: the winding-number hierarchy (host/fwn_bvh.hpp)
+    DeviceBuffer<float> d_fwn_data, d_fwn_cbox, d_fwn_trif;
     // K5: A* front-end collision kernels
     bool front_ready = false;
     FrontParams front{};
     std::vector<double> front_yaw;
     std::vector<unsigned char> front_cells, front_bytes;
-    unsigned char *d_front_bytes = nullptr;
-    unsigned *d_front_rowmask = nullptr;
-    unsigned *d_cspace = nullptr;
-    size_t cap_cspace = 0;
-    unsigned char *d_front_scratch = nullptr;  // grow-only device scratch of the batched front-end calls
-    size_t cap_front_scratch = 0;
-    unsigned char *d_astar_pool = nullptr;     // grow-only search slots of svsdf_front_astar_device
-    size_t cap_astar_pool = 0;
-    double *d_points = nullptr;  // packed xy
-    bool own_points = true;
+    DeviceBuffer<unsigned char> d_front_bytes;
+    DeviceBuffer<unsigned> d_front_rowmask;
+    DeviceBuffer<unsigned> d_cspace;
+    DeviceBuffer<unsigned char> d_front_scratch;  // device scratch of the batched front-end calls
+    DeviceBuffer<unsigned char> d_astar_pool;     // search slots of svsdf_front_astar_device (exactly sized, see kAstarPoolCap)
+    // packed xy: the caller's block (svsdf_set_points_device) when one is set, else points_buf
+    DeviceBuffer<double> points_buf;
+    const double *points_ext = nullptr;
+    const double *points() const { return points_ext ? points_ext : points_buf.get(); }
     int64_t P = 0;
-    int64_t cap_points = 0;
     // scratch sized by P
-    unsigned char *d_flag = nullptr;
-    double *d_inside_tstar = nullptr;
-    int *d_inside_list = nullptr;
-    double *d_gsip_contrib = nullptr;
-    int *d_gsip_piece = nullptr;
-    int64_t cap_scratch = 0;
-    int *d_n_inside = nullptr;
-    unsigned long long *d_eval_counter = nullptr;
+    DeviceBuffer<unsigned char> d_flag;
+    DeviceBuffer<double> d_inside_tstar;
+    DeviceBuffer<int> d_inside_list;
+    DeviceBuffer<double> d_gsip_contrib;
+    DeviceBuffer<int> d_gsip_piece;
+    DeviceBuffer<int> d_n_inside;
+    DeviceBuffer<unsigned long long> d_eval_counter;
     bool count_evals = false;
     // trajectory blob
-    double *d_blob = nullptr;
-    int cap_blob = 0;
-    double *h_blob = nullptr;  // pinned
-    int cap_hblob = 0;
+    DeviceBuffer<double> d_blob;
+    PinnedBuffer<double> h_blob;
     BlobLayout layout{};
     int traj_N = 0;
     double traj_D = 0.0;
-    int occ_N = -1, occ_blob = -1, occ_outer = 2, occ_gsip = 2;  // cached occupancy query
-    int occ_scaled = -1;          // which kernels (rigid 0 / scaled 1) the cached occupancy belongs to
+    std::map<std::tuple<int, int, int>, Occupancy> occ_cache;  // (N, blob doubles, scaled) -> resident CTAs per SM
     // deformable robot (svsdf_set_scale): the scaled kernels run with this schedule
     bool scaled = false;
     ScaleSched sched{};
     int64_t last_n_inside = -1;  // interior points seen by the previous cost evaluation (picks the k_gsip variant)
     // reduction
-    double *d_partials = nullptr;
-    int64_t cap_partials = 0;
-    double *d_out = nullptr;  // 1 + 19N + 1
-    double *d_tot = nullptr;  // 19N + 1 (finalize scratch)
-    unsigned int *d_ticket = nullptr;
-    double *h_out = nullptr;  // pinned
-    int cap_out = 0;
+    DeviceBuffer<double> d_partials;
+    DeviceBuffer<double> d_out;  // 1 + 19N + 1
+    DeviceBuffer<double> d_tot;  // 19N + 1 (finalize scratch)
+    DeviceBuffer<unsigned int> d_ticket;
+    PinnedBuffer<double> h_out;
     // query scratch (per-point outputs)
-    double *d_q_points = nullptr, *d_q_sdf = nullptr, *d_q_ts = nullptr, *d_q_grad = nullptr;
-    int *d_q_rounds = nullptr;
-    int64_t cap_q = 0;
-    double *h_stage = nullptr;  // pinned staging for results download and the small uploads of the other entry points
-    size_t cap_stage = 0;
+    DeviceBuffer<double> d_q_points, d_q_sdf, d_q_ts, d_q_grad;
+    DeviceBuffer<int> d_q_rounds;
+    PinnedBuffer<unsigned char> h_stage;  // staging for results download and the small uploads of the other entry points
     // svsdf_set_points has its own pinned stage and does NOT wait for its copies: the kernels that follow are ordered behind them
     // on the context's stream, and the host goes on (builds the trajectory blob) while the DMA runs.  ev_pts marks the end of the
     // last upload: the next svsdf_set_points (which overwrites the stage) and svsdf_device_ptr_points (which hands the buffer to
     // other streams) wait on it.
     svsdf_lmbm *lmbm = nullptr;          // svsdf_set_lmbm_library: this context's private instance of the reference's LMBM
     svsdf_lmbm_params lmbm_params;
-    double *h_pts_stage = nullptr;
-    size_t cap_pts_stage = 0;
+    PinnedBuffer<double> h_pts_stage;
     cudaEvent_t ev_pts = nullptr;
     bool pts_inflight = false;
 
     // packed map kernel (K3)
-    unsigned char *d_map = nullptr;
-    bool own_map = true;
-    size_t cap_map = 0;
+    // the caller's block (svsdf_set_map_device) when one is set, else map_buf
+    DeviceBuffer<unsigned char> map_buf;
+    const unsigned char *map_ext = nullptr;
+    const unsigned char *map() const { return map_ext ? map_ext : map_buf.get(); }
     int map_X = 0, map_Y = 0, map_h = 0, map_row_bytes = 0;
     int map_Z = 1;             // z layers held on the device (svsdf_set_map3d), each in the 2-D layout; layer 0 first
     double map_ox = 0, map_oy = 0, map_oz = 0, map_res = 0;
-    int *d_block_counts = nullptr;
-    int cap_block_counts = 0;
-    int64_t *d_n_total = nullptr;
+    DeviceBuffer<int> d_block_counts;
+    DeviceBuffer<int64_t> d_n_total;
 
     // optimiser state (R3/R4)
     HostEval he;
@@ -204,24 +258,18 @@ struct svsdf_ctx {
     // CTA runs every search on the same slot); -1 = not set
     int force_grid_astar = -1;
     // svsdf_cost_grad_multi / svsdf_optimize_lockstep: packed inputs (one pinned stage mirrored by one device block, one copy in),
-    // grow-only scratch, pinned outputs (one copy out)
-    unsigned char *h_multi_in = nullptr, *d_multi_in = nullptr;
-    size_t cap_multi_in = 0;
-    unsigned char *d_multi_scratch = nullptr;
-    size_t cap_multi_scratch = 0;
-    double *h_multi_out = nullptr;
-    size_t cap_multi_out = 0;
-    unsigned int *d_multi_tickets = nullptr;  // [0] k_compact_multi's, [1 + k] problem k's k_finalize_multi ticket; zero between calls
-    int cap_multi_tickets = 0;
+    // scratch, pinned outputs (one copy out)
+    PinnedBuffer<unsigned char> h_multi_in;
+    DeviceBuffer<unsigned char> d_multi_in;
+    DeviceBuffer<unsigned char> d_multi_scratch;
+    PinnedBuffer<double> h_multi_out;
+    DeviceBuffer<unsigned int> d_multi_tickets;  // [0] k_compact_multi's, [1 + k] problem k's k_finalize_multi ticket; zero between calls
     int64_t multi_last_inside = -1;  // inside points of the previous multi evaluation (picks the k_gsip_multi variant)
-    std::map<std::tuple<int, int, int>, int> occ_cache;  // (N, blob doubles, scaled) -> resident single-problem k_outer CTAs per SM
     int64_t lockstep_rounds = 0;  // rounds of the last svsdf_optimize_lockstep
-    // svsdf_swept_contour: grow-only device buffers (per corner, per needed corner, per CTA, outputs) and the samples' upload
-    unsigned char *d_sw_corner = nullptr, *d_sw_point = nullptr, *d_sw_small = nullptr, *d_sw_out = nullptr;
-    size_t cap_sw_corner = 0, cap_sw_point = 0, cap_sw_small = 0, cap_sw_out = 0;
-    // svsdf_map_clearance: grow-only device buffers (header, samples and per-CTA counts; band bits per map word; band cells)
-    unsigned char *d_cl_small = nullptr, *d_cl_band = nullptr, *d_cl_point = nullptr;
-    size_t cap_cl_small = 0, cap_cl_band = 0, cap_cl_point = 0;
+    // svsdf_swept_contour: device buffers (per corner, per needed corner, per CTA, outputs) and the samples' upload
+    DeviceBuffer<unsigned char> d_sw_corner, d_sw_point, d_sw_small, d_sw_out;
+    // svsdf_map_clearance: device buffers (header, samples and per-CTA counts; band bits per map word; band cells)
+    DeviceBuffer<unsigned char> d_cl_small, d_cl_band, d_cl_point;
 };
 
 namespace {
@@ -234,6 +282,30 @@ namespace {
             return SVSDF_ERR_CUDA;                                                                 \
         }                                                                                          \
     } while (0)
+
+// The launchers of one kernel variant, kKernels[strict][scaled]: FMA contraction or not (-fmad=false, the reference's rounding), rigid
+// or deformable robot.  The scaled variants share the rigid units' pose table, finalize, shape evaluation and multi-problem helpers.
+struct Kernels {
+    decltype(&fast::query_occupancy) query_occupancy;
+    decltype(&fast::launch_cost_kernels) cost_kernels;
+    decltype(&fast::launch_pose_table) pose_table;
+    decltype(&fast::launch_finalize) finalize;
+    decltype(&fast::launch_shape_eval) shape_eval;
+    decltype(&fast::launch_sincos) sincos;
+    decltype(&fast_multi::launch_multi) multi;
+    decltype(&fast_multi::launch_pose_multi) pose_multi;
+    decltype(&fast_multi::launch_compact_multi) compact_multi;
+    decltype(&fast_multi::launch_finalize_multi) finalize_multi;
+};
+#define SVSDF_VARIANT(NS, SCALED)                                                                                      \
+    {NS##SCALED::query_occupancy,  NS##SCALED::launch_cost_kernels, NS::launch_pose_table,                            \
+     NS::launch_finalize,          NS::launch_shape_eval,           NS::launch_sincos,                                \
+     NS##_multi##SCALED::launch_multi, NS##_multi::launch_pose_multi, NS##_multi::launch_compact_multi,              \
+     NS##_multi::launch_finalize_multi}
+const Kernels kKernels[2][2] = {{SVSDF_VARIANT(fast, ), SVSDF_VARIANT(fast, _scaled)}, {SVSDF_VARIANT(strict, ), SVSDF_VARIANT(strict, _scaled)}};
+#undef SVSDF_VARIANT
+
+const Kernels &kernels(const svsdf_ctx *ctx) { return kKernels[ctx->strict][ctx->scaled]; }
 
 const char *kShapeNames[] = {"star",      "sdHorseshoe", "sdPie",      "sdPie2", "sdArc",          "sdTunnel",
                              "sdCutDisk", "sdTrapezoid", "sdRhombus",  "sdHeart", "sdRoundedX",    "bigX",
@@ -336,39 +408,18 @@ void build_shape(const svsdf_config &cfg, ShapeParams &S) {
 }
 
 int ensure_scratch(svsdf_ctx *ctx, int64_t P) {
-    if (P <= ctx->cap_scratch) return SVSDF_OK;
-    cudaFree(ctx->d_flag); cudaFree(ctx->d_inside_tstar); cudaFree(ctx->d_inside_list);
-    cudaFree(ctx->d_gsip_contrib); cudaFree(ctx->d_gsip_piece);
-    ctx->d_flag = nullptr; ctx->d_inside_tstar = nullptr; ctx->d_inside_list = nullptr;
-    ctx->d_gsip_contrib = nullptr; ctx->d_gsip_piece = nullptr;
-    ctx->cap_scratch = 0;
-    int64_t cap = P + P / 8 + 1024;
-    CK(cudaMalloc(&ctx->d_flag, cap));
-    CK(cudaMalloc(&ctx->d_inside_tstar, cap * sizeof(double)));
-    CK(cudaMalloc(&ctx->d_inside_list, cap * sizeof(int)));
-    CK(cudaMalloc(&ctx->d_gsip_contrib, cap * 20 * sizeof(double)));
-    CK(cudaMalloc(&ctx->d_gsip_piece, cap * sizeof(int)));
-    ctx->cap_scratch = cap;
-    return SVSDF_OK;
-}
-
-int ensure_stage(svsdf_ctx *ctx, size_t bytes) {
-    if (bytes <= ctx->cap_stage) return SVSDF_OK;
-    if (ctx->h_stage) cudaFreeHost(ctx->h_stage);
-    ctx->h_stage = nullptr;
-    ctx->cap_stage = 0;
-    size_t cap = bytes + bytes / 4 + 4096;
-    CK(cudaMallocHost(&ctx->h_stage, cap));
-    ctx->cap_stage = cap;
+    CK(ctx->d_flag.reserve(P));
+    CK(ctx->d_inside_tstar.reserve(P));
+    CK(ctx->d_inside_list.reserve(P));
+    CK(ctx->d_gsip_contrib.reserve((size_t)P * 20));
+    CK(ctx->d_gsip_piece.reserve(P));
     return SVSDF_OK;
 }
 
 // updateTraj (sw_manager.hpp:376-385) + the layer-1 lattice of choiceTInit (:538-581): builds the blob in
 // pinned memory, uploads it and launches the pose-table kernel.
 int pose_table(svsdf_ctx *ctx) {
-    cudaError_t e = ctx->strict ? strict::launch_pose_table(ctx->d_blob, ctx->layout.K1, ctx->stream)
-                                : fast::launch_pose_table(ctx->d_blob, ctx->layout.K1, ctx->stream);
-    CK(e);
+    CK(kernels(ctx).pose_table(ctx->d_blob, ctx->layout.K1, ctx->stream));
     ctx->launches += 1;
     return SVSDF_OK;
 }
@@ -426,20 +477,8 @@ int upload_traj(svsdf_ctx *ctx, int N, const double *T, const double *coeffs, bo
         ctx->err = msg;
         return SVSDF_ERR_INVALID;
     }
-    if (L.total > ctx->cap_hblob) {
-        if (ctx->h_blob) cudaFreeHost(ctx->h_blob);
-        ctx->h_blob = nullptr;
-        ctx->cap_hblob = 0;
-        CK(cudaMallocHost(&ctx->h_blob, (size_t)(L.total + 1024) * sizeof(double)));
-        ctx->cap_hblob = L.total + 1024;
-    }
-    if (L.total > ctx->cap_blob) {
-        cudaFree(ctx->d_blob);
-        ctx->d_blob = nullptr;
-        ctx->cap_blob = 0;
-        CK(cudaMalloc(&ctx->d_blob, (size_t)(L.total + 1024) * sizeof(double)));
-        ctx->cap_blob = L.total + 1024;
-    }
+    CK(ctx->h_blob.reserve(L.total));
+    CK(ctx->d_blob.reserve(L.total));
     double *h = ctx->h_blob;
     fill_blob(h, L, T, coeffs, D);
     CK(cudaMemcpyAsync(ctx->d_blob, h, (size_t)L.off_pose * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
@@ -447,24 +486,6 @@ int upload_traj(svsdf_ctx *ctx, int N, const double *T, const double *coeffs, bo
     ctx->traj_N = N;
     ctx->traj_D = D;
     if (launch_pose) return pose_table(ctx);
-    return SVSDF_OK;
-}
-
-int refresh_occupancy(svsdf_ctx *ctx) {
-    const int sc = ctx->scaled ? 1 : 0;
-    if (ctx->occ_N == ctx->traj_N && ctx->occ_blob == ctx->layout.total && ctx->occ_scaled == sc) return SVSDF_OK;
-    int oo = 0, og = 0;
-    const int N = ctx->traj_N, nb = ctx->layout.total;
-    cudaError_t e;
-    if (sc) e = ctx->strict ? strict_scaled::query_occupancy(ctx->shape, N, nb, &oo, &og)
-                            : fast_scaled::query_occupancy(ctx->shape, N, nb, &oo, &og);
-    else e = ctx->strict ? strict::query_occupancy(ctx->shape, N, nb, &oo, &og) : fast::query_occupancy(ctx->shape, N, nb, &oo, &og);
-    CK(e);
-    ctx->occ_outer = oo > 0 ? oo : 1;
-    ctx->occ_gsip = og > 0 ? og : 1;
-    ctx->occ_N = ctx->traj_N;
-    ctx->occ_blob = ctx->layout.total;
-    ctx->occ_scaled = sc;
     return SVSDF_OK;
 }
 
@@ -507,13 +528,49 @@ bool scale_valid(const svsdf_scale &z) {
     return true;
 }
 
-int grid_for(const svsdf_ctx *ctx, int64_t P) {
-    // one warp per point, 8 warps per CTA, warp-stride loop.  The grid is exactly one full wave (SMs x resident CTAs
-    // per SM, from the occupancy query): a larger grid would run a partially filled second wave.
+// Resident CTAs per SM of the single-problem k_outer and k_gsip for a trajectory of N pieces and `blob` doubles: the grids are sized
+// as SMs x occupancy so that the warp-stride loops run as exactly one full wave (no partial second wave).
+int occupancy(svsdf_ctx *ctx, int N, int blob, Occupancy *occ) {
+    const auto key = std::make_tuple(N, blob, ctx->scaled ? 1 : 0);
+    auto it = ctx->occ_cache.find(key);
+    if (it == ctx->occ_cache.end()) {
+        int oo = 0, og = 0;
+        CK(kernels(ctx).query_occupancy(ctx->shape, N, blob, &oo, &og));
+        it = ctx->occ_cache.emplace(key, Occupancy{oo > 0 ? oo : 1, og > 0 ? og : 1}).first;
+    }
+    *occ = it->second;
+    return SVSDF_OK;
+}
+
+// k_outer's launch for P points, shared by svsdf_cost_grad and every problem of svsdf_cost_grad_multi (which is what gives a multi
+// problem the bits of its single call).  One warp per point, 8 warps per CTA, warp-stride loop; the grid is at most one full wave.
+// The batched schedule pays off once every warp owns a couple of dozen points; small problems keep one point per warp.
+struct OuterPlan {
+    int grid, batched;
+};
+OuterPlan outer_plan(const svsdf_ctx *ctx, int64_t P, const Occupancy &occ) {
     int64_t need = (P + kWarpsPerBlock - 1) / kWarpsPerBlock;
-    int64_t cap = (int64_t)ctx->sm_count * ctx->occ_outer;
+    const int64_t cap = (int64_t)ctx->sm_count * occ.outer;
     if (need < 1) need = 1;
-    return (int)(need < cap ? need : cap);
+    OuterPlan plan;
+    plan.grid = (int)(need < cap ? need : cap);
+    if (ctx->force_grid_outer > 0) plan.grid = ctx->force_grid_outer;  // test hook
+    plan.batched = (P >= (int64_t)16 * plan.grid * kWarpsPerBlock) ? 1 : 0;
+    if (ctx->force_batched >= 0) plan.batched = ctx->force_batched;  // test hook
+    return plan;
+}
+
+// k_gsip's variant from the interior points of the previous evaluation (-1: none): few -> 22-warp CTAs (one warp per ring sample,
+// lower latency; the variant does not change the bits, tests/test_gpu_gsip.py).  grid: the test hook's, or 0 for one full wave.
+struct GsipPlan {
+    int wide, grid;
+};
+GsipPlan gsip_plan(const svsdf_ctx *ctx, int64_t prev_inside) {
+    GsipPlan plan;
+    plan.wide = (prev_inside >= 0 && prev_inside <= ctx->sm_count) ? 1 : 0;
+    if (ctx->force_gsip_wide >= 0) plan.wide = ctx->force_gsip_wide ? 1 : 0;  // test hook
+    plan.grid = ctx->force_grid_gsip > 0 ? ctx->force_grid_gsip : 0;        // test hook
+    return plan;
 }
 
 // Runs K1 (+compact, K2) (+finalize).  Inputs resident on the device.
@@ -522,31 +579,17 @@ int run_kernels(svsdf_ctx *ctx, const double *d_points, int64_t P, bool reduce, 
     const int N = ctx->traj_N;
     int rc = ensure_scratch(ctx, P);
     if (rc) return rc;
-    rc = refresh_occupancy(ctx);
+    Occupancy occ;
+    rc = occupancy(ctx, N, ctx->layout.total, &occ);
     if (rc) return rc;
-    int grid = grid_for(ctx, P);
-    if (ctx->force_grid_outer > 0) grid = ctx->force_grid_outer;  // test hook
+    const OuterPlan plan = outer_plan(ctx, P, occ);
+    const int grid = plan.grid;
     const int nacc = 19 * N + 1;
     if (reduce) {
-        int64_t need = (int64_t)grid * nacc;
-        if (need > ctx->cap_partials) {
-            cudaFree(ctx->d_partials);
-            ctx->d_partials = nullptr;
-            ctx->cap_partials = 0;
-            CK(cudaMalloc(&ctx->d_partials, (size_t)(need + 4096) * sizeof(double)));
-            ctx->cap_partials = need + 4096;
-        }
-        if (nacc + 1 > ctx->cap_out) {
-            cudaFree(ctx->d_out);
-            if (ctx->h_out) cudaFreeHost(ctx->h_out);
-            ctx->d_out = nullptr; ctx->h_out = nullptr; ctx->cap_out = 0;
-            CK(cudaMalloc(&ctx->d_out, (size_t)(nacc + 64) * sizeof(double)));
-            cudaFree(ctx->d_tot);
-            ctx->d_tot = nullptr;
-            CK(cudaMalloc(&ctx->d_tot, (size_t)(nacc + 64) * sizeof(double)));
-            CK(cudaMallocHost(&ctx->h_out, (size_t)(nacc + 64) * sizeof(double)));
-            ctx->cap_out = nacc + 64;
-        }
+        CK(ctx->d_partials.reserve((size_t)grid * nacc));
+        CK(ctx->d_out.reserve(nacc + 1));
+        CK(ctx->d_tot.reserve(nacc + 1));
+        CK(ctx->h_out.reserve(nacc + 1));
     }
     KernelArgs A;
     std::memset(&A, 0, sizeof(A));
@@ -559,21 +602,16 @@ int run_kernels(svsdf_ctx *ctx, const double *d_points, int64_t P, bool reduce, 
     A.partials = ctx->d_partials;
     A.want_reduce = reduce ? 1 : 0;
     A.want_gsip = gsip ? 1 : 0;
-    // batched path pays off once every warp owns a couple of dozen points; small problems keep one point per warp
-    A.batched = (P >= (int64_t)16 * grid * kWarpsPerBlock) ? 1 : 0;
-    if (ctx->force_batched >= 0) A.batched = ctx->force_batched;  // test hook
+    A.batched = plan.batched;
     A.inside_flag = ctx->d_flag;
     A.inside_tstar = ctx->d_inside_tstar;
     A.inside_list = ctx->d_inside_list;
     A.n_inside = ctx->d_n_inside;
     A.gsip_contrib = ctx->d_gsip_contrib;
     A.gsip_piece = ctx->d_gsip_piece;
-    A.eval_counter = ctx->count_evals ? ctx->d_eval_counter : nullptr;
-    // previous evaluation had few interior points -> 22-warp CTAs (one warp per ring sample, lower latency)
-    int gsip_wide = (reduce && ctx->last_n_inside >= 0 && ctx->last_n_inside <= ctx->sm_count) ? 1 : 0;
-    if (ctx->force_gsip_wide >= 0) gsip_wide = ctx->force_gsip_wide ? 1 : 0;  // test hook
-    int grid_gsip = gsip_wide ? ctx->sm_count : ctx->sm_count * ctx->occ_gsip;
-    if (ctx->force_grid_gsip > 0) grid_gsip = ctx->force_grid_gsip;  // test hook
+    A.eval_counter = ctx->count_evals ? ctx->d_eval_counter.get() : nullptr;
+    GsipPlan gp = gsip_plan(ctx, reduce ? ctx->last_n_inside : -1);
+    if (gp.grid == 0) gp.grid = gp.wide ? ctx->sm_count : ctx->sm_count * occ.gsip;
     if (!gsip) CK(cudaMemsetAsync(ctx->d_n_inside, 0, sizeof(int), ctx->stream));
     size_t smem = outer_smem_doubles(A.blob_doubles, N) * sizeof(double);
     if (smem > 200 * 1024) {
@@ -581,22 +619,13 @@ int run_kernels(svsdf_ctx *ctx, const double *d_points, int64_t P, bool reduce, 
         return SVSDF_ERR_INVALID;
     }
     cudaEvent_t mark = ctx->mark_kernels ? ctx->evk[2] : nullptr;
-    cudaError_t e;
-    if (ctx->scaled)
-        e = ctx->strict ? strict_scaled::launch_cost_kernels(A, ctx->shape, ctx->sched, N, grid, grid_gsip, ctx->stream, mark, gsip_wide)
-                        : fast_scaled::launch_cost_kernels(A, ctx->shape, ctx->sched, N, grid, grid_gsip, ctx->stream, mark, gsip_wide);
-    else
-        e = ctx->strict ? strict::launch_cost_kernels(A, ctx->shape, N, grid, grid_gsip, ctx->stream, mark, gsip_wide)
-                        : fast::launch_cost_kernels(A, ctx->shape, N, grid, grid_gsip, ctx->stream, mark, gsip_wide);
-    CK(e);
+    const Kernels &K = kernels(ctx);
+    CK(K.cost_kernels(A, ctx->shape, ctx->scaled ? &ctx->sched : nullptr, N, grid, gp.grid, ctx->stream, mark, gp.wide));
     ctx->launches += gsip ? 3 : 1;
     if (ctx->mark_kernels) CK(cudaEventRecord(ctx->evk[3], ctx->stream));
     if (reduce) {
-        e = ctx->strict ? strict::launch_finalize(ctx->d_partials, grid, N, ctx->d_n_inside, ctx->d_gsip_contrib,
-                                                  ctx->d_gsip_piece, ctx->d_tot, ctx->d_ticket, ctx->d_out, ctx->stream)
-                        : fast::launch_finalize(ctx->d_partials, grid, N, ctx->d_n_inside, ctx->d_gsip_contrib,
-                                                ctx->d_gsip_piece, ctx->d_tot, ctx->d_ticket, ctx->d_out, ctx->stream);
-        CK(e);
+        CK(K.finalize(ctx->d_partials, grid, N, ctx->d_n_inside, ctx->d_gsip_contrib, ctx->d_gsip_piece, ctx->d_tot, ctx->d_ticket,
+                      ctx->d_out, ctx->stream));
         ctx->launches += 1;
     }
     return SVSDF_OK;
@@ -604,14 +633,14 @@ int run_kernels(svsdf_ctx *ctx, const double *d_points, int64_t P, bool reduce, 
 
 // R1 on the context's points; result (1 + 19N + 1 doubles) lands in ctx->h_out after the stream sync.
 int cost_grad_raw(svsdf_ctx *ctx, int N, const double *T, const double *coeffs) {
-    if (!ctx->d_points || ctx->P < 0) {
+    if (!ctx->points() || ctx->P < 0) {
         ctx->err = "svsdf: query points not set";
         return SVSDF_ERR_NOT_READY;
     }
     int rc = upload_traj(ctx, N, T, coeffs);
     if (rc) return rc;
     if (ctx->time_kernels) CK(cudaEventRecord(ctx->ev0, ctx->stream));
-    rc = run_kernels(ctx, ctx->d_points, ctx->P, true, true, nullptr, nullptr, nullptr, nullptr);
+    rc = run_kernels(ctx, ctx->points(), ctx->P, true, true, nullptr, nullptr, nullptr, nullptr);
     if (rc) return rc;
     if (ctx->time_kernels) CK(cudaEventRecord(ctx->ev1, ctx->stream));
     const int nout = 1 + 19 * N + 1;
@@ -657,37 +686,7 @@ struct MultiItem {
     int rc = SVSDF_OK;
 };
 
-// Resident CTAs per SM of the SINGLE-problem k_outer for this trajectory size: problem k's virtual grid is the grid svsdf_cost_grad
-// would launch for it.
-int single_outer_occupancy(svsdf_ctx *ctx, int N, int blob, int *occ) {
-    const int sc = ctx->scaled ? 1 : 0;
-    const auto key = std::make_tuple(N, blob, sc);
-    auto it = ctx->occ_cache.find(key);
-    if (it != ctx->occ_cache.end()) { *occ = it->second; return SVSDF_OK; }
-    int oo = 0, og = 0;
-    cudaError_t e;
-    if (sc) e = ctx->strict ? strict_scaled::query_occupancy(ctx->shape, N, blob, &oo, &og) : fast_scaled::query_occupancy(ctx->shape, N, blob, &oo, &og);
-    else e = ctx->strict ? strict::query_occupancy(ctx->shape, N, blob, &oo, &og) : fast::query_occupancy(ctx->shape, N, blob, &oo, &og);
-    CK(e);
-    *occ = oo > 0 ? oo : 1;
-    ctx->occ_cache[key] = *occ;
-    return SVSDF_OK;
-}
-
 size_t align16(size_t b) { return (b + 15) & ~(size_t)15; }
-
-// Sizes a grow-only device buffer.
-template <class T>
-int grow_device(svsdf_ctx *ctx, T *&p, size_t &cap, size_t bytes) {
-    if (bytes <= cap) return SVSDF_OK;
-    cudaFree(p);
-    p = nullptr;
-    cap = 0;
-    const size_t c = bytes + bytes / 4 + 4096;
-    CK(cudaMalloc(&p, c));
-    cap = c;
-    return SVSDF_OK;
-}
 
 // One cost + gradient evaluation of every item with rc == SVSDF_OK, in one set of launches.  Items whose trajectory or points are
 // invalid get rc = SVSDF_ERR_INVALID and take no part; a CUDA error fails the call (and every item).  *ms: device time of the launches.
@@ -712,16 +711,12 @@ int run_multi(svsdf_ctx *ctx, MultiItem *items, int n, float *ms) {
             it.rc = SVSDF_ERR_INVALID;
             continue;
         }
-        int occ = 1;
-        int rc = single_outer_occupancy(ctx, it.N, L.total, &occ);
+        // problem k's virtual grid is the grid svsdf_cost_grad would launch for it
+        Occupancy occ;
+        int rc = occupancy(ctx, it.N, L.total, &occ);
         if (rc) return rc;
-        // grid_for with that occupancy, and the single call's test hooks
-        int64_t need = (it.P + kWarpsPerBlock - 1) / kWarpsPerBlock, cap = (int64_t)ctx->sm_count * occ;
-        if (need < 1) need = 1;
-        int G = (int)(need < cap ? need : cap);
-        if (ctx->force_grid_outer > 0) G = ctx->force_grid_outer;
-        int batched = (it.P >= (int64_t)16 * G * kWarpsPerBlock) ? 1 : 0;
-        if (ctx->force_batched >= 0) batched = ctx->force_batched;
+        const OuterPlan plan = outer_plan(ctx, it.P, occ);
+        const int G = plan.grid, batched = plan.batched;
         MultiProblem m;
         m.blob_off = blob_tot; m.pt_off = pt_tot; m.flag_off = flag_tot; m.part_off = part_tot; m.out_off = out_tot;
         m.P = it.P; m.blob_doubles = L.total; m.N = it.N; m.K1 = L.K1; m.grid = G;
@@ -753,15 +748,8 @@ int run_multi(svsdf_ctx *ctx, MultiItem *items, int n, float *ms) {
     const size_t o_prob = 0, o_ms = align16(o_prob + m * sizeof(MultiProblem)), o_mb = align16(o_ms + map_s.size() * sizeof(int)),
                  o_blob = align16(o_mb + map_b.size() * sizeof(int)), o_pts = align16(o_blob + (size_t)blob_tot * 8),
                  in_bytes = align16(o_pts + (size_t)pt_tot * 16);
-    if (in_bytes > ctx->cap_multi_in) {
-        if (ctx->h_multi_in) cudaFreeHost(ctx->h_multi_in);
-        cudaFree(ctx->d_multi_in);
-        ctx->h_multi_in = nullptr; ctx->d_multi_in = nullptr; ctx->cap_multi_in = 0;
-        const size_t c = in_bytes + in_bytes / 4 + 4096;
-        CK(cudaMallocHost(&ctx->h_multi_in, c));
-        CK(cudaMalloc(&ctx->d_multi_in, c));
-        ctx->cap_multi_in = c;
-    }
+    CK(ctx->h_multi_in.reserve(in_bytes));
+    CK(ctx->d_multi_in.reserve(in_bytes));
     // the previous call's copy has completed (every call ends with a stream synchronise)
     unsigned char *h = ctx->h_multi_in, *d = ctx->d_multi_in;
     std::memcpy(h + o_prob, pr.data(), m * sizeof(MultiProblem));
@@ -783,25 +771,12 @@ int run_multi(svsdf_ctx *ctx, MultiItem *items, int n, float *ms) {
                  s_part = align16(s_pc + (size_t)pt_tot * 4), s_out = align16(s_part + (size_t)part_tot * 8),
                  s_tot = align16(s_out + (size_t)out_tot * 8), s_cnt = align16(s_tot + (size_t)out_tot * 8), s_off = align16(s_cnt + (size_t)m * 4),
                  s_bytes = align16(s_off + (size_t)(m + 1) * 4);
-    int rc = grow_device(ctx, ctx->d_multi_scratch, ctx->cap_multi_scratch, s_bytes);
-    if (rc) return rc;
-    if (m + 1 > ctx->cap_multi_tickets) {
-        cudaFree(ctx->d_multi_tickets);
-        ctx->d_multi_tickets = nullptr;
-        ctx->cap_multi_tickets = 0;
-        const int c = m + 1 + 1024;
-        CK(cudaMalloc(&ctx->d_multi_tickets, (size_t)c * sizeof(unsigned int)));
-        CK(cudaMemsetAsync(ctx->d_multi_tickets, 0, (size_t)c * sizeof(unsigned int), ctx->stream));
-        ctx->cap_multi_tickets = c;
+    CK(ctx->d_multi_scratch.reserve(s_bytes));
+    if ((size_t)m + 1 > ctx->d_multi_tickets.capacity()) {  // a new block: its tickets start at zero
+        CK(ctx->d_multi_tickets.reserve(m + 1));
+        CK(cudaMemsetAsync(ctx->d_multi_tickets, 0, ctx->d_multi_tickets.capacity() * sizeof(unsigned int), ctx->stream));
     }
-    if ((size_t)out_tot * 8 > ctx->cap_multi_out) {
-        if (ctx->h_multi_out) cudaFreeHost(ctx->h_multi_out);
-        ctx->h_multi_out = nullptr;
-        ctx->cap_multi_out = 0;
-        const size_t c = (size_t)out_tot * 8 + (size_t)out_tot * 2 + 4096;
-        CK(cudaMallocHost(&ctx->h_multi_out, c));
-        ctx->cap_multi_out = c;
-    }
+    CK(ctx->h_multi_out.reserve(out_tot));
     unsigned char *sc = ctx->d_multi_scratch;
     KernelArgs A;
     std::memset(&A, 0, sizeof(A));
@@ -816,7 +791,7 @@ int run_multi(svsdf_ctx *ctx, MultiItem *items, int n, float *ms) {
     A.inside_list = reinterpret_cast<int *>(sc + s_list);
     A.gsip_contrib = reinterpret_cast<double *>(sc + s_con);
     A.gsip_piece = reinterpret_cast<int *>(sc + s_pc);
-    A.eval_counter = ctx->count_evals ? ctx->d_eval_counter : nullptr;
+    A.eval_counter = ctx->count_evals ? ctx->d_eval_counter.get() : nullptr;
     MultiArgs M;
     std::memset(&M, 0, sizeof(M));
     M.n = m;
@@ -828,34 +803,24 @@ int run_multi(svsdf_ctx *ctx, MultiItem *items, int n, float *ms) {
     M.out = reinterpret_cast<double *>(sc + s_out);
     M.tot = reinterpret_cast<double *>(sc + s_tot);
     const ScaleSched *Z = ctx->scaled ? &ctx->sched : nullptr;
-    auto launch = [&](int what, int grid, size_t smem, int wide) -> cudaError_t {
-        if (ctx->scaled)
-            return ctx->strict ? strict_multi_scaled::launch_multi(what, A, M, ctx->shape, Z, grid, smem, wide, ctx->sm_count, ctx->stream)
-                               : fast_multi_scaled::launch_multi(what, A, M, ctx->shape, Z, grid, smem, wide, ctx->sm_count, ctx->stream);
-        return ctx->strict ? strict_multi::launch_multi(what, A, M, ctx->shape, Z, grid, smem, wide, ctx->sm_count, ctx->stream)
-                           : fast_multi::launch_multi(what, A, M, ctx->shape, Z, grid, smem, wide, ctx->sm_count, ctx->stream);
-    };
+    const Kernels &K = kernels(ctx);
     CK(cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, ctx->stream));
     if (ms) CK(cudaEventRecord(ctx->ev0, ctx->stream));
-    double *d_blobs = reinterpret_cast<double *>(d + o_blob);
-    CK(ctx->strict ? strict_multi::launch_pose_multi(d_blobs, M, max_K1, ctx->stream) : fast_multi::launch_pose_multi(d_blobs, M, max_K1, ctx->stream));
+    CK(K.pose_multi(reinterpret_cast<double *>(d + o_blob), M, max_K1, ctx->stream));
     int launches = 1;
     for (int b = 0; b < 2; ++b) {
         const std::vector<int> &mp = b ? map_b : map_s;
         if (mp.empty()) continue;
         M.cta_map = reinterpret_cast<const int *>(d + (b ? o_mb : o_ms));
-        CK(launch(b, (int)(mp.size() / 2), outer_smem_doubles(smax_blob[b], smax_N[b]) * sizeof(double), 0));
+        CK(K.multi(b, A, M, ctx->shape, Z, (int)(mp.size() / 2), outer_smem_doubles(smax_blob[b], smax_N[b]) * sizeof(double), 0,
+                   ctx->sm_count, ctx->stream));
         ++launches;
     }
     M.cta_map = nullptr;
-    CK(ctx->strict ? strict_multi::launch_compact_multi(A.inside_flag, A.inside_list, M, ctx->stream)
-                   : fast_multi::launch_compact_multi(A.inside_flag, A.inside_list, M, ctx->stream));
-    // few inside points in the previous round: 22-warp CTAs (the variant does not change the bits, tests/test_gpu_gsip.py)
-    int wide = (ctx->multi_last_inside >= 0 && ctx->multi_last_inside <= ctx->sm_count) ? 1 : 0;
-    if (ctx->force_gsip_wide >= 0) wide = ctx->force_gsip_wide ? 1 : 0;
-    CK(launch(2, ctx->force_grid_gsip > 0 ? ctx->force_grid_gsip : 0, (size_t)max_blob * sizeof(double), wide));
-    CK(ctx->strict ? strict_multi::launch_finalize_multi(A.partials, A.gsip_contrib, A.gsip_piece, M, max_N, ctx->stream)
-                   : fast_multi::launch_finalize_multi(A.partials, A.gsip_contrib, A.gsip_piece, M, max_N, ctx->stream));
+    CK(K.compact_multi(A.inside_flag, A.inside_list, M, ctx->stream));
+    const GsipPlan gp = gsip_plan(ctx, ctx->multi_last_inside);
+    CK(K.multi(2, A, M, ctx->shape, Z, gp.grid, (size_t)max_blob * sizeof(double), gp.wide, ctx->sm_count, ctx->stream));
+    CK(K.finalize_multi(A.partials, A.gsip_contrib, A.gsip_piece, M, max_N, ctx->stream));
     launches += 3;
     if (ms) CK(cudaEventRecord(ctx->ev1, ctx->stream));
     CK(cudaMemcpyAsync(ctx->h_multi_out, M.out, (size_t)out_tot * 8, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1141,18 +1106,15 @@ int svsdf_front_init(svsdf_ctx *ctx, int kernel_size, int kernel_yaw_num, double
     int ind = 0;
     for (double yaw = -PI; yaw < PI && ind < kernel_yaw_num; yaw += yaw_res, ind++) ctx->front_yaw[ind] = yaw;  // :401
     const int K = kernel_yaw_num, ks = kernel_size, bpr = (ks + 7) / 8;
-    double *d_yaw = nullptr;
-    unsigned char *d_cells = nullptr;
-    CK(cudaMalloc(&d_yaw, K * sizeof(double)));
-    cudaError_t e = cudaMalloc(&d_cells, (size_t)K * ks * ks);
-    if (e != cudaSuccess) { cudaFree(d_yaw); ctx->err = cudaGetErrorString(e); return SVSDF_ERR_CUDA; }
+    DeviceBuffer<double> d_yaw;
+    DeviceBuffer<unsigned char> d_cells;
+    CK(d_yaw.reserve(K));
+    CK(d_cells.reserve((size_t)K * ks * ks));
     ctx->front_cells.assign((size_t)K * ks * ks, 0);
-    e = cudaMemcpyAsync(d_yaw, ctx->front_yaw.data(), K * sizeof(double), cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess) e = launch_front_cells(ctx->shape, F, d_yaw, d_cells, ctx->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(ctx->front_cells.data(), d_cells, ctx->front_cells.size(), cudaMemcpyDeviceToHost, ctx->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    cudaFree(d_yaw); cudaFree(d_cells);
-    if (e != cudaSuccess) { ctx->err = std::string("svsdf_front_init: ") + cudaGetErrorString(e); return SVSDF_ERR_CUDA; }
+    CK(cudaMemcpyAsync(d_yaw, ctx->front_yaw.data(), K * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    CK(launch_front_cells(ctx->shape, F, d_yaw, d_cells, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->front_cells.data(), d_cells, ctx->front_cells.size(), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
     ctx->launches += 1;
     // generateByteKernel (Shape.hpp:194-216) + the same rows as 32-bit masks (bit 31 - b <-> column b)
     static const unsigned char or_mask[8] = {0x80, 0x40, 0x20, 0x10, 0x08, 0x04, 0x02, 0x01};
@@ -1165,10 +1127,8 @@ int svsdf_front_init(svsdf_ctx *ctx, int kernel_size, int kernel_yaw_num, double
                     ctx->front_bytes[((size_t)k * ks + a) * bpr + b / 8] |= or_mask[b % 8];
                     rowmask[(size_t)k * ks + a] |= 0x80000000u >> b;
                 }
-    cudaFree(ctx->d_front_bytes); cudaFree(ctx->d_front_rowmask);
-    ctx->d_front_bytes = nullptr; ctx->d_front_rowmask = nullptr;
-    CK(cudaMalloc(&ctx->d_front_bytes, ctx->front_bytes.size()));
-    CK(cudaMalloc(&ctx->d_front_rowmask, rowmask.size() * sizeof(unsigned)));
+    CK(ctx->d_front_bytes.reserve(ctx->front_bytes.size()));
+    CK(ctx->d_front_rowmask.reserve(rowmask.size()));
     CK(cudaMemcpy(ctx->d_front_bytes, ctx->front_bytes.data(), ctx->front_bytes.size(), cudaMemcpyHostToDevice));
     CK(cudaMemcpy(ctx->d_front_rowmask, rowmask.data(), rowmask.size() * sizeof(unsigned), cudaMemcpyHostToDevice));
     ctx->front = F;
@@ -1185,20 +1145,9 @@ int svsdf_front_get_kernels(svsdf_ctx *ctx, double *yaw_out, unsigned char *cell
     return SVSDF_OK;
 }
 
-static int front_scratch(svsdf_ctx *ctx, size_t bytes) {
-    if (bytes <= ctx->cap_front_scratch) return SVSDF_OK;
-    cudaFree(ctx->d_front_scratch);
-    ctx->d_front_scratch = nullptr;
-    ctx->cap_front_scratch = 0;
-    const size_t cap = bytes + bytes / 2 + 4096;
-    CK(cudaMalloc(&ctx->d_front_scratch, cap));
-    ctx->cap_front_scratch = cap;
-    return SVSDF_OK;
-}
-
 static int front_params_with_map(svsdf_ctx *ctx, FrontParams &F, const char *who) {
     if (!ctx->front_ready) { ctx->err = std::string(who) + ": call svsdf_front_init first"; return SVSDF_ERR_NOT_READY; }
-    if (!ctx->d_map) { ctx->err = std::string(who) + ": map not set (svsdf_set_map)"; return SVSDF_ERR_NOT_READY; }
+    if (!ctx->map()) { ctx->err = std::string(who) + ": map not set (svsdf_set_map)"; return SVSDF_ERR_NOT_READY; }
     F = ctx->front;
     F.X = ctx->map_X; F.Y = ctx->map_Y; F.h = ctx->map_h; F.row_bytes = ctx->map_row_bytes;
     F.out_words = (ctx->map_Y + 31) / 32;
@@ -1221,15 +1170,9 @@ int svsdf_front_cspace(svsdf_ctx *ctx, uint32_t *words_out, float *ms_out, const
     if (rc != SVSDF_OK) return rc;
     CK(cudaSetDevice(ctx->device));
     const size_t n = (size_t)F.kernel_count * F.X * F.out_words;
-    if (n > ctx->cap_cspace) {
-        cudaFree(ctx->d_cspace);
-        ctx->d_cspace = nullptr;
-        ctx->cap_cspace = 0;
-        CK(cudaMalloc(&ctx->d_cspace, n * sizeof(unsigned)));
-        ctx->cap_cspace = n;
-    }
+    CK(ctx->d_cspace.reserve(n));
     CK(cudaEventRecord(ctx->ev0, ctx->stream));
-    CK(launch_front_cspace(F, ctx->d_map, ctx->d_front_rowmask, ctx->d_cspace, ctx->stream));
+    CK(launch_front_cspace(F, ctx->map(), ctx->d_front_rowmask, ctx->d_cspace, ctx->stream));
     CK(cudaEventRecord(ctx->ev1, ctx->stream));
     ctx->launches += 1;
     if (words_out) CK(cudaMemcpyAsync(words_out, ctx->d_cspace, n * sizeof(unsigned), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1259,11 +1202,9 @@ int svsdf_front_expand(svsdf_ctx *ctx, int64_t n, const int32_t *node_ij, const 
     // 8 bytes), then inputs (father yaws [n] f64 | node indices [2n] i32) — one copy in, one launch, one copy out.
     const size_t un = (size_t)n;
     const size_t out_bytes = (9 * un * 8 + 18 * un + 7) & ~(size_t)7, in_bytes = un * 8 + 2 * un * 4;
-    rc = front_scratch(ctx, out_bytes + in_bytes + 64);
-    if (rc != SVSDF_OK) return rc;
-    rc = ensure_stage(ctx, out_bytes + in_bytes + 64);
-    if (rc != SVSDF_OK) return rc;
-    unsigned char *hb = reinterpret_cast<unsigned char *>(ctx->h_stage), *db = ctx->d_front_scratch;
+    CK(ctx->d_front_scratch.reserve(out_bytes + in_bytes + 64));
+    CK(ctx->h_stage.reserve(out_bytes + in_bytes + 64));
+    unsigned char *hb = ctx->h_stage, *db = ctx->d_front_scratch;
     double *d_cy = reinterpret_cast<double *>(db);
     unsigned char *d_ok = db + 9 * un * 8, *d_parts = d_ok + 9 * un;
     double *d_fy = reinterpret_cast<double *>(db + out_bytes);
@@ -1271,7 +1212,7 @@ int svsdf_front_expand(svsdf_ctx *ctx, int64_t n, const int32_t *node_ij, const 
     std::memcpy(hb + out_bytes, node_yaw, un * 8);
     std::memcpy(hb + out_bytes + un * 8, node_ij, 2 * un * 4);
     cudaError_t e = cudaMemcpyAsync(db + out_bytes, hb + out_bytes, in_bytes, cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess) e = launch_front_expand(ctx->shape, F, P, ctx->d_map, ctx->d_front_bytes, n, d_ij, d_fy, d_ok, d_cy, d_parts, ctx->stream);
+    if (e == cudaSuccess) e = launch_front_expand(ctx->shape, F, P, ctx->map(), ctx->d_front_bytes, n, d_ij, d_fy, d_ok, d_cy, d_parts, ctx->stream);
     if (e == cudaSuccess) e = cudaMemcpyAsync(hb, db, out_bytes, cudaMemcpyDeviceToHost, ctx->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
     if (e == cudaSuccess) {
@@ -1341,26 +1282,18 @@ int svsdf_front_astar_device(svsdf_ctx *ctx, int n, const double *start_xy, cons
     }
     AstarArgs A{};
     int per_sm = 0;
-    CK(launch_front_astar(ctx->shape, F, P, ctx->d_map, ctx->d_front_bytes, A, 0, &per_sm, ctx->stream));
+    CK(launch_front_astar(ctx->shape, F, P, ctx->map(), ctx->d_front_bytes, A, 0, &per_sm, ctx->stream));
     int64_t grid = ctx->force_grid_astar > 0 ? ctx->force_grid_astar : std::min<int64_t>(n, (int64_t)std::max(per_sm, 1) * ctx->sm_count);
     grid = std::min(grid, fit);
-    if ((size_t)(grid * slot_bytes) > ctx->cap_astar_pool) {
-        cudaFree(ctx->d_astar_pool);
-        ctx->d_astar_pool = nullptr;
-        ctx->cap_astar_pool = 0;
-        CK(cudaMalloc(&ctx->d_astar_pool, (size_t)(grid * slot_bytes)));
-        ctx->cap_astar_pool = (size_t)(grid * slot_bytes);
-    }
+    CK(ctx->d_astar_pool.reserve_exact((size_t)(grid * slot_bytes)));
     // One device block: cells [4n] i32 | len, expansions, status [3n] i32 | counter (padded to 16 bytes) | paths [n][max_path][3] f64.
     // Only the lengths come back first, then at most the longest returned path of every row.
     const size_t cells_bytes = 16 * un, out_bytes = 12 * un, head = (cells_bytes + out_bytes + 16 + 15) & ~(size_t)15;
     const size_t row = (size_t)max_path * 3 * sizeof(double);
-    rc = front_scratch(ctx, head + un * row);
-    if (rc != SVSDF_OK) return rc;
-    rc = ensure_stage(ctx, cells_bytes + out_bytes);
-    if (rc != SVSDF_OK) return rc;
+    CK(ctx->d_front_scratch.reserve(head + un * row));
+    CK(ctx->h_stage.reserve(cells_bytes + out_bytes));
     unsigned char *db = ctx->d_front_scratch;
-    int32_t *hb = reinterpret_cast<int32_t *>(ctx->h_stage);
+    int32_t *hb = reinterpret_cast<int32_t *>(ctx->h_stage.get());
     std::memcpy(hb, cells.data(), cells_bytes);
     A.n = n; A.max_path = max_path; A.max_expansions = max_expansions;
     A.cells = reinterpret_cast<const int *>(db);
@@ -1374,7 +1307,7 @@ int svsdf_front_astar_device(svsdf_ctx *ctx, int n, const double *start_xy, cons
     cudaError_t e = cudaMemcpyAsync(db, hb, cells_bytes, cudaMemcpyHostToDevice, ctx->stream);
     if (e == cudaSuccess) e = cudaMemsetAsync(A.next, 0, sizeof(int), ctx->stream);
     if (e == cudaSuccess) e = cudaEventRecord(ctx->ev0, ctx->stream);
-    if (e == cudaSuccess) e = launch_front_astar(ctx->shape, F, P, ctx->d_map, ctx->d_front_bytes, A, (int)grid, nullptr, ctx->stream);
+    if (e == cudaSuccess) e = launch_front_astar(ctx->shape, F, P, ctx->map(), ctx->d_front_bytes, A, (int)grid, nullptr, ctx->stream);
     if (e == cudaSuccess) e = cudaEventRecord(ctx->ev1, ctx->stream);
     if (e == cudaSuccess) e = cudaMemcpyAsync(hb, A.len, out_bytes, cudaMemcpyDeviceToHost, ctx->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
@@ -1405,15 +1338,14 @@ int svsdf_front_check_kernel_value(svsdf_ctx *ctx, int64_t n, const double *fath
         }
     CK(cudaSetDevice(ctx->device));
     const size_t un = (size_t)n;
-    rc = front_scratch(ctx, un * 8 + un * 8 + 2 * un * 4 + un + 64);
-    if (rc != SVSDF_OK) return rc;
-    double *d_fy = reinterpret_cast<double *>(ctx->d_front_scratch);
+    CK(ctx->d_front_scratch.reserve(un * 8 + un * 8 + 2 * un * 4 + un + 64));
+    double *d_fy = reinterpret_cast<double *>(ctx->d_front_scratch.get());
     double *d_cy = d_fy + un;
     int *d_ind = reinterpret_cast<int *>(d_cy + un);
     unsigned char *d_ok = reinterpret_cast<unsigned char *>(d_ind + 2 * un);
     cudaError_t e = cudaMemcpyAsync(d_fy, father_yaw, n * sizeof(double), cudaMemcpyHostToDevice, ctx->stream);
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_ind, ind_xy, 2 * n * sizeof(int), cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess) e = launch_front_check(F, ctx->d_map, ctx->d_front_bytes, n, d_fy, d_ind, d_ok, d_cy, ctx->stream);
+    if (e == cudaSuccess) e = launch_front_check(F, ctx->map(), ctx->d_front_bytes, n, d_fy, d_ind, d_ok, d_cy, ctx->stream);
     if (e == cudaSuccess) e = cudaMemcpyAsync(ok_out, d_ok, n, cudaMemcpyDeviceToHost, ctx->stream);
     if (e == cudaSuccess) e = cudaMemcpyAsync(child_yaw_out, d_cy, n * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
@@ -1471,9 +1403,9 @@ int svsdf_create(const svsdf_config *cfg, svsdf_ctx **out) {
     if ((e = cudaEventCreate(&ctx->ev1)) != cudaSuccess) return fail(e);
     for (int k = 0; k < 5; ++k)
         if ((e = cudaEventCreate(&ctx->evk[k])) != cudaSuccess) return fail(e);
-    if ((e = cudaMalloc(&ctx->d_n_inside, sizeof(int))) != cudaSuccess) return fail(e);
-    if ((e = cudaMalloc(&ctx->d_eval_counter, sizeof(unsigned long long))) != cudaSuccess) return fail(e);
-    if ((e = cudaMalloc(&ctx->d_ticket, sizeof(unsigned int))) != cudaSuccess) return fail(e);
+    if ((e = ctx->d_n_inside.reserve(1)) != cudaSuccess) return fail(e);
+    if ((e = ctx->d_eval_counter.reserve(1)) != cudaSuccess) return fail(e);
+    if ((e = ctx->d_ticket.reserve(1)) != cudaSuccess) return fail(e);
     cudaMemset(ctx->d_ticket, 0, sizeof(unsigned int));
     cudaMemset(ctx->d_n_inside, 0, sizeof(int));
     cudaMemset(ctx->d_eval_counter, 0, sizeof(unsigned long long));
@@ -1498,8 +1430,11 @@ int svsdf_create(const svsdf_config *cfg, svsdf_ctx **out) {
             const double ac = std::sqrt((rec[6] - rec[0]) * (rec[6] - rec[0]) + (rec[7] - rec[1]) * (rec[7] - rec[1]) + (rec[8] - rec[2]) * (rec[8] - rec[2]));
             rec[9] = std::max(ab, ac) * (1.0 + 1e-12) + 1e-300;
         }
-        if ((e = cudaMalloc(&ctx->d_mesh_tri, tri.size() * sizeof(double))) != cudaSuccess) return fail(e);
-        if ((e = cudaMemcpy(ctx->d_mesh_tri, tri.data(), tri.size() * sizeof(double), cudaMemcpyHostToDevice)) != cudaSuccess) return fail(e);
+        auto up = [](auto &buf, const auto &v) -> cudaError_t {
+            const cudaError_t e2 = buf.reserve(v.size());
+            return e2 != cudaSuccess ? e2 : cudaMemcpy(buf, v.data(), v.size() * sizeof(v[0]), cudaMemcpyHostToDevice);
+        };
+        if ((e = up(ctx->d_mesh_tri, tri)) != cudaSuccess) return fail(e);
         ctx->shape.mesh_tri = ctx->d_mesh_tri;
         ctx->shape.mesh_nf = cfg->mesh_nf;
         ctx->shape.has_xform = 0;
@@ -1542,17 +1477,10 @@ int svsdf_create(const svsdf_config *cfg, svsdf_ctx **out) {
         for (int f = 0; f < cfg->mesh_nf; ++f)
             for (int k = 0; k < 3; ++k)
                 for (int j = 0; j < 3; ++j) tf[12 * (size_t)f + 3 * k + j] = B.U[3 * (size_t)B.F[3 * f + k] + j];
-        const size_t b_child = B.child.size() * sizeof(uint32_t), b_data = B.data.size() * sizeof(float), b_box = cb.size() * sizeof(float),
-                     b_tri = tf.size() * sizeof(float);
-        auto up = [&](void **dst, const void *src, size_t bytes) -> cudaError_t {
-            cudaError_t e2 = cudaMalloc(dst, bytes);
-            if (e2 != cudaSuccess) return e2;
-            return cudaMemcpy(*dst, src, bytes, cudaMemcpyHostToDevice);
-        };
-        if ((e = up((void **)&ctx->d_fwn_child, B.child.data(), b_child)) != cudaSuccess) return fail(e);
-        if ((e = up((void **)&ctx->d_fwn_data, B.data.data(), b_data)) != cudaSuccess) return fail(e);
-        if ((e = up((void **)&ctx->d_fwn_cbox, cb.data(), b_box)) != cudaSuccess) return fail(e);
-        if ((e = up((void **)&ctx->d_fwn_trif, tf.data(), b_tri)) != cudaSuccess) return fail(e);
+        if ((e = up(ctx->d_fwn_child, B.child)) != cudaSuccess) return fail(e);
+        if ((e = up(ctx->d_fwn_data, B.data)) != cudaSuccess) return fail(e);
+        if ((e = up(ctx->d_fwn_cbox, cb)) != cudaSuccess) return fail(e);
+        if ((e = up(ctx->d_fwn_trif, tf)) != cudaSuccess) return fail(e);
         // Far-field bound for choiceTInit's layer-1 pruning (thread_choice_t_init): sdf = (1 - 2 w) d with d >= |q| - Rv (Rv: the
         // largest vertex norm; the query has z = 0, the origin is the body origin).  Beyond rho0 = max_i(|P_i| + 2 sqrt(maxPDist2_i))
         // none of the root's children is entered, w is the sum of their four expansions / (4 pi), and each expansion is bounded
@@ -1608,33 +1536,14 @@ void svsdf_destroy(svsdf_ctx *ctx) {
     if (!ctx) return;
     cudaSetDevice(ctx->device);
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);
-    if (ctx->own_points) cudaFree(ctx->d_points);
-    cudaFree(ctx->d_mesh_tri); cudaFree(ctx->d_fwn_child); cudaFree(ctx->d_fwn_data); cudaFree(ctx->d_fwn_cbox); cudaFree(ctx->d_fwn_trif);
-    cudaFree(ctx->d_front_bytes); cudaFree(ctx->d_front_rowmask); cudaFree(ctx->d_cspace); cudaFree(ctx->d_front_scratch); cudaFree(ctx->d_astar_pool);
-    cudaFree(ctx->d_flag); cudaFree(ctx->d_inside_tstar); cudaFree(ctx->d_inside_list);
-    cudaFree(ctx->d_gsip_contrib); cudaFree(ctx->d_gsip_piece); cudaFree(ctx->d_n_inside);
-    cudaFree(ctx->d_eval_counter); cudaFree(ctx->d_tot); cudaFree(ctx->d_ticket); cudaFree(ctx->d_blob); cudaFree(ctx->d_partials); cudaFree(ctx->d_out);
-    cudaFree(ctx->d_q_points); cudaFree(ctx->d_q_sdf); cudaFree(ctx->d_q_ts); cudaFree(ctx->d_q_grad);
-    cudaFree(ctx->d_q_rounds);
-    if (ctx->own_map) cudaFree(ctx->d_map);
-    cudaFree(ctx->d_block_counts); cudaFree(ctx->d_n_total);
-    if (ctx->h_blob) cudaFreeHost(ctx->h_blob);
-    if (ctx->h_out) cudaFreeHost(ctx->h_out);
-    if (ctx->h_stage) cudaFreeHost(ctx->h_stage);
-    if (ctx->h_pts_stage) cudaFreeHost(ctx->h_pts_stage);
-    if (ctx->h_multi_in) cudaFreeHost(ctx->h_multi_in);
-    if (ctx->h_multi_out) cudaFreeHost(ctx->h_multi_out);
-    cudaFree(ctx->d_multi_in); cudaFree(ctx->d_multi_scratch); cudaFree(ctx->d_multi_tickets);
-    cudaFree(ctx->d_sw_corner); cudaFree(ctx->d_sw_point); cudaFree(ctx->d_sw_small); cudaFree(ctx->d_sw_out);
-    cudaFree(ctx->d_cl_small); cudaFree(ctx->d_cl_band); cudaFree(ctx->d_cl_point);
-    if (ctx->ev_pts) cudaEventDestroy(ctx->ev_pts);
     if (ctx->lmbm) svsdf_lmbm_close(ctx->lmbm);
+    if (ctx->ev_pts) cudaEventDestroy(ctx->ev_pts);
     if (ctx->ev0) cudaEventDestroy(ctx->ev0);
     if (ctx->ev1) cudaEventDestroy(ctx->ev1);
     for (int k = 0; k < 5; ++k)
         if (ctx->evk[k]) cudaEventDestroy(ctx->evk[k]);
     if (ctx->stream) cudaStreamDestroy(ctx->stream);
-    delete ctx;
+    delete ctx;  // the buffers free themselves
 }
 
 const char *svsdf_last_error(const svsdf_ctx *ctx) { return ctx ? ctx->err.c_str() : "null context"; }
@@ -1643,33 +1552,14 @@ int svsdf_set_points(svsdf_ctx *ctx, const double *pts, int64_t P, int stride) {
     if (!ctx || P < 0 || stride < 2 || (P > 0 && !pts)) return SVSDF_ERR_INVALID;
     if (P > 2000000000LL) { ctx->err = "svsdf: too many points"; return SVSDF_ERR_INVALID; }
     CK(cudaSetDevice(ctx->device));
-    if (!ctx->own_points) { ctx->d_points = nullptr; ctx->own_points = true; ctx->cap_points = 0; }
-    if (P > ctx->cap_points) {
-        cudaFree(ctx->d_points);
-        ctx->d_points = nullptr;
-        ctx->cap_points = 0;
-        CK(cudaMalloc(&ctx->d_points, (size_t)(P + 1024) * 2 * sizeof(double)));
-        ctx->cap_points = P + 1024;
-    }
-    if (!ctx->d_points) {  // P == 0 and nothing allocated yet
-        CK(cudaMalloc(&ctx->d_points, 1024 * 2 * sizeof(double)));
-        ctx->cap_points = 1024;
-    }
+    ctx->points_ext = nullptr;
+    CK(ctx->points_buf.reserve((size_t)P * 2));  // never null, also for P == 0
     if (ctx->pts_inflight) {  // the previous upload still reads the stage
         CK(cudaEventSynchronize(ctx->ev_pts));
         ctx->pts_inflight = false;
     }
     if (!ctx->ev_pts) CK(cudaEventCreateWithFlags(&ctx->ev_pts, cudaEventDisableTiming));
-    const size_t need = (size_t)P * 2 * sizeof(double);
-    if (need > ctx->cap_pts_stage) {
-        if (ctx->h_pts_stage) cudaFreeHost(ctx->h_pts_stage);
-        ctx->h_pts_stage = nullptr;
-        ctx->cap_pts_stage = 0;
-        const size_t cap = need + need / 4 + 4096;
-        CK(cudaMallocHost(&ctx->h_pts_stage, cap));
-        ctx->cap_pts_stage = cap;
-    }
-    int rc = SVSDF_OK;
+    CK(ctx->h_pts_stage.reserve((size_t)P * 2));
     double *h = ctx->h_pts_stage;
     // pos_eva(2) = 0 (back_end_optimizer.hpp:791): only x, y are kept.  Packed into the pinned stage chunk by chunk by a few
     // host threads; every chunk is handed to the copy engine as soon as it is packed (packing of the next chunks overlaps the
@@ -1684,7 +1574,7 @@ int svsdf_set_points(svsdf_ctx *ctx, const double *pts, int64_t P, int stride) {
 #endif
     int first_err = (int)cudaSuccess;
     const int dev = ctx->device;
-    double *d_points = ctx->d_points;
+    double *d_points = ctx->points_buf;
     cudaStream_t stream = ctx->stream;
 #pragma omp parallel num_threads(nth) if (nth > 1)
     {
@@ -1715,17 +1605,14 @@ int svsdf_set_points(svsdf_ctx *ctx, const double *pts, int64_t P, int stride) {
     ctx->pts_inflight = true;
     ctx->P = P;
     ctx->last_n_inside = -1;
-    (void)rc;
     return ensure_scratch(ctx, P);
 }
 
 int svsdf_set_points_device(svsdf_ctx *ctx, const double *dev_xy, int64_t P) {
     if (!ctx || P < 0 || (P > 0 && !dev_xy)) return SVSDF_ERR_INVALID;
     CK(cudaSetDevice(ctx->device));
-    if (ctx->own_points) cudaFree(ctx->d_points);
-    ctx->d_points = const_cast<double *>(dev_xy);
-    ctx->own_points = false;
-    ctx->cap_points = 0;
+    ctx->points_buf.release();
+    ctx->points_ext = dev_xy;
     ctx->P = P;
     return ensure_scratch(ctx, P);
 }
@@ -1737,7 +1624,7 @@ int svsdf_device_ptr_points(svsdf_ctx *ctx, const double **dev_xy) {
         CK(cudaEventSynchronize(ctx->ev_pts));
         ctx->pts_inflight = false;
     }
-    *dev_xy = ctx->d_points;
+    *dev_xy = ctx->points();
     return SVSDF_OK;
 }
 
@@ -1794,23 +1681,13 @@ int svsdf_query(svsdf_ctx *ctx, int N, const double *T, const double *coeffs, in
     int rc = upload_traj(ctx, N, T, coeffs);
     if (rc) return rc;
     if (P == 0) { CK(cudaStreamSynchronize(ctx->stream)); return SVSDF_OK; }
-    if (P > ctx->cap_q) {
-        cudaFree(ctx->d_q_points); cudaFree(ctx->d_q_sdf); cudaFree(ctx->d_q_ts); cudaFree(ctx->d_q_grad);
-        cudaFree(ctx->d_q_rounds);
-        ctx->d_q_points = ctx->d_q_sdf = ctx->d_q_ts = ctx->d_q_grad = nullptr;
-        ctx->d_q_rounds = nullptr;
-        ctx->cap_q = 0;
-        int64_t cap = P + 1024;
-        CK(cudaMalloc(&ctx->d_q_points, cap * 2 * sizeof(double)));
-        CK(cudaMalloc(&ctx->d_q_sdf, cap * sizeof(double)));
-        CK(cudaMalloc(&ctx->d_q_ts, cap * sizeof(double)));
-        CK(cudaMalloc(&ctx->d_q_grad, cap * 3 * sizeof(double)));
-        CK(cudaMalloc(&ctx->d_q_rounds, cap * sizeof(int)));
-        ctx->cap_q = cap;
-    }
-    rc = ensure_stage(ctx, (size_t)P * 5 * sizeof(double) + (size_t)P * sizeof(int));
-    if (rc) return rc;
-    double *h = ctx->h_stage;
+    CK(ctx->d_q_points.reserve((size_t)P * 2));
+    CK(ctx->d_q_sdf.reserve(P));
+    CK(ctx->d_q_ts.reserve(P));
+    CK(ctx->d_q_grad.reserve((size_t)P * 3));
+    CK(ctx->d_q_rounds.reserve(P));
+    CK(ctx->h_stage.reserve((size_t)P * 5 * sizeof(double) + (size_t)P * sizeof(int)));
+    double *h = reinterpret_cast<double *>(ctx->h_stage.get());
     for (int64_t i = 0; i < P; ++i) { h[2 * i] = pts[3 * i]; h[2 * i + 1] = pts[3 * i + 1]; }
     CK(cudaMemcpyAsync(ctx->d_q_points, h, (size_t)P * 2 * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
     rc = run_kernels(ctx, ctx->d_q_points, P, false, outer_only == 0, ctx->d_q_sdf, ctx->d_q_ts, ctx->d_q_grad,
@@ -1970,24 +1847,21 @@ int svsdf_swept_contour(svsdf_ctx *ctx, int N, const double *T, const double *co
     A.n_samp = n_samp;
     // per corner: need (n bytes), field (n doubles), vertex ids (3 n ints)
     const size_t off_field = align16((size_t)n), off_vid = off_field + align16((size_t)n * 8);
-    int rc = grow_device(ctx, ctx->d_sw_corner, ctx->cap_sw_corner, off_vid + (size_t)n * 12);
-    if (rc) return rc;
+    CK(ctx->d_sw_corner.reserve(off_vid + (size_t)n * 12));
     A.need = ctx->d_sw_corner;
     A.field = reinterpret_cast<double *>(ctx->d_sw_corner + off_field);
     A.vid = reinterpret_cast<int *>(ctx->d_sw_corner + off_vid);
     // small: header [0] non-finite, [1] clipped, [2..6] channel totals, [7] needed corners; samples; tile counts; per-CTA counts
     const size_t off_samp = 64, off_tile = off_samp + align16(samp.size() * 8), off_blk = off_tile + align16((size_t)(tiles + 1) * 4);
-    rc = grow_device(ctx, ctx->d_sw_small, ctx->cap_sw_small, off_blk + (size_t)5 * (nblk + 1) * 4);
-    if (rc) return rc;
-    int *d_hdr = reinterpret_cast<int *>(ctx->d_sw_small);
+    CK(ctx->d_sw_small.reserve(off_blk + (size_t)5 * (nblk + 1) * 4));
+    int *d_hdr = reinterpret_cast<int *>(ctx->d_sw_small.get());
     A.status = d_hdr;
     A.samp = reinterpret_cast<double *>(ctx->d_sw_small + off_samp);
     A.tile_off = reinterpret_cast<int *>(ctx->d_sw_small + off_tile);
     A.blk = reinterpret_cast<int *>(ctx->d_sw_small + off_blk);
-    rc = ensure_stage(ctx, std::max<size_t>(64 + samp.size() * 8, 64));
-    if (rc) return rc;
+    CK(ctx->h_stage.reserve(64 + samp.size() * 8));
     std::memset(ctx->h_stage, 0, 64);
-    std::memcpy(reinterpret_cast<unsigned char *>(ctx->h_stage) + 64, samp.data(), samp.size() * 8);
+    std::memcpy(ctx->h_stage + 64, samp.data(), samp.size() * 8);
     CK(cudaMemcpyAsync(ctx->d_sw_small, ctx->h_stage, 64 + samp.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
     cudaStream_t st = ctx->stream;
     // classify the tiles and their corners, count and compact the needed corners
@@ -1999,16 +1873,15 @@ int svsdf_swept_contour(svsdf_ctx *ctx, int N, const double *T, const double *co
     std::memcpy(hdr, ctx->h_stage, sizeof(hdr));
     const int64_t P = hdr[7];
     ctx->launches += 2;
-    rc = grow_device(ctx, ctx->d_sw_point, ctx->cap_sw_point, (size_t)std::max<int64_t>(P, 1) * 28 + 32);
-    if (rc) return rc;
+    CK(ctx->d_sw_point.reserve((size_t)std::max<int64_t>(P, 1) * 28 + 32));
     A.P = P;
-    A.pts = reinterpret_cast<double *>(ctx->d_sw_point);
+    A.pts = reinterpret_cast<double *>(ctx->d_sw_point.get());
     A.val = reinterpret_cast<double *>(ctx->d_sw_point + (size_t)std::max<int64_t>(P, 1) * 16);
     A.idx = reinterpret_cast<int *>(ctx->d_sw_point + (size_t)std::max<int64_t>(P, 1) * 24);
     if (P > 0) {
         // the outer solve of svsdf_query (outer_only = 1) on the mesher's own points: the same kernels, so the same bits per point
         CK(launch_swept(1, A, st));
-        rc = upload_traj(ctx, N, T, coeffs);
+        int rc = upload_traj(ctx, N, T, coeffs);
         if (rc) return rc;
         rc = run_kernels(ctx, A.pts, P, false, false, const_cast<double *>(A.val), nullptr, nullptr, nullptr);
         if (rc) return rc;
@@ -2029,18 +1902,16 @@ int svsdf_swept_contour(svsdf_ctx *ctx, int N, const double *T, const double *co
     const int64_t V = (int64_t)hdr[2] + hdr[3] + hdr[4], Sg = hdr[5], F = hdr[6];
     const size_t b_verts = (size_t)V * 16, b_segs = (size_t)Sg * 8, b_tris = (size_t)F * 12;
     const size_t o_segs = align16(b_verts), o_tris = o_segs + align16(b_segs), o_end = o_tris + align16(b_tris);
-    rc = grow_device(ctx, ctx->d_sw_out, ctx->cap_sw_out, o_end + 16);
-    if (rc) return rc;
-    A.verts = reinterpret_cast<double *>(ctx->d_sw_out);
+    CK(ctx->d_sw_out.reserve(o_end + 16));
+    A.verts = reinterpret_cast<double *>(ctx->d_sw_out.get());
     A.segs = reinterpret_cast<int *>(ctx->d_sw_out + o_segs);
     A.tris = reinterpret_cast<int *>(ctx->d_sw_out + o_tris);
     CK(launch_swept(4, A, st));
     CK(launch_swept(5, A, st));
     ctx->launches += 2;
     const size_t b_field = prm->want_field ? (size_t)n * 8 : 0;
-    rc = ensure_stage(ctx, o_end + b_field + 16);
-    if (rc) return rc;
-    unsigned char *hs = reinterpret_cast<unsigned char *>(ctx->h_stage);
+    CK(ctx->h_stage.reserve(o_end + b_field + 16));
+    unsigned char *hs = ctx->h_stage;
     if (o_end) CK(cudaMemcpyAsync(hs, ctx->d_sw_out, o_end, cudaMemcpyDeviceToHost, st));
     if (b_field) CK(cudaMemcpyAsync(hs + o_end, A.field, b_field, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
@@ -2094,7 +1965,7 @@ int svsdf_map_clearance(svsdf_ctx *ctx, int N, const double *T, const double *co
     if (traj_layout(N, T, coeffs, L, D, &msg) != SVSDF_OK) return invalid(msg);
     for (int64_t e = 0; e < 18 * (int64_t)N; ++e)
         if (!std::isfinite(coeffs[e])) return invalid("svsdf_map_clearance: non-finite trajectory coefficient");
-    if (!ctx->d_map) {
+    if (!ctx->map()) {
         ctx->err = "svsdf_map_clearance: map not set";
         return SVSDF_ERR_NOT_READY;
     }
@@ -2111,7 +1982,7 @@ int svsdf_map_clearance(svsdf_ctx *ctx, int N, const double *T, const double *co
     CK(cudaSetDevice(ctx->device));
     ClearanceArgs A;
     std::memset(&A, 0, sizeof(A));
-    A.map = ctx->d_map;
+    A.map = ctx->map();
     A.X = ctx->map_X; A.Y = ctx->map_Y; A.h = ctx->map_h; A.row_bytes = ctx->map_row_bytes; A.Z = ctx->map_Z;
     A.layer = (int64_t)(A.X + 2 * A.h) * A.row_bytes;
     A.ox = ctx->map_ox; A.oy = ctx->map_oy; A.res = ctx->map_res;
@@ -2123,18 +1994,15 @@ int svsdf_map_clearance(svsdf_ctx *ctx, int N, const double *T, const double *co
     const int nblk = (int)((A.n_items + 255) / 256);
     // small: header [0] occupied columns (u64), [8] band cells (int); samples; per-CTA counts
     const size_t off_samp = 64, off_blk = off_samp + align16(samp.size() * 8);
-    int rc = grow_device(ctx, ctx->d_cl_small, ctx->cap_cl_small, off_blk + (size_t)(nblk + 1) * 4);
-    if (rc) return rc;
-    rc = grow_device(ctx, ctx->d_cl_band, ctx->cap_cl_band, (size_t)A.n_items * 4);
-    if (rc) return rc;
-    A.n_occ = reinterpret_cast<unsigned long long *>(ctx->d_cl_small);
+    CK(ctx->d_cl_small.reserve(off_blk + (size_t)(nblk + 1) * 4));
+    CK(ctx->d_cl_band.reserve((size_t)A.n_items * 4));
+    A.n_occ = reinterpret_cast<unsigned long long *>(ctx->d_cl_small.get());
     int *d_total = reinterpret_cast<int *>(ctx->d_cl_small + 8);
     A.samp = reinterpret_cast<double *>(ctx->d_cl_small + off_samp);
     A.blk = reinterpret_cast<int *>(ctx->d_cl_small + off_blk);
-    A.band = reinterpret_cast<unsigned *>(ctx->d_cl_band);
-    rc = ensure_stage(ctx, 64 + samp.size() * 8);
-    if (rc) return rc;
-    unsigned char *hs = reinterpret_cast<unsigned char *>(ctx->h_stage);
+    A.band = reinterpret_cast<unsigned *>(ctx->d_cl_band.get());
+    CK(ctx->h_stage.reserve(64 + samp.size() * 8));
+    unsigned char *hs = ctx->h_stage;
     std::memset(hs, 0, 64);
     if (!samp.empty()) std::memcpy(hs + 64, samp.data(), samp.size() * 8);
     cudaStream_t st = ctx->stream;
@@ -2151,22 +2019,20 @@ int svsdf_map_clearance(svsdf_ctx *ctx, int N, const double *T, const double *co
     const int64_t P = P32;
     // band cells: (i, j) int32 pairs, centres, values, t* — contiguous, so one download brings them all
     const size_t o_pts = align16((size_t)P * 8), o_sdf = o_pts + (size_t)P * 16, o_ts = o_sdf + (size_t)P * 8, o_end = o_ts + (size_t)P * 8;
-    rc = grow_device(ctx, ctx->d_cl_point, ctx->cap_cl_point, o_end + 16);
-    if (rc) return rc;
-    A.ij = reinterpret_cast<int *>(ctx->d_cl_point);
+    CK(ctx->d_cl_point.reserve(o_end + 16));
+    A.ij = reinterpret_cast<int *>(ctx->d_cl_point.get());
     A.pts = reinterpret_cast<double *>(ctx->d_cl_point + o_pts);
     double *d_sdf = reinterpret_cast<double *>(ctx->d_cl_point + o_sdf), *d_ts = reinterpret_cast<double *>(ctx->d_cl_point + o_ts);
     if (P > 0) {
         CK(launch_clearance(1, A, st));
         ctx->launches += 1;
         // svsdf_query's path (outer solve, then the interior branch) on the band: the same kernels, so the same bits per point
-        rc = upload_traj(ctx, N, T, coeffs);
+        int rc = upload_traj(ctx, N, T, coeffs);
         if (rc) return rc;
         rc = run_kernels(ctx, A.pts, P, false, true, d_sdf, d_ts, nullptr, nullptr);
         if (rc) return rc;
-        rc = ensure_stage(ctx, o_end);
-        if (rc) return rc;
-        hs = reinterpret_cast<unsigned char *>(ctx->h_stage);
+        CK(ctx->h_stage.reserve(o_end));
+        hs = ctx->h_stage;
         CK(cudaMemcpyAsync(hs, ctx->d_cl_point, o_end, cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
     }
@@ -2229,7 +2095,7 @@ void svsdf_clearance_free(svsdf_clearance *c) {
 int svsdf_cost_grad_device(svsdf_ctx *ctx, int N, const double *T, const double *coeffs, int repeats,
                            float *ms_per_eval, double *out_host) {
     if (!ctx || repeats < 1) return SVSDF_ERR_INVALID;
-    if (!ctx->d_points) { ctx->err = "svsdf: query points not set"; return SVSDF_ERR_NOT_READY; }
+    if (!ctx->points()) { ctx->err = "svsdf: query points not set"; return SVSDF_ERR_NOT_READY; }
     CK(cudaSetDevice(ctx->device));
     int rc = upload_traj(ctx, N, T, coeffs, false);
     if (rc) return rc;
@@ -2241,7 +2107,7 @@ int svsdf_cost_grad_device(svsdf_ctx *ctx, int N, const double *T, const double 
         rc = pose_table(ctx);
         if (rc) return rc;
         if (ctx->mark_kernels) CK(cudaEventRecord(ctx->evk[1], ctx->stream));
-        rc = run_kernels(ctx, ctx->d_points, ctx->P, true, true, nullptr, nullptr, nullptr, nullptr);
+        rc = run_kernels(ctx, ctx->points(), ctx->P, true, true, nullptr, nullptr, nullptr, nullptr);
         if (ctx->mark_kernels) cudaEventRecord(ctx->evk[4], ctx->stream);
         ctx->mark_kernels = false;
         if (rc) return rc;
@@ -2355,20 +2221,7 @@ int svsdf_optimize(svsdf_ctx *ctx, const double *initS, const double *finalS, do
     }
     auto t1 = std::chrono::steady_clock::now();
     ctx->time_kernels = false;
-    // final trajectory from the returned iterate (optimize_traj_lmbm does the same on success and failure,
-    // back_end_optimizer.cpp:44-94)
-    for (int i = 0; i < N; ++i) ctx->he.times[i] = host::forwardT(opt_x[i]);
-    ctx->he.minco.setParameters(opt_x + N, ctx->he.times.data());
-    if (T_out) std::memcpy(T_out, ctx->he.times.data(), sizeof(double) * N);
-    if (coeffs_out) std::memcpy(coeffs_out, ctx->he.minco.getCoeffs(), sizeof(double) * 18 * N);
-    if (stats) {
-        stats->final_cost = R.f;
-        stats->iterations = R.iterations;
-        stats->evaluations = R.evaluations;
-        stats->status = R.status;
-        stats->seconds = std::chrono::duration<double>(t1 - t0).count();
-        stats->gpu_seconds = ctx->gpu_ms_total * 1e-3;
-    }
+    ctx->he.finish(opt_x, R, std::chrono::duration<double>(t1 - t0).count(), ctx->gpu_ms_total * 1e-3, T_out, coeffs_out, stats);
     // an evaluation that failed (points not set, CUDA error, duration >= 300 s) is an error of the run, whatever the
     // solver made of the NaN it was handed
     if (ctx->last_status != SVSDF_OK) return ctx->last_status;
@@ -2564,17 +2417,8 @@ int svsdf_optimize_lockstep(svsdf_ctx *ctx, const svsdf_lockstep_problem *proble
         const auto t0 = std::chrono::steady_clock::now();
         const host::LbfgsResult R = solver.minimize(p.opt_x, nv, lockstep_evaluate, &s, nullptr, nullptr);
         const auto t1 = std::chrono::steady_clock::now();
-        // final trajectory from the returned iterate, as svsdf_optimize
-        for (int i = 0; i < N; ++i) s.he.times[i] = host::forwardT(p.opt_x[i]);
-        s.he.minco.setParameters(p.opt_x + N, s.he.times.data());
-        if (p.T_out) std::memcpy(p.T_out, s.he.times.data(), sizeof(double) * N);
-        if (p.coeffs_out) std::memcpy(p.coeffs_out, s.he.minco.getCoeffs(), sizeof(double) * 18 * N);
-        if (stats_out) {
-            svsdf_opt_stats &st = stats_out[k];
-            st.final_cost = R.f; st.iterations = R.iterations; st.evaluations = R.evaluations; st.status = R.status;
-            st.seconds = std::chrono::duration<double>(t1 - t0).count();
-            st.gpu_seconds = s.gpu_ms * 1e-3;
-        }
+        s.he.finish(p.opt_x, R, std::chrono::duration<double>(t1 - t0).count(), s.gpu_ms * 1e-3, p.T_out, p.coeffs_out,
+                    stats_out ? &stats_out[k] : nullptr);
         int ret = R.status == 0 ? 1 : R.status;
         if (s.last_status != SVSDF_OK) ret = s.last_status;
         if (status_out) status_out[k] = ret;
@@ -2655,24 +2499,18 @@ static int shape_eval(svsdf_ctx *ctx, int64_t n, const double *rel, double *out,
     if (n == 0) return SVSDF_OK;
     CK(cudaSetDevice(ctx->device));
     const int ow = grad ? 3 : 1;
-    int rc = ensure_stage(ctx, (size_t)n * (2 + ow) * sizeof(double));
-    if (rc) return rc;
-    double *d_in = nullptr, *d_out = nullptr;
-    CK(cudaMalloc(&d_in, (size_t)n * 2 * sizeof(double)));
-    if (cudaMalloc(&d_out, (size_t)n * ow * sizeof(double)) != cudaSuccess) { cudaFree(d_in); ctx->err = "cudaMalloc"; return SVSDF_ERR_CUDA; }
-    double *h = ctx->h_stage;
+    CK(ctx->h_stage.reserve((size_t)n * (2 + ow) * sizeof(double)));
+    DeviceBuffer<double> d_in, d_out;
+    CK(d_in.reserve((size_t)n * 2));
+    CK(d_out.reserve((size_t)n * ow));
+    double *h = reinterpret_cast<double *>(ctx->h_stage.get());
     for (int64_t i = 0; i < n; ++i) { h[2 * i] = rel[3 * i]; h[2 * i + 1] = rel[3 * i + 1]; }
-    cudaError_t e = cudaMemcpyAsync(d_in, h, (size_t)n * 2 * sizeof(double), cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess)
-        e = ctx->strict ? strict::launch_shape_eval(ctx->shape, d_in, n, d_out, grad, ctx->stream)
-                        : fast::launch_shape_eval(ctx->shape, d_in, n, d_out, grad, ctx->stream);
+    CK(cudaMemcpyAsync(d_in, h, (size_t)n * 2 * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    CK(kernels(ctx).shape_eval(ctx->shape, d_in, n, d_out, grad, ctx->stream));
     ctx->launches += 1;
     double *ho = h + 2 * n;
-    if (e == cudaSuccess) e = cudaMemcpyAsync(ho, d_out, (size_t)n * ow * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    cudaFree(d_in);
-    cudaFree(d_out);
-    if (e != cudaSuccess) { ctx->err = cudaGetErrorString(e); return SVSDF_ERR_CUDA; }
+    CK(cudaMemcpyAsync(ho, d_out, (size_t)n * ow * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
     std::memcpy(out, ho, (size_t)n * ow * sizeof(double));
     return SVSDF_OK;
 }
@@ -2698,15 +2536,9 @@ int svsdf_set_map(svsdf_ctx *ctx, const unsigned char *kernel_bytes, int X, int 
     int rc = set_map_meta(ctx, X, Y, kernel_size, origin_x, origin_y, res);
     if (rc) return rc;
     const size_t bytes = (size_t)(X + 2 * ctx->map_h) * ctx->map_row_bytes;
-    if (!ctx->own_map) { ctx->d_map = nullptr; ctx->own_map = true; ctx->cap_map = 0; }
-    if (bytes > ctx->cap_map) {
-        cudaFree(ctx->d_map);
-        ctx->d_map = nullptr;
-        ctx->cap_map = 0;
-        CK(cudaMalloc(&ctx->d_map, bytes + 64));
-        ctx->cap_map = bytes + 64;
-    }
-    CK(cudaMemcpyAsync(ctx->d_map, kernel_bytes, bytes, cudaMemcpyHostToDevice, ctx->stream));
+    ctx->map_ext = nullptr;
+    CK(ctx->map_buf.reserve(bytes));
+    CK(cudaMemcpyAsync(ctx->map_buf, kernel_bytes, bytes, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     return SVSDF_OK;
 }
@@ -2717,10 +2549,8 @@ int svsdf_set_map_device(svsdf_ctx *ctx, const unsigned char *dev_kernel_bytes, 
     CK(cudaSetDevice(ctx->device));
     int rc = set_map_meta(ctx, X, Y, kernel_size, origin_x, origin_y, res);
     if (rc) return rc;
-    if (ctx->own_map) cudaFree(ctx->d_map);
-    ctx->d_map = const_cast<unsigned char *>(dev_kernel_bytes);
-    ctx->own_map = false;
-    ctx->cap_map = 0;
+    ctx->map_buf.release();
+    ctx->map_ext = dev_kernel_bytes;
     return SVSDF_OK;
 }
 
@@ -2749,15 +2579,9 @@ int svsdf_set_map3d(svsdf_ctx *ctx, const unsigned char *kernel_bytes, int X, in
             }
         }
     const size_t bytes = L.size();
-    if (!ctx->own_map) { ctx->d_map = nullptr; ctx->own_map = true; ctx->cap_map = 0; }
-    if (bytes > ctx->cap_map) {
-        cudaFree(ctx->d_map);
-        ctx->d_map = nullptr;
-        ctx->cap_map = 0;
-        CK(cudaMalloc(&ctx->d_map, bytes + 64));
-        ctx->cap_map = bytes + 64;
-    }
-    CK(cudaMemcpyAsync(ctx->d_map, L.data(), bytes, cudaMemcpyHostToDevice, ctx->stream));
+    ctx->map_ext = nullptr;
+    CK(ctx->map_buf.reserve(bytes));
+    CK(cudaMemcpyAsync(ctx->map_buf, L.data(), bytes, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     ctx->map_Z = Z;
     ctx->map_oz = origin_xyz[2];
@@ -2767,7 +2591,7 @@ int svsdf_set_map3d(svsdf_ctx *ctx, const unsigned char *kernel_bytes, int X, in
 // Shared by the flat and the 3-D entry points.  wp: W x 3 waypoint centres, half: box half sizes (x, y, z).
 static int extract_impl(svsdf_ctx *ctx, const char *who, const double *wp, int W, const double *half, const double *keepout_xy,
                         int n_keepout, double clearance, int64_t *n_points) {
-    if (!ctx->d_map) { ctx->err = std::string(who) + ": map not set"; return SVSDF_ERR_NOT_READY; }
+    if (!ctx->map()) { ctx->err = std::string(who) + ": map not set"; return SVSDF_ERR_NOT_READY; }
     CK(cudaSetDevice(ctx->device));
     ExtractArgs E;
     std::memset(&E, 0, sizeof(E));
@@ -2819,18 +2643,12 @@ static int extract_impl(svsdf_ctx *ctx, const char *who, const double *wp, int W
     for (int q = 0; q < 2 * n_keepout; ++q) E.keepout[q] = keepout_xy[q];
     const int n_blocks = (int)((E.n_items + 255) / 256);
     const size_t need_counts = (size_t)(n_blocks + 1) * (size_t)Z;
-    if (need_counts > (size_t)ctx->cap_block_counts) {
-        cudaFree(ctx->d_block_counts);
-        ctx->d_block_counts = nullptr;
-        ctx->cap_block_counts = 0;
-        CK(cudaMalloc(&ctx->d_block_counts, (need_counts + 1024) * sizeof(int)));
-        ctx->cap_block_counts = (int)(need_counts + 1024);
-    }
-    if (!ctx->d_n_total) CK(cudaMalloc(&ctx->d_n_total, kMaxMapLayers * sizeof(int64_t)));
+    CK(ctx->d_block_counts.reserve(need_counts));
+    CK(ctx->d_n_total.reserve(kMaxMapLayers));
     const size_t layer = (size_t)(E.X + 2 * E.h) * E.row_bytes;
     auto layer_args = [&](int k) {
         ExtractArgs Ek = E;
-        Ek.map = ctx->d_map + (size_t)k * layer;
+        Ek.map = ctx->map() + (size_t)k * layer;
         for (int w = 0; w < W; ++w) {
             Ek.act[w] = (k >= bz1[w + 1] && k <= bz2[w + 1]) ? 1 : 0;
             Ek.excl[w] = (k >= bz1[w] && k <= bz2[w]) ? 1 : 0;
@@ -2847,17 +2665,11 @@ static int extract_impl(svsdf_ctx *ctx, const char *who, const double *wp, int W
     int64_t total = 0;
     for (int k = 0; k < Z; ++k) total += totals[k];
     if (total > 2000000000LL) { ctx->err = std::string(who) + ": too many points"; return SVSDF_ERR_INVALID; }
-    if (!ctx->own_points) { ctx->d_points = nullptr; ctx->own_points = true; ctx->cap_points = 0; }
-    if (total > ctx->cap_points || !ctx->d_points) {
-        cudaFree(ctx->d_points);
-        ctx->d_points = nullptr;
-        ctx->cap_points = 0;
-        CK(cudaMalloc(&ctx->d_points, (size_t)(total + 1024) * 2 * sizeof(double)));
-        ctx->cap_points = total + 1024;
-    }
+    ctx->points_ext = nullptr;
+    CK(ctx->points_buf.reserve((size_t)total * 2));
     int64_t base = 0;
     for (int k = 0; k < Z; ++k) {  // layer-major output: layer 0's cells in ascending (i * Y + j) order, then layer 1's, ...
-        CK(launch_extract_write(layer_args(k), ctx->d_block_counts + (size_t)k * (n_blocks + 1), n_blocks, ctx->d_points + 2 * base, totals[k], ctx->stream));
+        CK(launch_extract_write(layer_args(k), ctx->d_block_counts + (size_t)k * (n_blocks + 1), n_blocks, ctx->points_buf + 2 * base, totals[k], ctx->stream));
         ctx->launches += 1;
         base += totals[k];
     }
@@ -2899,7 +2711,7 @@ int svsdf_get_points(svsdf_ctx *ctx, double *xy_out, int64_t capacity, int64_t *
     if (!xy_out || capacity <= 0 || ctx->P == 0) return SVSDF_OK;
     CK(cudaSetDevice(ctx->device));
     const int64_t n = ctx->P < capacity ? ctx->P : capacity;
-    CK(cudaMemcpy(xy_out, ctx->d_points, (size_t)n * 2 * sizeof(double), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(xy_out, ctx->points(), (size_t)n * 2 * sizeof(double), cudaMemcpyDeviceToHost));
     return SVSDF_OK;
 }
 
@@ -2907,18 +2719,14 @@ int svsdf_sincos(svsdf_ctx *ctx, int64_t n, const double *x, double *sin_out, do
     if (!ctx || n < 0 || (n > 0 && (!x || !sin_out || !cos_out))) return SVSDF_ERR_INVALID;
     if (n == 0) return SVSDF_OK;
     CK(cudaSetDevice(ctx->device));
-    double *d = nullptr;
-    CK(cudaMalloc(&d, (size_t)n * 3 * sizeof(double)));
-    cudaError_t e = cudaMemcpyAsync(d, x, (size_t)n * sizeof(double), cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess)
-        e = ctx->strict ? strict::launch_sincos(d, n, d + n, d + 2 * n, ctx->stream)
-                        : fast::launch_sincos(d, n, d + n, d + 2 * n, ctx->stream);
+    DeviceBuffer<double> d;
+    CK(d.reserve((size_t)n * 3));
+    CK(cudaMemcpyAsync(d, x, (size_t)n * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    CK(kernels(ctx).sincos(d, n, d + n, d + 2 * n, ctx->stream));
     ctx->launches += 1;
-    if (e == cudaSuccess) e = cudaMemcpyAsync(sin_out, d + n, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(cos_out, d + 2 * n, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    cudaFree(d);
-    if (e != cudaSuccess) { ctx->err = cudaGetErrorString(e); return SVSDF_ERR_CUDA; }
+    CK(cudaMemcpyAsync(sin_out, d + n, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(cos_out, d + 2 * n, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
     return SVSDF_OK;
 }
 
@@ -2952,13 +2760,12 @@ int svsdf_fp64_peak(svsdf_ctx *ctx, double *tflops) {
     if (!ctx || !tflops) return SVSDF_ERR_INVALID;
     CK(cudaSetDevice(ctx->device));
     const int grid = ctx->sm_count * 8, iters = 1 << 16;
-    double *d = nullptr;
-    CK(cudaMalloc(&d, (size_t)grid * 256 * sizeof(double)));
+    DeviceBuffer<double> d;
+    CK(d.reserve((size_t)grid * 256));
     float best = 1e30f;
     for (int r = 0; r < 5; ++r) {
         CK(cudaEventRecord(ctx->ev0, ctx->stream));
-        cudaError_t e = fast::launch_fp64_peak(d, grid, iters, ctx->stream);
-        if (e != cudaSuccess) { cudaFree(d); ctx->err = cudaGetErrorString(e); return SVSDF_ERR_CUDA; }
+        CK(fast::launch_fp64_peak(d, grid, iters, ctx->stream));
         CK(cudaEventRecord(ctx->ev1, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
         float ms = 0;
@@ -2966,7 +2773,6 @@ int svsdf_fp64_peak(svsdf_ctx *ctx, double *tflops) {
         if (r > 0 && ms < best) best = ms;
         ctx->launches += 1;
     }
-    cudaFree(d);
     const double flops = 2.0 * 8.0 * (double)iters * (double)grid * 256.0;
     *tflops = flops / (best * 1e-3) / 1e12;
     return SVSDF_OK;

@@ -152,7 +152,7 @@ struct KernelArgs {
 
 // svsdf_cost_grad_multi (svsdf_kernels_multi.cuh): n problems in one set of launches.  The KernelArgs of a multi launch hold the
 // BASES of the packed buffers; MultiProblem says where problem k's pieces start.  Each problem keeps the decomposition of its
-// single-problem call: its virtual grid `grid` (grid_for with the single-problem k_outer's occupancy) and its `batched` schedule.
+// single-problem call: its virtual grid `grid` (outer_plan with the single-problem k_outer's occupancy) and its `batched` schedule.
 constexpr int kMaxMultiProblems = 65535;  // problems per multi evaluation (k_finalize_multi's grid.y)
 struct MultiProblem {
     int64_t blob_off;    // doubles into the packed blobs (even: every blob starts 16-byte aligned, as the TMA load needs)
