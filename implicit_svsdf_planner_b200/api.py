@@ -165,6 +165,11 @@ class ClearanceOut(C.Structure):
                 ("min_sdf", C.c_double), ("argmin", C.c_int64), ("ij", C.POINTER(C.c_int32)), ("xy", dp), ("sdf", dp), ("tstar", dp)]
 
 
+class ClearanceProblem(C.Structure):
+    """svsdf_clearance_problem (include/svsdf.h)."""
+    _fields_ = [("N", C.c_int), ("T", dp), ("coeffs", dp)]
+
+
 @dataclasses.dataclass
 class Clearance:
     """Result of Context.map_clearance: the occupied map cells whose swept-volume SDF value is <= d_max, in map order (i * Y + j).
@@ -186,6 +191,20 @@ class Clearance:
     @property
     def collision_free(self) -> bool:
         return self.min_sdf > 0.0
+
+
+def _take_clearance(m: ClearanceOut, d_max) -> Clearance:
+    """Copies an svsdf_clearance into a Clearance and releases its arrays."""
+    try:
+        n = m.n_within
+        ij = np.ctypeslib.as_array(m.ij, shape=(n, 2)).copy() if n else np.empty((0, 2), dtype=np.int32)
+        xy = np.ctypeslib.as_array(m.xy, shape=(n, 2)).copy() if n else np.empty((0, 2))
+        sdf = np.ctypeslib.as_array(m.sdf, shape=(n,)).copy() if n else np.empty(0)
+        ts = np.ctypeslib.as_array(m.tstar, shape=(n,)).copy() if n else np.empty(0)
+        return Clearance(float(d_max), ij, xy, sdf, ts, int(m.n_occupied), int(m.n_evaluated), int(n), int(m.n_colliding),
+                         float(m.min_sdf), int(m.argmin))
+    finally:
+        lib().svsdf_clearance_free(C.byref(m))
 
 
 def write_prism_obj(path, contour: "SweptContour", z0=0.0, z1=1.0):
@@ -222,7 +241,7 @@ EXPORTED_SYMBOLS = [
     "svsdf_front_init", "svsdf_front_get_kernels", "svsdf_front_cspace", "svsdf_front_check_kernel_value", "svsdf_front_expand", "svsdf_front_astar",
     "svsdf_front_astar_device", "svsdf_set_scale", "svsdf_scale_matrix",
     "svsdf_cost_grad_multi", "svsdf_optimize_lockstep", "svsdf_lockstep_rounds", "svsdf_swept_contour", "svsdf_swept_free",
-    "svsdf_map_clearance", "svsdf_clearance_free",
+    "svsdf_map_clearance", "svsdf_clearance_free", "svsdf_map_clearance_multi",
 ]
 
 
@@ -309,6 +328,8 @@ def lib():
     L.svsdf_map_clearance.argtypes = [vp, C.c_int, dp, dp, C.c_double, C.POINTER(ClearanceOut)]
     L.svsdf_clearance_free.argtypes = [C.POINTER(ClearanceOut)]
     L.svsdf_clearance_free.restype = None
+    L.svsdf_map_clearance_multi.argtypes = [vp, C.c_int, C.POINTER(ClearanceProblem), C.c_double, C.POINTER(ClearanceOut),
+                                            C.POINTER(C.c_int)]
     _lib = L
     return L
 
@@ -674,18 +695,26 @@ class Context:
         T = _f64(T)
         c = _f64(coeffs_colmajor).reshape(-1)
         m = ClearanceOut()
-        L = lib()
-        self._ck(L.svsdf_map_clearance(self.h, T.shape[0], _p(T), _p(c), float(d_max), C.byref(m)), "svsdf_map_clearance")
-        try:
-            n = m.n_within
-            ij = np.ctypeslib.as_array(m.ij, shape=(n, 2)).copy() if n else np.empty((0, 2), dtype=np.int32)
-            xy = np.ctypeslib.as_array(m.xy, shape=(n, 2)).copy() if n else np.empty((0, 2))
-            sdf = np.ctypeslib.as_array(m.sdf, shape=(n,)).copy() if n else np.empty(0)
-            ts = np.ctypeslib.as_array(m.tstar, shape=(n,)).copy() if n else np.empty(0)
-            return Clearance(float(d_max), ij, xy, sdf, ts, int(m.n_occupied), int(m.n_evaluated), int(n), int(m.n_colliding),
-                             float(m.min_sdf), int(m.argmin))
-        finally:
-            L.svsdf_clearance_free(C.byref(m))
+        self._ck(lib().svsdf_map_clearance(self.h, T.shape[0], _p(T), _p(c), float(d_max), C.byref(m)), "svsdf_map_clearance")
+        return _take_clearance(m, d_max)
+
+    def map_clearance_multi(self, trajs, d_max=math.inf) -> list:
+        """svsdf_map_clearance_multi: map_clearance of every trajectory in trajs (a list of (T, coeffs_colmajor)) in one set of launches,
+        each the bits of its own map_clearance call.  Returns one entry per trajectory: a Clearance, or an SvsdfError for a trajectory whose
+        single call would have failed with a non-finite value.  An invalid trajectory or d_max raises for the whole call."""
+        n = len(trajs)
+        arr = (ClearanceProblem * max(n, 1))()
+        keep = []
+        for k, (T, co) in enumerate(trajs):
+            T, co = _f64(T).reshape(-1), _f64(co).reshape(-1)
+            arr[k].N, arr[k].T, arr[k].coeffs = T.shape[0], _p(T), _p(co)
+            keep += [T, co]
+        outs = (ClearanceOut * max(n, 1))()
+        status = np.zeros(max(n, 1), dtype=np.int32)
+        self._ck(lib().svsdf_map_clearance_multi(self.h, n, arr, float(d_max), outs, status.ctypes.data_as(C.POINTER(C.c_int))),
+                 "svsdf_map_clearance_multi")
+        return [_take_clearance(outs[k], d_max) if status[k] == 0 else
+                SvsdfError(f"svsdf_map_clearance_multi: problem {k}: status {int(status[k])}") for k in range(n)]
 
     def query(self, T, coeffs_colmajor, pts, outer_only=False):
         T = _f64(T)

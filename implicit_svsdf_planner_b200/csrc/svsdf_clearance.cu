@@ -10,6 +10,9 @@
 //   k_sw_scan    exclusive prefix of the per-CTA counts (svsdf_swept.cu, one CTA).
 //   k_cl_write   the band's cells (i, j) and centres, in map order, into the clearance's own point buffer.
 //   (svsdf_query's kernels, outer solve and interior branch, run on that buffer)
+// svsdf_map_clearance_multi runs the same per-CTA test over each problem's reach rectangle (k_cl_count_multi, k_sw_scan,
+// k_cl_write_multi: the bands of all problems, concatenated in problem order, each in map order); the multi-problem kernels of
+// svsdf_kernels_multi.cuh evaluate them.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -69,41 +72,46 @@ __device__ __forceinline__ unsigned column_word(const ClearanceArgs &A, int i, i
     return w & interval_mask(A.h - 32 * wy, A.h + A.Y - 1 - 32 * wy);
 }
 
-__global__ void __launch_bounds__(256) k_cl_count(const __grid_constant__ ClearanceArgs A) {
-    __shared__ int s_list[kSweptMaxSamples];
-    __shared__ int s_n;
-    __shared__ int s_w[2][8];
-    const int64_t first = (int64_t)blockIdx.x * blockDim.x;
-    const int64_t last = min(first + (int64_t)blockDim.x - 1, A.n_items - 1);
-    const int64_t item = first + threadIdx.x;
+// The items of one CTA: item t = t0 + threadIdx.x (< n_items) is word wy0 + t % nW of map row i0 + t / nW.  Returns the item's band bits
+// (its occupied columns whose centre lies within some sample's reach; all of them when `all`) and its occupied bits in *occ.
+struct CtaItems {
+    int64_t t0, n_items;
+    int i0, wy0, nW, all, n_samp;
+    const double *samp;
+};
+__device__ __forceinline__ unsigned cta_band(const ClearanceArgs &A, const CtaItems &C, int *s_list, int *s_n, unsigned *occ_out) {
+    const int64_t first = C.t0;
+    const int64_t last = min(first + (int64_t)blockDim.x - 1, C.n_items - 1);
+    const int64_t t = first + threadIdx.x;
     int i = 0, wy = 0;
     unsigned occ = 0u;
-    if (item < A.n_items) {
-        i = (int)(item / A.nW);
-        wy = A.wy0 + (int)(item % A.nW);
+    if (t < C.n_items) {
+        i = C.i0 + (int)(t / C.nW);
+        wy = C.wy0 + (int)(t % C.nW);
         occ = column_word(A, i, wy);
     }
-    unsigned band = A.all ? occ : 0u;
-    if (!A.all) {  // uniform over the CTA
+    *occ_out = occ;
+    unsigned band = C.all ? occ : 0u;
+    if (!C.all) {  // uniform over the CTA
         // box of the CTA's cell centres: its rows, and the y range of its words when it lies in one row (the whole map's otherwise)
-        const int i0 = (int)(first / A.nW), i1 = (int)(last / A.nW);
+        const int i0 = C.i0 + (int)(first / C.nW), i1 = C.i0 + (int)(last / C.nW);
         int j0 = 0, j1 = A.Y - 1;
         if (i0 == i1) {
-            j0 = max(32 * (A.wy0 + (int)(first % A.nW)) - A.h, 0);
-            j1 = min(32 * (A.wy0 + (int)(last % A.nW)) + 31 - A.h, A.Y - 1);
+            j0 = max(32 * (C.wy0 + (int)(first % C.nW)) - A.h, 0);
+            j1 = min(32 * (C.wy0 + (int)(last % C.nW)) + 31 - A.h, A.Y - 1);
         }
         const double bx0 = centre_x(A, i0), bx1 = centre_x(A, i1), by0 = centre_y(A, j0), by1 = centre_y(A, j1);
-        if (threadIdx.x == 0) s_n = 0;
+        if (threadIdx.x == 0) *s_n = 0;
         __syncthreads();
         // a sample that reaches a centre of the CTA reaches its box: the centres are monotone in the index and the rounded differences
         // and squares are monotone, so the box distance is never larger than the centre distance computed below (k_sw_classify's test)
-        for (int k = threadIdx.x; k < A.n_samp; k += blockDim.x) {
-            const double sx = A.samp[3 * k], sy = A.samp[3 * k + 1], r = A.samp[3 * k + 2];
+        for (int k = threadIdx.x; k < C.n_samp; k += blockDim.x) {
+            const double sx = C.samp[3 * k], sy = C.samp[3 * k + 1], r = C.samp[3 * k + 2];
             const double dx = fmax(fmax(bx0 - sx, sx - bx1), 0.0), dy = fmax(fmax(by0 - sy, sy - by1), 0.0);
-            if (dx * dx + dy * dy <= r * r) s_list[atomicAdd(&s_n, 1)] = k;
+            if (dx * dx + dy * dy <= r * r) s_list[atomicAdd(s_n, 1)] = k;
         }
         __syncthreads();
-        const int n = s_n;
+        const int n = *s_n;
         if (occ && n) {
             const double cx = centre_x(A, i);
             const int ybase = 32 * wy - A.h;
@@ -113,13 +121,38 @@ __global__ void __launch_bounds__(256) k_cl_count(const __grid_constant__ Cleara
                 bool in = false;
                 for (int q = 0; q < n && !in; ++q) {
                     const int s = s_list[q];
-                    const double dx = cx - A.samp[3 * s], dy = cy - A.samp[3 * s + 1], r = A.samp[3 * s + 2];
+                    const double dx = cx - C.samp[3 * s], dy = cy - C.samp[3 * s + 1], r = C.samp[3 * s + 2];
                     in = dx * dx + dy * dy <= r * r;
                 }
                 if (in) band |= 1u << k;
             }
         }
     }
+    return band;
+}
+
+// the band cells of word wy of row i, from list position pos on
+__device__ __forceinline__ void write_cells(const ClearanceArgs &A, unsigned band, int i, int wy, int64_t pos) {
+    const int ybase = 32 * wy - A.h;
+    const double cx = centre_x(A, i);
+    for (; band; band &= band - 1) {
+        const int j = ybase + __ffs(band) - 1;
+        A.ij[2 * pos] = i;
+        A.ij[2 * pos + 1] = j;
+        A.pts[2 * pos] = cx;
+        A.pts[2 * pos + 1] = centre_y(A, j);
+        ++pos;
+    }
+}
+
+__global__ void __launch_bounds__(256) k_cl_count(const __grid_constant__ ClearanceArgs A) {
+    __shared__ int s_list[kSweptMaxSamples];
+    __shared__ int s_n;
+    __shared__ int s_w[2][8];
+    const CtaItems C{(int64_t)blockIdx.x * blockDim.x, A.n_items, 0, A.wy0, A.nW, A.all, A.n_samp, A.samp};
+    unsigned occ;
+    const unsigned band = cta_band(A, C, s_list, &s_n, &occ);
+    const int64_t item = C.t0 + threadIdx.x;
     if (item < A.n_items) A.band[item] = band;
     int n_band, n_occ;
     block_scan256(__popc(band), s_w[0], &n_band);
@@ -133,21 +166,55 @@ __global__ void __launch_bounds__(256) k_cl_count(const __grid_constant__ Cleara
 __global__ void __launch_bounds__(256) k_cl_write(const __grid_constant__ ClearanceArgs A) {
     __shared__ int s_w[8];
     const int64_t item = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    unsigned band = item < A.n_items ? A.band[item] : 0u;
+    const unsigned band = item < A.n_items ? A.band[item] : 0u;
     int total;
-    int64_t pos = (int64_t)A.blk[blockIdx.x] + block_scan256(__popc(band), s_w, &total);
+    const int64_t pos = (int64_t)A.blk[blockIdx.x] + block_scan256(__popc(band), s_w, &total);
     if (!band) return;
-    const int i = (int)(item / A.nW), wy = A.wy0 + (int)(item % A.nW);
-    const int ybase = 32 * wy - A.h;
-    const double cx = centre_x(A, i);
-    for (; band; band &= band - 1) {
-        const int j = ybase + __ffs(band) - 1;
-        A.ij[2 * pos] = i;
-        A.ij[2 * pos + 1] = j;
-        A.pts[2 * pos] = cx;
-        A.pts[2 * pos + 1] = centre_y(A, j);
-        ++pos;
+    write_cells(A, band, (int)(item / A.nW), A.wy0 + (int)(item % A.nW), pos);
+}
+
+// ---- svsdf_map_clearance_multi: the CTAs of problem k are cta0[k] .. cta0[k + 1] - 1, in problem order; the last segment counts the
+// occupied columns of the whole map and has no band.  Items: one per (CTA, thread), so band[] is indexed by blockIdx.x * 256 + threadIdx.x.
+__device__ __forceinline__ const ClearanceProblem &cta_problem(const ClearanceArgs &A) {
+    int lo = 0, hi = A.n_prob - 1;  // the last k with cta0 <= blockIdx.x (a problem without CTAs shares cta0 with the next one)
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (A.prob[mid].cta0 <= (int64_t)blockIdx.x) lo = mid;
+        else hi = mid - 1;
     }
+    return A.prob[lo];
+}
+
+__global__ void __launch_bounds__(256) k_cl_count_multi(const __grid_constant__ ClearanceArgs A) {
+    __shared__ int s_list[kSweptMaxSamples];
+    __shared__ int s_n;
+    __shared__ int s_w[2][8];
+    const ClearanceProblem &pr = cta_problem(A);
+    const CtaItems C{((int64_t)blockIdx.x - pr.cta0) * blockDim.x, pr.n_items, pr.i0, pr.wy0, pr.nW, pr.all, pr.n_samp,
+                     A.samp + 3 * (int64_t)pr.samp0};
+    unsigned occ;
+    unsigned band = cta_band(A, C, s_list, &s_n, &occ);
+    if (pr.occ_only) band = 0u;
+    else occ = 0u;
+    A.band[(int64_t)blockIdx.x * blockDim.x + threadIdx.x] = band;
+    int n_band, n_occ;
+    block_scan256(__popc(band), s_w[0], &n_band);
+    block_scan256(__popc(occ), s_w[1], &n_occ);
+    if (threadIdx.x == 0) {
+        A.blk[blockIdx.x] = n_band;
+        if (n_occ) atomicAdd(A.n_occ, (unsigned long long)n_occ);
+    }
+}
+
+__global__ void __launch_bounds__(256) k_cl_write_multi(const __grid_constant__ ClearanceArgs A) {
+    __shared__ int s_w[8];
+    const unsigned band = A.band[(int64_t)blockIdx.x * blockDim.x + threadIdx.x];
+    int total;
+    const int64_t pos = (int64_t)A.blk[blockIdx.x] + block_scan256(__popc(band), s_w, &total);
+    if (!band) return;
+    const ClearanceProblem &pr = cta_problem(A);
+    const int64_t t = ((int64_t)blockIdx.x - pr.cta0) * blockDim.x + threadIdx.x;
+    write_cells(A, band, pr.i0 + (int)(t / pr.nW), pr.wy0 + (int)(t % pr.nW), pos);
 }
 
 }  // namespace
@@ -157,6 +224,8 @@ cudaError_t launch_clearance(int what, const ClearanceArgs &A, cudaStream_t st) 
     switch (what) {
         case 0: k_cl_count<<<nblk, 256, 0, st>>>(A); break;
         case 1: k_cl_write<<<nblk, 256, 0, st>>>(A); break;
+        case 2: k_cl_count_multi<<<nblk, 256, 0, st>>>(A); break;
+        case 3: k_cl_write_multi<<<nblk, 256, 0, st>>>(A); break;
         default: return cudaErrorInvalidValue;
     }
     return cudaGetLastError();

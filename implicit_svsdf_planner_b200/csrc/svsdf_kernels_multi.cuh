@@ -29,6 +29,8 @@ __device__ __forceinline__ void outer_multi_body(const KernelArgs &A, const Mult
     Ak.partials = A.partials + pr.part_off;
     Ak.inside_flag = A.inside_flag + pr.flag_off;
     Ak.inside_tstar = A.inside_tstar + pr.pt_off;
+    if (A.out_sdf) Ak.out_sdf = A.out_sdf + pr.pt_off;  // per-point outputs (svsdf_map_clearance_multi; null on the cost path)
+    if (A.out_tstar) Ak.out_tstar = A.out_tstar + pr.pt_off;
     outer_body<SHAPE, XFORM, BATCHED, SCALED>(Ak, S, Z, v, pr.grid);
 }
 template <int SHAPE, bool XFORM, bool BATCHED>
@@ -69,7 +71,9 @@ __device__ __forceinline__ void tma_reload_blob(double *smem_blob, const double 
 }
 
 // k_gsip_multi's view of the inside slots (gsip_body): slot s of the concatenated lists belongs to the last problem k with
-// ins_off[k] <= s (problems without inside points are skipped); the CTA's blob is reloaded when the problem changes.
+// ins_off[k] <= s (problems without inside points are skipped); the CTA's blob is reloaded when the problem changes.  The point index
+// it hands out counts from the start of the concatenated points (pt_off + the problem's own index), so the per-point outputs land at
+// the point's place in the concatenation.
 struct GsipMulti {
     const KernelArgs &A;
     const MultiArgs &M;
@@ -85,9 +89,9 @@ struct GsipMulti {
             else hi = mid - 1;
         }
         const MultiProblem &pr = M.prob[lo];
-        pt = A.inside_list[pr.pt_off + (slot - M.ins_off[lo])];
-        pts = A.points_xy + 2 * pr.pt_off;
-        tstar = A.inside_tstar + pr.pt_off;
+        pt = (int)pr.pt_off + A.inside_list[pr.pt_off + (slot - M.ins_off[lo])];
+        pts = A.points_xy;
+        tstar = A.inside_tstar;
         if (lo == *loaded) return false;
         if (*loaded < 0) {
             tma_load_blob(sblob, A.blob + pr.blob_off, pr.blob_doubles, bar);

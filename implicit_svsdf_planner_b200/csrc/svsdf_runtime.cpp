@@ -688,9 +688,17 @@ struct MultiItem {
 
 size_t align16(size_t b) { return (b + 15) & ~(size_t)15; }
 
+// svsdf_map_clearance_multi's evaluation: the items' points already on the device (concatenated in item order; MultiItem::pts and
+// ::out are not used) and svsdf_query's per-point values at the same places, instead of the cost and gradient.
+struct PointQuery {
+    const double *pts;
+    double *sdf, *tstar;
+};
+
 // One cost + gradient evaluation of every item with rc == SVSDF_OK, in one set of launches.  Items whose trajectory or points are
 // invalid get rc = SVSDF_ERR_INVALID and take no part; a CUDA error fails the call (and every item).  *ms: device time of the launches.
-int run_multi(svsdf_ctx *ctx, MultiItem *items, int n, float *ms) {
+// With pq: the per-point query of every item instead (no reduction, no finalize, nothing downloaded; multi_last_inside is kept).
+int run_multi(svsdf_ctx *ctx, MultiItem *items, int n, float *ms, const PointQuery *pq = nullptr) {
     if (ms) *ms = 0.0f;
     CK(cudaSetDevice(ctx->device));
     std::vector<MultiProblem> pr;
@@ -706,7 +714,7 @@ int run_multi(svsdf_ctx *ctx, MultiItem *items, int n, float *ms) {
         BlobLayout L;
         double D = 0.0;
         const char *msg = nullptr;
-        if (it.P < 0 || it.P > 2000000000LL || it.stride < 2 || (it.P > 0 && !it.pts) || !it.out ||
+        if (it.P < 0 || it.P > 2000000000LL || (!pq && (it.stride < 2 || (it.P > 0 && !it.pts) || !it.out)) ||
             traj_layout(it.N, it.T, it.coeffs, L, D, &msg) != SVSDF_OK) {
             it.rc = SVSDF_ERR_INVALID;
             continue;
@@ -744,10 +752,10 @@ int run_multi(svsdf_ctx *ctx, MultiItem *items, int n, float *ms) {
             ctx->err = "svsdf: trajectory blob does not fit in shared memory";
             return SVSDF_ERR_INVALID;
         }
-    // packed inputs: problem table | CTA maps (sparse, batched) | blobs | points (x, y)
+    // packed inputs: problem table | CTA maps (sparse, batched) | blobs | points (x, y; not with pq)
     const size_t o_prob = 0, o_ms = align16(o_prob + m * sizeof(MultiProblem)), o_mb = align16(o_ms + map_s.size() * sizeof(int)),
                  o_blob = align16(o_mb + map_b.size() * sizeof(int)), o_pts = align16(o_blob + (size_t)blob_tot * 8),
-                 in_bytes = align16(o_pts + (size_t)pt_tot * 16);
+                 in_bytes = align16(o_pts + (pq ? 0 : (size_t)pt_tot * 16));
     CK(ctx->h_multi_in.reserve(in_bytes));
     CK(ctx->d_multi_in.reserve(in_bytes));
     // the previous call's copy has completed (every call ends with a stream synchronise)
@@ -758,6 +766,7 @@ int run_multi(svsdf_ctx *ctx, MultiItem *items, int n, float *ms) {
     for (int j = 0; j < m; ++j) {
         const MultiItem &it = items[who[j]];
         fill_blob(reinterpret_cast<double *>(h + o_blob) + pr[j].blob_off, lay[j], it.T, it.coeffs, dur[j]);
+        if (pq) continue;
         double *xy = reinterpret_cast<double *>(h + o_pts) + 2 * pr[j].pt_off;
         if (it.stride == 2) {
             if (it.P) std::memcpy(xy, it.pts, (size_t)it.P * 16);
@@ -781,10 +790,11 @@ int run_multi(svsdf_ctx *ctx, MultiItem *items, int n, float *ms) {
     KernelArgs A;
     std::memset(&A, 0, sizeof(A));
     A.blob = reinterpret_cast<const double *>(d + o_blob);
-    A.points_xy = reinterpret_cast<const double *>(d + o_pts);
+    A.points_xy = pq ? pq->pts : reinterpret_cast<const double *>(d + o_pts);
     A.cp = ctx->cp;
     A.partials = reinterpret_cast<double *>(sc + s_part);
-    A.want_reduce = 1;
+    A.want_reduce = pq ? 0 : 1;
+    if (pq) { A.out_sdf = pq->sdf; A.out_tstar = pq->tstar; }
     A.want_gsip = 1;
     A.inside_flag = sc + s_flag;
     A.inside_tstar = reinterpret_cast<double *>(sc + s_ts);
@@ -818,10 +828,15 @@ int run_multi(svsdf_ctx *ctx, MultiItem *items, int n, float *ms) {
     }
     M.cta_map = nullptr;
     CK(K.compact_multi(A.inside_flag, A.inside_list, M, ctx->stream));
-    const GsipPlan gp = gsip_plan(ctx, ctx->multi_last_inside);
+    const GsipPlan gp = gsip_plan(ctx, pq ? -1 : ctx->multi_last_inside);  // the variant svsdf_query would pick
     CK(K.multi(2, A, M, ctx->shape, Z, gp.grid, (size_t)max_blob * sizeof(double), gp.wide, ctx->sm_count, ctx->stream));
+    launches += 2;
+    if (pq) {
+        ctx->launches += launches;
+        return SVSDF_OK;
+    }
     CK(K.finalize_multi(A.partials, A.gsip_contrib, A.gsip_piece, M, max_N, ctx->stream));
-    launches += 3;
+    launches += 1;
     if (ms) CK(cudaEventRecord(ctx->ev1, ctx->stream));
     CK(cudaMemcpyAsync(ctx->h_multi_out, M.out, (size_t)out_tot * 8, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
@@ -1948,38 +1963,82 @@ void svsdf_swept_free(svsdf_swept_mesh *mesh) {
 }
 
 // ---- svsdf_map_clearance (kernels: svsdf_clearance.cu; why the band is exact: DESIGN.md §7) -----------------------------------------
-int svsdf_map_clearance(svsdf_ctx *ctx, int N, const double *T, const double *coeffs, double d_max, svsdf_clearance *out) {
-    if (!ctx || !out) return SVSDF_ERR_INVALID;
+namespace {
+void clearance_empty(svsdf_clearance *out) {
     std::memset(out, 0, sizeof(*out));
     out->min_sdf = INFINITY;
     out->argmin = -1;
-    auto invalid = [&](const char *msg) {
-        ctx->err = msg;
-        return SVSDF_ERR_INVALID;
-    };
-    // the band proves only "outer value > d_max"; for d_max >= 0 that value is the whole answer (no interior branch), below 0 it is not
-    if (!(d_max >= 0.0)) return invalid("svsdf_map_clearance: d_max must be >= 0 or +INFINITY");
+}
+
+// svsdf_map_clearance's checks of one trajectory (D: its duration); on failure the message is in *err
+int clearance_traj(int N, const double *T, const double *coeffs, double &D, const char **err) {
     BlobLayout L;
-    double D = 0.0;
-    const char *msg = nullptr;
-    if (traj_layout(N, T, coeffs, L, D, &msg) != SVSDF_OK) return invalid(msg);
+    if (traj_layout(N, T, coeffs, L, D, err) != SVSDF_OK) return SVSDF_ERR_INVALID;
     for (int64_t e = 0; e < 18 * (int64_t)N; ++e)
-        if (!std::isfinite(coeffs[e])) return invalid("svsdf_map_clearance: non-finite trajectory coefficient");
-    if (!ctx->map()) {
-        ctx->err = "svsdf_map_clearance: map not set";
-        return SVSDF_ERR_NOT_READY;
-    }
-    if ((int64_t)ctx->map_X * ctx->map_Y > 2000000000LL) return invalid("svsdf_map_clearance: map has more than 2e9 columns");
-    // the band: rho and the samples of svsdf_swept_contour with iso = d_max
+        if (!std::isfinite(coeffs[e])) {
+            *err = "svsdf_map_clearance: non-finite trajectory coefficient";
+            return SVSDF_ERR_INVALID;
+        }
+    return SVSDF_OK;
+}
+
+// the band's samples: rho and the samples of svsdf_swept_contour with iso = d_max.  Returns `all` (every occupied column is in the band,
+// no samples): d_max = +inf or a shape without a far-field bound.
+bool clearance_samples(const svsdf_ctx *ctx, int N, const double *T, const double *coeffs, double D, double d_max, std::vector<double> &samp) {
     const ShapeParams &S = ctx->shape;
-    const bool all = !(S.rout < 1e299) || !std::isfinite(d_max);
-    std::vector<double> samp;
-    if (!all) {
-        const double rho = std::max(std::max(S.prune_rmin, S.rout + S.prune_scale * d_max), 0.0);
-        swept_samples(ctx, N, T, coeffs, D, rho, samp);
-        if ((int)(samp.size() / 3) > kSweptMaxSamples) return invalid("svsdf_map_clearance: too many path samples");
+    samp.clear();
+    if (!(S.rout < 1e299) || !std::isfinite(d_max)) return true;
+    const double rho = std::max(std::max(S.prune_rmin, S.rout + S.prune_scale * d_max), 0.0);
+    swept_samples(ctx, N, T, coeffs, D, rho, samp);
+    return false;
+}
+
+// The list and summary of one trajectory from its band (P cells in map order: ij, centres, values, t*): the cells with value <= d_max.
+int clearance_list(svsdf_ctx *ctx, int64_t P, const int32_t *h_ij, const double *h_xy, const double *h_sdf, const double *h_ts,
+                   unsigned long long n_occ, double d_max, svsdf_clearance *out) {
+    int64_t n_within = 0;
+    for (int64_t p = 0; p < P; ++p) {
+        if (!std::isfinite(h_sdf[p])) {
+            ctx->err = "svsdf_map_clearance: non-finite value";
+            return SVSDF_ERR_NONFINITE;
+        }
+        n_within += h_sdf[p] <= d_max;
     }
-    CK(cudaSetDevice(ctx->device));
+    out->ij = static_cast<int32_t *>(std::malloc((size_t)n_within * 8 + 16));
+    out->xy = static_cast<double *>(std::malloc((size_t)n_within * 16 + 16));
+    out->sdf = static_cast<double *>(std::malloc((size_t)n_within * 8 + 16));
+    out->tstar = static_cast<double *>(std::malloc((size_t)n_within * 8 + 16));
+    if (!out->ij || !out->xy || !out->sdf || !out->tstar) {
+        svsdf_clearance_free(out);
+        ctx->err = "svsdf_map_clearance: out of host memory";
+        return SVSDF_ERR_INVALID;
+    }
+    int64_t k = 0, n_coll = 0;
+    for (int64_t p = 0; p < P; ++p) {
+        const double v = h_sdf[p];
+        if (!(v <= d_max)) continue;
+        out->ij[2 * k] = h_ij[2 * p];
+        out->ij[2 * k + 1] = h_ij[2 * p + 1];
+        out->xy[2 * k] = h_xy[2 * p];
+        out->xy[2 * k + 1] = h_xy[2 * p + 1];
+        out->sdf[k] = v;
+        out->tstar[k] = h_ts[p];
+        n_coll += v <= 0.0;
+        if (v < out->min_sdf) {  // strict: the first in list order among ties
+            out->min_sdf = v;
+            out->argmin = k;
+        }
+        ++k;
+    }
+    out->n_occupied = (int64_t)n_occ;
+    out->n_evaluated = P;
+    out->n_within = n_within;
+    out->n_colliding = n_coll;
+    return SVSDF_OK;
+}
+
+// the map fields of the clearance kernels' arguments
+ClearanceArgs clearance_args(const svsdf_ctx *ctx) {
     ClearanceArgs A;
     std::memset(&A, 0, sizeof(A));
     A.map = ctx->map();
@@ -1988,6 +2047,40 @@ int svsdf_map_clearance(svsdf_ctx *ctx, int N, const double *T, const double *co
     A.ox = ctx->map_ox; A.oy = ctx->map_oy; A.res = ctx->map_res;
     A.wy0 = A.h / 32;
     A.nW = (A.h + A.Y - 1) / 32 - A.wy0 + 1;
+    return A;
+}
+
+// cell index range [lo, hi] of the map axis (n cells, origin o, resolution res) whose centres may lie in [a, b]: outward by one cell
+// beyond the rounding of the centres, clipped to the map (lo > hi: none)
+void cell_range(double a, double b, double o, double res, int n, int &lo, int &hi) {
+    const double l = std::floor((a - o) / res - 0.5) - 1.0, h = std::ceil((b - o) / res - 0.5) + 1.0;  // a, b: not NaN, maybe infinite
+    lo = (int)std::min(std::max(l, 0.0), (double)n);
+    hi = (int)std::max(std::min(h, (double)n - 1.0), -1.0);
+}
+}  // namespace
+
+int svsdf_map_clearance(svsdf_ctx *ctx, int N, const double *T, const double *coeffs, double d_max, svsdf_clearance *out) {
+    if (!ctx || !out) return SVSDF_ERR_INVALID;
+    clearance_empty(out);
+    auto invalid = [&](const char *msg) {
+        ctx->err = msg;
+        return SVSDF_ERR_INVALID;
+    };
+    // the band proves only "outer value > d_max"; for d_max >= 0 that value is the whole answer (no interior branch), below 0 it is not
+    if (!(d_max >= 0.0)) return invalid("svsdf_map_clearance: d_max must be >= 0 or +INFINITY");
+    double D = 0.0;
+    const char *msg = nullptr;
+    if (clearance_traj(N, T, coeffs, D, &msg) != SVSDF_OK) return invalid(msg);
+    if (!ctx->map()) {
+        ctx->err = "svsdf_map_clearance: map not set";
+        return SVSDF_ERR_NOT_READY;
+    }
+    if ((int64_t)ctx->map_X * ctx->map_Y > 2000000000LL) return invalid("svsdf_map_clearance: map has more than 2e9 columns");
+    std::vector<double> samp;
+    const bool all = clearance_samples(ctx, N, T, coeffs, D, d_max, samp);
+    if ((int)(samp.size() / 3) > kSweptMaxSamples) return invalid("svsdf_map_clearance: too many path samples");
+    CK(cudaSetDevice(ctx->device));
+    ClearanceArgs A = clearance_args(ctx);
     A.n_items = (int64_t)A.X * A.nW;
     A.all = all ? 1 : 0;
     A.n_samp = (int)(samp.size() / 3);
@@ -2036,47 +2129,144 @@ int svsdf_map_clearance(svsdf_ctx *ctx, int N, const double *T, const double *co
         CK(cudaMemcpyAsync(hs, ctx->d_cl_point, o_end, cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
     }
-    const int32_t *h_ij = reinterpret_cast<const int32_t *>(hs);
-    const double *h_xy = reinterpret_cast<const double *>(hs + o_pts), *h_sdf = reinterpret_cast<const double *>(hs + o_sdf),
-                 *h_ts = reinterpret_cast<const double *>(hs + o_ts);
-    int64_t n_within = 0;
-    for (int64_t p = 0; p < P; ++p) {
-        if (!std::isfinite(h_sdf[p])) {
-            ctx->err = "svsdf_map_clearance: non-finite value";
-            return SVSDF_ERR_NONFINITE;
-        }
-        n_within += h_sdf[p] <= d_max;
-    }
-    out->ij = static_cast<int32_t *>(std::malloc((size_t)n_within * 8 + 16));
-    out->xy = static_cast<double *>(std::malloc((size_t)n_within * 16 + 16));
-    out->sdf = static_cast<double *>(std::malloc((size_t)n_within * 8 + 16));
-    out->tstar = static_cast<double *>(std::malloc((size_t)n_within * 8 + 16));
-    if (!out->ij || !out->xy || !out->sdf || !out->tstar) {
-        svsdf_clearance_free(out);
-        ctx->err = "svsdf_map_clearance: out of host memory";
+    return clearance_list(ctx, P, reinterpret_cast<const int32_t *>(hs), reinterpret_cast<const double *>(hs + o_pts),
+                          reinterpret_cast<const double *>(hs + o_sdf), reinterpret_cast<const double *>(hs + o_ts), n_occ, d_max, out);
+}
+
+// The bands of all problems in one count / scan / write, then one multi-problem evaluation of the concatenated bands (DESIGN.md §7).
+int svsdf_map_clearance_multi(svsdf_ctx *ctx, int n, const svsdf_clearance_problem *problems, double d_max, svsdf_clearance *out,
+                              int *status_out) {
+    if (!ctx) return SVSDF_ERR_INVALID;
+    auto invalid = [&](const std::string &msg) {
+        ctx->err = msg;
         return SVSDF_ERR_INVALID;
+    };
+    if (n < 0 || n > kMaxMultiProblems || (n > 0 && (!problems || !out || !status_out)))
+        return invalid("svsdf_map_clearance_multi: needs 0 <= n <= 65535 and the problem, output and status arrays");
+    for (int k = 0; k < n; ++k) {
+        clearance_empty(&out[k]);
+        status_out[k] = SVSDF_ERR_INVALID;
     }
-    int64_t k = 0, n_coll = 0;
-    for (int64_t p = 0; p < P; ++p) {
-        const double v = h_sdf[p];
-        if (!(v <= d_max)) continue;
-        out->ij[2 * k] = h_ij[2 * p];
-        out->ij[2 * k + 1] = h_ij[2 * p + 1];
-        out->xy[2 * k] = h_xy[2 * p];
-        out->xy[2 * k + 1] = h_xy[2 * p + 1];
-        out->sdf[k] = v;
-        out->tstar[k] = h_ts[p];
-        n_coll += v <= 0.0;
-        if (v < out->min_sdf) {  // strict: the first in list order among ties
-            out->min_sdf = v;
-            out->argmin = k;
+    if (!(d_max >= 0.0)) return invalid("svsdf_map_clearance_multi: d_max must be >= 0 or +INFINITY");
+    std::vector<double> dur(n);
+    for (int k = 0; k < n; ++k) {
+        const char *msg = nullptr;
+        if (clearance_traj(problems[k].N, problems[k].T, problems[k].coeffs, dur[k], &msg) != SVSDF_OK)
+            return invalid(std::string("svsdf_map_clearance_multi: problem ") + std::to_string(k) + ": " + msg);
+    }
+    if (n == 0) return SVSDF_OK;
+    if (!ctx->map()) {
+        ctx->err = "svsdf_map_clearance_multi: map not set";
+        return SVSDF_ERR_NOT_READY;
+    }
+    if ((int64_t)ctx->map_X * ctx->map_Y > 2000000000LL) return invalid("svsdf_map_clearance_multi: map has more than 2e9 columns");
+    ClearanceArgs A = clearance_args(ctx);
+    // per problem: its samples and its reach rectangle (the bounding box of the samples' discs, padded outwards by a relative margin far
+    // above the rounding of the kernel's test dx*dx + dy*dy <= r*r, then by one cell; clipped to the map), padded to whole CTAs
+    std::vector<ClearanceProblem> cp(n + 1);
+    std::vector<double> samp_all, samp;
+    int64_t cta = 0, cells = 0;
+    for (int k = 0; k <= n; ++k) {
+        ClearanceProblem &c = cp[k];
+        std::memset(&c, 0, sizeof(c));
+        c.cta0 = cta;
+        int i0 = 0, i1 = A.X - 1, j0 = 0, j1 = A.Y - 1;
+        if (k == n) {
+            c.all = c.occ_only = 1;
+        } else {
+            const svsdf_clearance_problem &p = problems[k];
+            c.all = clearance_samples(ctx, p.N, p.T, p.coeffs, dur[k], d_max, samp) ? 1 : 0;
+            c.n_samp = (int)(samp.size() / 3);
+            if (c.n_samp > kSweptMaxSamples) return invalid("svsdf_map_clearance_multi: too many path samples");
+            c.samp0 = (int)(samp_all.size() / 3);
+            samp_all.insert(samp_all.end(), samp.begin(), samp.end());
+            if (!c.all) {
+                double x0 = INFINITY, x1 = -INFINITY, y0 = INFINITY, y1 = -INFINITY;
+                for (int s = 0; s < c.n_samp; ++s) {
+                    const double sx = samp[3 * s], sy = samp[3 * s + 1], r = samp[3 * s + 2];
+                    const double m = r + 1e-9 * (std::fabs(sx) + std::fabs(sy) + r + 1.0);
+                    x0 = std::min(x0, sx - m); x1 = std::max(x1, sx + m);
+                    y0 = std::min(y0, sy - m); y1 = std::max(y1, sy + m);
+                }
+                cell_range(x0, x1, A.ox, A.res, A.X, i0, i1);
+                cell_range(y0, y1, A.oy, A.res, A.Y, j0, j1);
+            }
         }
-        ++k;
+        if (i0 <= i1 && j0 <= j1) {
+            c.i0 = i0;
+            c.wy0 = (j0 + A.h) / 32;
+            c.nW = (j1 + A.h) / 32 - c.wy0 + 1;
+            c.n_items = (int64_t)(i1 - i0 + 1) * c.nW;
+            if (k < n) cells += 32 * c.n_items;
+        } else {
+            c.nW = 1;
+        }
+        cta += (c.n_items + 255) / 256;
     }
-    out->n_occupied = (int64_t)n_occ;
-    out->n_evaluated = P;
-    out->n_within = n_within;
-    out->n_colliding = n_coll;
+    if (cells > 2147483647LL || cta > 2147483647LL / 256)
+        return invalid("svsdf_map_clearance_multi: the problems' rectangles hold more than 2^31 - 1 cells");
+    CK(cudaSetDevice(ctx->device));
+    const int nblk = (int)cta;
+    A.n_items = (int64_t)nblk * 256;
+    A.n_prob = n + 1;
+    // small: header [0] occupied columns (u64), [8] band cells (int) | per-CTA counts | problem table | samples
+    const size_t off_blk = 64, off_prob = align16(off_blk + (size_t)(nblk + 1) * 4), off_samp = align16(off_prob + cp.size() * sizeof(ClearanceProblem)),
+                 small = off_samp + samp_all.size() * 8;
+    CK(ctx->d_cl_small.reserve(small));
+    CK(ctx->d_cl_band.reserve((size_t)A.n_items * 4));
+    CK(ctx->h_stage.reserve(small));
+    unsigned char *hs = ctx->h_stage;
+    std::memset(hs, 0, off_prob);
+    std::memcpy(hs + off_prob, cp.data(), cp.size() * sizeof(ClearanceProblem));
+    if (!samp_all.empty()) std::memcpy(hs + off_samp, samp_all.data(), samp_all.size() * 8);
+    A.n_occ = reinterpret_cast<unsigned long long *>(ctx->d_cl_small.get());
+    A.blk = reinterpret_cast<int *>(ctx->d_cl_small + off_blk);
+    A.prob = reinterpret_cast<const ClearanceProblem *>(ctx->d_cl_small + off_prob);
+    A.samp = reinterpret_cast<const double *>(ctx->d_cl_small + off_samp);
+    A.band = reinterpret_cast<unsigned *>(ctx->d_cl_band.get());
+    cudaStream_t st = ctx->stream;
+    CK(cudaMemcpyAsync(ctx->d_cl_small, hs, small, cudaMemcpyHostToDevice, st));
+    CK(launch_clearance(2, A, st));
+    CK(launch_swept_scan(A.blk, nblk, 1, reinterpret_cast<int *>(ctx->d_cl_small + 8), st));
+    CK(cudaMemcpyAsync(hs, ctx->d_cl_small, off_prob, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    ctx->launches += 2;
+    unsigned long long n_occ;
+    std::memcpy(&n_occ, hs, 8);
+    std::vector<int64_t> off(n + 1);  // problem k's band: cells off[k] .. off[k + 1] - 1 of the concatenation
+    for (int k = 0; k <= n; ++k) off[k] = reinterpret_cast<const int *>(hs + off_blk)[cp[k].cta0];
+    const int64_t P = off[n];
+    const size_t o_pts = align16((size_t)P * 8), o_sdf = o_pts + (size_t)P * 16, o_ts = o_sdf + (size_t)P * 8, o_end = o_ts + (size_t)P * 8;
+    if (P > 0) {
+        CK(ctx->d_cl_point.reserve(o_end + 16));
+        A.ij = reinterpret_cast<int *>(ctx->d_cl_point.get());
+        A.pts = reinterpret_cast<double *>(ctx->d_cl_point + o_pts);
+        CK(launch_clearance(3, A, st));
+        ctx->launches += 1;
+        // the problems with a band, in problem order: their points are the concatenation's, in the same order
+        std::vector<MultiItem> items;
+        for (int k = 0; k < n; ++k) {
+            if (off[k + 1] == off[k]) continue;
+            MultiItem it;
+            it.N = problems[k].N; it.T = problems[k].T; it.coeffs = problems[k].coeffs; it.P = off[k + 1] - off[k];
+            items.push_back(it);
+        }
+        const PointQuery pq{A.pts, reinterpret_cast<double *>(ctx->d_cl_point + o_sdf), reinterpret_cast<double *>(ctx->d_cl_point + o_ts)};
+        int rc = run_multi(ctx, items.data(), (int)items.size(), nullptr, &pq);
+        if (rc) return rc;
+        for (const MultiItem &it : items)
+            if (it.rc != SVSDF_OK) return invalid("svsdf_map_clearance_multi: a problem was refused by the evaluation");
+        CK(ctx->h_stage.reserve(o_end));
+        hs = ctx->h_stage;
+        CK(cudaMemcpyAsync(hs, ctx->d_cl_point, o_end, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+    }
+    for (int k = 0; k < n; ++k) {
+        const int64_t o = off[k];
+        status_out[k] = clearance_list(ctx, off[k + 1] - o, reinterpret_cast<const int32_t *>(hs) + 2 * o, reinterpret_cast<const double *>(hs + o_pts) + 2 * o,
+                                       reinterpret_cast<const double *>(hs + o_sdf) + o, reinterpret_cast<const double *>(hs + o_ts) + o, n_occ,
+                                       d_max, &out[k]);
+    }
     return SVSDF_OK;
 }
 

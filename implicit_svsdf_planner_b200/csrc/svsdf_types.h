@@ -224,6 +224,16 @@ struct SweptArgs {
 
 // svsdf_map_clearance (svsdf_clearance.cu): the occupied map columns near a trajectory.  One item per 32-cell word of a map row (the
 // words that hold real cells, rows 0 .. X - 1), 256 items per CTA, row-major: the CTA order is the map order.
+// svsdf_map_clearance_multi: problem k covers the words of its reach rectangle, row-major, padded to whole CTAs (cta0[k] ..).
+struct ClearanceProblem {
+    int64_t cta0;              // first CTA
+    int64_t n_items;           // rows * nW (0: the rectangle misses the map)
+    int i0, wy0, nW;           // first row, first word of a row, words per row
+    int all;                   // every occupied column of the rectangle is in the band
+    int samp0, n_samp;         // its samples in ClearanceArgs::samp
+    int occ_only;              // the last segment: the whole map, counts the occupied columns, no band
+    int pad_;
+};
 struct ClearanceArgs {
     const unsigned char *map;  // Z layers of (X + 2h) x row_bytes, MSB-first bits along y (svsdf_set_map / svsdf_set_map3d)
     int X, Y, h, row_bytes, Z;
@@ -239,6 +249,8 @@ struct ClearanceArgs {
     unsigned long long *n_occ; // occupied columns of the map
     int *ij;                   // [P][2] band cells in map order: (i, j)
     double *pts;               // [P][2] their centres
+    int n_prob;                // svsdf_map_clearance_multi: problems + 1 (the occupied-column segment); 0 for the single call
+    const ClearanceProblem *prob;
 };
 
 // K5 (svsdf_frontend.cu): collision kernels of the A* front end

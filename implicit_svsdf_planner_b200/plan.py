@@ -76,9 +76,12 @@ def rot_z(yaw: float) -> np.ndarray:
 
 def generate_traj(ctx: "api.Context", cmap: CloudMap, start_xy, goal_xy, kernel_size: int = scenes.YAML["kernel_size"], kernel_yaw_num: int = 18,
                   front_end_safeh: float = 0.0, traj_parlength: float = 3.0, inittime: float = scenes.YAML["inittime"],
-                  mid_cfg: Optional["api.MidConfig"] = None, lbfgs_params=None, max_path: int = 4096, certify: bool = False) -> dict:
+                  mid_cfg: Optional["api.MidConfig"] = None, lbfgs_params=None, max_path: int = 4096, certify: bool = False,
+                  repair: int = 0) -> dict:
     """generatePath + generateTraj for one start / goal on the map `cmap` (the context's shape is the robot).  certify=True adds
-    `clearance` (see certificate) to a result that reached the back end."""
+    `clearance` (see certificate) to a result that reached the back end.  repair=R > 0 (implies certify) then runs up to R repair rounds
+    (see Repair): the top-level trajectory keys and `clearance` describe the final trajectory, `repair` what the rounds did, and
+    the context's resident points are the last query set."""
     X, Y, Z = cmap.occ.shape
     res = cmap.res
     ctx.set_map3d(pack_map_kernel3d(cmap.occ, kernel_size), X, Y, Z, kernel_size, cmap.boundary_min, res)
@@ -104,16 +107,78 @@ def generate_traj(ctx: "api.Context", cmap: CloudMap, start_xy, goal_xy, kernel_
                mid=dict(status=int(rc_mid), cost=float(cost_mid), iterations=int(it_mid), T=T_mid), cost_at_warm_start=float(f0),
                final_cost=float(st["final_cost"]), iterations=int(st["iterations"]), evaluations=int(st["evaluations"]), T=T, coeffs=b, x=x,
                seconds=float(st["seconds"]))
-    if certify:
+    if repair > 0:
+        rp = Repair(ctx.get_points())
+        cl = ctx.map_clearance(T, np.asarray(b).reshape(-1), ctx.safety_hor)
+        while rp.next_points(cl, repair) is not None:
+            ctx.set_points(rp.points)
+            rc, x, T, b, st = ctx.optimize(init_s, final_s, x, N, params)
+            out.update(ok=rc >= 0, status=int(rc), final_cost=float(st["final_cost"]), iterations=int(st["iterations"]),
+                       evaluations=int(st["evaluations"]), T=T, coeffs=b, x=x)
+            cl = ctx.map_clearance(T, np.asarray(b).reshape(-1), ctx.safety_hor)
+        out["clearance"], out["repair"] = certificate_of(cl), rp.summary()
+    elif certify:
         out["clearance"] = certificate(ctx, T, b)
     return out
+
+
+def _xy(points) -> np.ndarray:
+    """The x and y columns of a [P, >= 2] point array (P may be 0)."""
+    p = np.asarray(points, dtype=np.float64)
+    return p.reshape(p.shape[0], -1)[:, :2] if p.size else np.empty((0, 2))
+
+
+def new_cells(cells_xy, query_xy) -> np.ndarray:
+    """The repair rule: the centres of the listed cells (a clearance's xy, in its list order) that are not bit-equal, in both x and y, to
+    a point of the query set (query_xy [P, >= 2]; repeated (x, y), e.g. z layers of one column, count once).  One row per new column, in
+    list order.  Exact: clearance centres round as the extraction rounds the query points."""
+    c = np.ascontiguousarray(np.asarray(cells_xy, dtype=np.float64).reshape(-1, 2))
+    q = np.ascontiguousarray(_xy(query_xy))
+    seen = set(map(tuple, q.view(np.uint64).tolist()))
+    keep = []
+    for k, key in enumerate(map(tuple, c.view(np.uint64).tolist())):
+        if key not in seen:
+            seen.add(key)
+            keep.append(k)
+    return c[keep]
+
+
+class Repair:
+    """The bookkeeping of generate_traj's and plan_batch's repair rounds for one problem.  Each round certifies the current trajectory at
+    d_max = safety_hor, appends the new cells (new_cells) to the query set and re-runs the back end from the previous x; it stops when a
+    certificate has no new cell ("closed": the query set holds every occupied cell within the penalty's horizon) or after `limit`
+    re-runs ("limit")."""
+
+    def __init__(self, points):
+        self.points = _xy(points)
+        self.added, self.min_sdf, self.stopped = [], [], None
+
+    def next_points(self, cl: "api.Clearance", limit: int):
+        """Takes the certificate of the current trajectory; returns the augmented query set for the next back-end run, or None when
+        the rounds stop."""
+        self.min_sdf.append(float(cl.min_sdf))
+        new = new_cells(cl.xy, self.points)
+        if len(new) == 0 or len(self.added) >= limit:
+            self.stopped = "closed" if len(new) == 0 else "limit"
+            return None
+        self.added.append(new)
+        self.points = np.concatenate([self.points, new])
+        return self.points
+
+    def summary(self) -> dict:
+        return dict(rounds=len(self.added), added=np.concatenate(self.added) if self.added else np.empty((0, 2)),
+                    added_per_round=[len(a) for a in self.added], min_sdf_per_round=self.min_sdf, stopped=self.stopped)
 
 
 def certificate(ctx: "api.Context", T, coeffs) -> dict:
     """The trajectory checked against every occupied cell of the context's map (svsdf_map_clearance, the reference's getMinSVSDF) with
     d_max = the context's safety_hor: the least swept-volume SDF value over the cells within the penalty's horizon, where it is reached,
     and collision_free = min_sdf > 0.  `ok` says only that the solver returned status >= 0; this says whether the robot misses the map."""
-    c = ctx.map_clearance(T, np.asarray(coeffs).reshape(-1), ctx.safety_hor)
+    return certificate_of(ctx.map_clearance(T, np.asarray(coeffs).reshape(-1), ctx.safety_hor))
+
+
+def certificate_of(c: "api.Clearance") -> dict:
+    """certificate's summary of a clearance at d_max = safety_hor."""
     k = c.argmin
     return dict(min_sdf=c.min_sdf, argmin_xy=c.xy[k].copy() if k >= 0 else None, t_star=float(c.tstar[k]) if k >= 0 else None,
                 n_colliding=c.n_colliding, n_within=c.n_within, n_evaluated=c.n_evaluated, collision_free=bool(c.min_sdf > 0.0))
@@ -132,7 +197,8 @@ _ASTAR_REASON = {0: "start or goal outside the map", 2: "front end found no path
 def plan_batch(ctx: "api.Context", cmap: CloudMap, starts, goals, kernel_size: int = scenes.YAML["kernel_size"], kernel_yaw_num: int = 18,
                front_end_safeh: float = 0.0, traj_parlength: float = 3.0, inittime: float = scenes.YAML["inittime"],
                mid_cfg: Optional["api.MidConfig"] = None, lbfgs_params=None, max_path: int = 4096, max_in_flight: int = 0,
-               workers: Optional[int] = None, stats: Optional[dict] = None, back_end: bool = True, certify: bool = False) -> list:
+               workers: Optional[int] = None, stats: Optional[dict] = None, back_end: bool = True, certify: bool = False,
+               repair: int = 0) -> list:
     """generate_traj for n start / goal pairs on one map: one device A* launch for all searches (svsdf_front_astar_device), per problem the
     waypoints, the query points (extract_points3d, on the context) and the warm start (mid_get_ori_traj, on a thread pool: the mid end is
     host code and ctypes releases the GIL), then ONE lock-step back end (svsdf_optimize_lockstep) for every problem whose mid end succeeded.
@@ -140,8 +206,10 @@ def plan_batch(ctx: "api.Context", cmap: CloudMap, starts, goals, kernel_size: i
     a failed problem has ok=False and the reason (an exception of one problem's extraction or mid end fails that problem only).
     stats (optional dict) receives the wall seconds of each stage, the back end's rounds and its kernel launches.  back_end=False stops
     before the back end: the problems that would enter it are returned with its inputs (init_s, final_s, x0, points) instead.
-    certify=True adds generate_traj's `clearance` to every problem that went through the back end (one svsdf_map_clearance per problem,
-    after the back end; stats then also holds its wall seconds, certify_s)."""
+    certify=True adds generate_traj's `clearance` to every problem that went through the back end (one svsdf_map_clearance_multi for
+    all of them, after the back end; stats then also holds its wall seconds, certify_s).  repair=R > 0 (implies certify) adds
+    generate_traj(repair=R)'s keys and bits: each round is one lock-step back end over the problems that gained cells and one
+    svsdf_map_clearance_multi over them (stats: repair_s, the rounds' wall seconds, and repair_rounds)."""
     st = np.asarray(starts, dtype=np.float64).reshape(-1, 2)
     go = np.asarray(goals, dtype=np.float64).reshape(-1, 2)
     n = st.shape[0]
@@ -219,11 +287,42 @@ def plan_batch(ctx: "api.Context", cmap: CloudMap, starts, goals, kernel_size: i
                       expansions=int(expansions[q]), mid=p["mid"], cost_at_warm_start=r["cost_at_start"], final_cost=float(r["final_cost"]),
                       iterations=int(r["iterations"]), evaluations=int(r["evaluations"]), T=r["T"], coeffs=r["coeffs"], x=r["x"],
                       seconds=float(r["seconds"]), points=p["points"])
-    if certify:
+    if certify or repair > 0:
         t5 = time.perf_counter()
-        for p in back:
-            r = out[p["q"]]
-            r["clearance"] = certificate(ctx, r["T"], r["coeffs"])
+        final = dict(zip([p["q"] for p in back], certify_all(ctx, [out[p["q"]] for p in back])))
+        t6 = time.perf_counter()
         if stats is not None:
-            stats["certify_s"] = time.perf_counter() - t5
+            stats["certify_s"] = t6 - t5
+        if repair > 0:
+            reps = {p["q"]: Repair(p["points"]) for p in back}
+            live, n_rounds = back, 0
+            while True:  # one lock-step back end and one certification per round, over the problems that gained cells
+                todo = [(p, reps[p["q"]].next_points(final[p["q"]], repair)) for p in live]
+                todo = [(p, pts) for p, pts in todo if pts is not None]
+                if not todo:
+                    break
+                results, _ = ctx.optimize_lockstep([dict(N=p["N"], init_s=p["init_s"], final_s=p["final_s"], x0=out[p["q"]]["x"], points=pts)
+                                                    for p, pts in todo], params, max_in_flight)
+                for (p, _), r in zip(todo, results):
+                    out[p["q"]].update(ok=r["status"] >= 0, status=r["status"], final_cost=float(r["final_cost"]), iterations=int(r["iterations"]),
+                                       evaluations=int(r["evaluations"]), T=r["T"], coeffs=r["coeffs"], x=r["x"])
+                live = [p for p, _ in todo]
+                final.update(zip([p["q"] for p in live], certify_all(ctx, [out[p["q"]] for p in live])))
+                n_rounds += 1
+            for q, rp in reps.items():
+                out[q]["repair"] = rp.summary()
+            if stats is not None:
+                stats.update(repair_s=time.perf_counter() - t6, repair_rounds=n_rounds)
+        for q, c in final.items():
+            out[q]["clearance"] = certificate_of(c)
     return out
+
+
+def certify_all(ctx: "api.Context", results: list) -> list:
+    """map_clearance_multi of every result's trajectory at d_max = safety_hor, in one set of launches.  A problem whose certificate
+    fails raises, as certificate does."""
+    cls = ctx.map_clearance_multi([(r["T"], np.asarray(r["coeffs"]).reshape(-1)) for r in results], ctx.safety_hor)
+    for c in cls:
+        if isinstance(c, Exception):
+            raise c
+    return cls

@@ -212,6 +212,24 @@ typedef struct {
 } svsdf_clearance;
 int svsdf_map_clearance(svsdf_ctx *ctx, int N, const double *T, const double *coeffs, double d_max, svsdf_clearance *out);
 void svsdf_clearance_free(svsdf_clearance *c);
+/* svsdf_map_clearance_multi: svsdf_map_clearance of n trajectories against the context's map in one set of launches.  out[k] equals
+ * svsdf_map_clearance(ctx, N_k, T_k, coeffs_k, d_max, ...) on the same context bit for bit (counts, list and summary), and status_out[k]
+ * is the status that call would return (SVSDF_OK or SVSDF_ERR_NONFINITE; a problem whose status is not OK has no arrays allocated).
+ *   0 <= n <= 65535; n = 0 does nothing.  The call is refused before any work (SVSDF_ERR_INVALID, nothing allocated) for a bad d_max,
+ *   any bad trajectory (N outside 1 .. 64, bad durations, non-finite coefficients), or when the problems' reach rectangles together hold
+ *   more than 2^31 - 1 cells; SVSDF_ERR_NOT_READY without a map.
+ *   Each problem evaluates only the occupied columns of its reach rectangle (the bounding box of its samples' reach, padded outwards):
+ *   the band is that of the single call.  The occupied columns of the map are counted once per call.  A fixed number of kernel
+ *   launches, whatever n and the map size (none of the evaluation's when no problem has a band); the context's resident points,
+ *   last_n_inside and everything svsdf_cost_grad and svsdf_cost_grad_multi depend on keep their values.  Release each out[k] with
+ *   svsdf_clearance_free. */
+typedef struct {
+    int N;
+    const double *T;       /* N */
+    const double *coeffs;  /* 18 N, column-major 6N x 3 */
+} svsdf_clearance_problem;
+int svsdf_map_clearance_multi(svsdf_ctx *ctx, int n, const svsdf_clearance_problem *problems, double d_max, svsdf_clearance *out,
+                              int *status_out);
 
 /* R2: per-point swept-volume SDF query on the trajectory given by (N, T, coeffs).
  * pts: P x 3 (x, y, z) host doubles (z ignored).  Outputs (host, may be NULL): sdf[P], tstar[P], grad3[3P]
