@@ -191,6 +191,14 @@ __device__ __forceinline__ void rel_from_pose(double px, double py, double x, do
     ry = -sy * d0 + cy * d1;
 }
 
+// one record of the pose windows (read-only during the kernel that reads it): two 16-byte loads of one 32-byte sector
+__device__ __forceinline__ PoseRec ld_pose(const PoseRec *p) {
+    const double2 a = __ldg(reinterpret_cast<const double2 *>(p)), b = __ldg(reinterpret_cast<const double2 *>(p) + 1);
+    PoseRec r;
+    r.x = a.x; r.y = a.y; r.c = b.x; r.s = b.y;
+    return r;
+}
+
 // Deformable robot (useScale == true): getScale(t) = diag(sx, sy, 1) (ScaleSched) and the diagonal (ix, iy) of St.inverse()
 // by Eigen 3.3's size-3 cofactor formula: 1/det with det = sy * sx, then ix = sy * (1/det), iy = sx * (1/det) — not 1/sx.
 // t is the absolute time of the sample.
@@ -278,10 +286,11 @@ struct OuterResult {
 // accepted halving is the first (largest step) whose candidate decreases f.
 // SCALED (deformable robot, schedule *Z): only the descent evaluates the scaled shape; choiceTInit's 2-argument overload
 // (:538-581) never reads its template flag, so the four seed layers stay rigid.
+// w2 / w3: the pose windows of layers 2 and 3 (thread_choice_t_init); null: the layer evaluates the trajectory.
 template <int SHAPE, bool XFORM, bool SCALED = false>
 __device__ __forceinline__ OuterResult solve_outer(const TrajView &tv, const ShapeParams &S, double px, double py,
-                                                   bool have_seed = false, double seed_in = 0.0, double min_in = 1e9,
-                                                   const ScaleSched *Z = nullptr) {
+                                                   const PoseRec *w2, const PoseRec *w3, bool have_seed = false,
+                                                   double seed_in = 0.0, double min_in = 1e9, const ScaleSched *Z = nullptr) {
     const int lane = threadIdx.x & 31;
     const double D = tv.D;
     const double INF = __longlong_as_double(0x7ff0000000000000LL);
@@ -293,6 +302,7 @@ __device__ __forceinline__ OuterResult solve_outer(const TrajView &tv, const Sha
     // round: this already contains the minimum almost always), then every block of 32 is revisited and only samples with
     // |p - x_k| <= min + rout are evaluated (usually none).  (Skipped when the caller ran choiceTInit thread-per-point.)
     double min_dis = have_seed ? min_in : 1e9, seed = have_seed ? seed_in : 0.0;
+    int kb = -1;
     if (!have_seed) {
         const uint32_t row = 8u * (uint32_t)tv.K1pad;
         const int K1 = tv.K1;
@@ -311,7 +321,6 @@ __device__ __forceinline__ OuterResult solve_outer(const TrajView &tv, const Sha
             k0 = __shfl_sync(FULL, k0, src);
         }
         const int w0 = max(0, min(k0 - 16, K1 - 32));   // window [w0, w0 + 32) (whole lattice when K1 <= 32)
-        int kb = -1;
         double thr2 = INF;
         // it = -1: the window; it >= 0: block it (samples of the window are not evaluated twice)
         for (int it = -1; 32 * it < K1; ++it) {
@@ -348,6 +357,9 @@ __device__ __forceinline__ OuterResult solve_outer(const TrajView &tv, const Sha
     if (!have_seed) {
         double dt = 0.15;
         int hint = 0;
+        // layers 2 and 3: lane m reads sample m's pose from the window of kb (layer 2) or of (kb, m2) (layer 3) when it is built
+        const PoseRec *win = w2 ? w2 + kWinLen * (kb + 1) : nullptr;
+        int m2 = -1;
 #pragma unroll 1
         for (int layer = 2; layer <= 4; ++layer) {
             dt *= 0.1;
@@ -356,16 +368,26 @@ __device__ __forceinline__ OuterResult solve_outer(const TrajView &tv, const Sha
 #pragma unroll
             for (int i = 0; i < 20; ++i)
                 if (i < lane) t += dt;  // lane k (<= 20) holds t0 + dt added k times (same rounding as the loop)
-            const double fq = eval_sdf<SHAPE, XFORM>(tv, S, px, py, t, hint);
+            double fq;
+            if (win) {
+                const PoseRec ps = ld_pose(win + min(lane, kWinLen - 1));
+                double rx, ry;
+                rel_from_pose(px, py, ps.x, ps.y, ps.c, ps.s, rx, ry);
+                fq = dev::shape_sdf<SHAPE, XFORM>(S, rx, ry);
+            } else {
+                fq = eval_sdf<SHAPE, XFORM>(tv, S, px, py, t, hint);
+            }
             const bool lat_valid = (lane <= 20) && (t <= term);
             double fl = (lat_valid && (fq == fq)) ? fq : INF;
             evals += __popc(__ballot_sync(FULL, lat_valid));
-            const int kb = warp_argmin_lane(fl);  // fl := warp minimum
-            const double tb = __shfl_sync(FULL, t, kb);
+            const int src = warp_argmin_lane(fl);  // fl := warp minimum
+            const double tb = __shfl_sync(FULL, t, src);
             if (__any_sync(FULL, fl < min_dis)) {
                 min_dis = fl;
                 seed = tb;
+                if (layer == 2) m2 = src;
             }
+            win = (layer == 2 && w3) ? w3 + kWinLen * (kWin3Stride * (kb + 1) + m2 + 1) : nullptr;
         }
     }
 
@@ -632,9 +654,13 @@ __device__ __forceinline__ Contribution point_contribution(const TrajView &tv, c
 // (5 flops per sample) and evaluates it: m; pass 2 walks k upwards and evaluates only samples with
 // |p - x_k| <= m + rout, tightening m as it goes.  A skipped sample has f_k > m >= the final minimum.  Typically ~15 of
 // the 134 samples survive; bits identical to the full scan (GPU parity tests, strict build).
+//
+// Layers 2 and 3 read their samples' poses from the pose windows (w2, w3; k_pose_table) when those are built: the window is named by
+// the layer-1 winner kb and, for layer 3, the layer-2 sample m2 that set the minimum.  The loop's own t still becomes the seed.
 template <int SHAPE, bool XFORM>
 __device__ __forceinline__ void thread_choice_t_init(const TrajView &tv, const ShapeParams &S, double px, double py,
-                                                     double &seed, double &min_dis, int &evals) {
+                                                     const PoseRec *w2, const PoseRec *w3, double &seed, double &min_dis,
+                                                     int &evals) {
     const double INF = __longlong_as_double(0x7ff0000000000000LL);
     const uint32_t row = 8u * (uint32_t)tv.K1pad;
     const int K1 = tv.K1;
@@ -682,20 +708,32 @@ __device__ __forceinline__ void thread_choice_t_init(const TrajView &tv, const S
     evals += ne;
     double dt = 0.15;
     int hint = 0;  // piece of the previous sample (the windows are <= 0.3 s wide)
+    const PoseRec *win = w2 ? w2 + kWinLen * (kb + 1) : nullptr;  // this layer's window, null: evaluate the trajectory
+    int m2 = -1;
 #pragma unroll 1
     for (int layer = 2; layer <= 4; ++layer) {
         dt *= 0.1;
         double t = smaxd(0.0, seed - 10 * dt);
         const double term = smind(tv.D, seed + 10 * dt);
 #pragma unroll 1
-        for (; t <= term; t += dt) {
-            const double f = eval_sdf<SHAPE, XFORM>(tv, S, px, py, t, hint);
+        for (int m = 0; t <= term; t += dt, ++m) {
+            double f;
+            if (win) {
+                const PoseRec cur = ld_pose(win + m);
+                double rx, ry;
+                rel_from_pose(px, py, cur.x, cur.y, cur.c, cur.s, rx, ry);
+                f = dev::shape_sdf<SHAPE, XFORM>(S, rx, ry);
+            } else {
+                f = eval_sdf<SHAPE, XFORM>(tv, S, px, py, t, hint);
+            }
             ++evals;
             if (f < min_dis) {
                 seed = t;
                 min_dis = f;
+                if (layer == 2) m2 = m;
             }
         }
+        win = (layer == 2 && w3) ? w3 + kWinLen * (kWin3Stride * (kb + 1) + m2 + 1) : nullptr;
     }
 }
 
@@ -1015,8 +1053,47 @@ __device__ __forceinline__ void pose_table_entry(double *blob, int k) {
     double *ps = blob + L.off_pose + k;
     ps[0] = x; ps[L.K1pad] = y; ps[2 * L.K1pad] = cy; ps[3 * L.K1pad] = sy;
 }
+// Record e of the pose windows of choiceTInit layers 2 (e < win2_records) and 3 (the rest; w3 null: none), svsdf_types.h:PoseRec.
+// The thread replays the scan loops' arithmetic on the window's seed: dt *= 0.1 per layer, the clamped start smaxd(0, seed - 10 dt),
+// then t += dt once per earlier sample (for layer 3 first the layer-2 chain up to sample m2, which is the seed) — the same operations
+// on the same bits, so the pose is the one eval_sdf computes at the loop's t.  Rigid: the seed layers never read the scale.
+__device__ __forceinline__ void pose_window_entry(const double *blob, PoseRec *w2, PoseRec *w3, int64_t e) {
+    const TrajView tv = make_view(blob);
+    const int64_t n2 = win2_records(tv.K1);
+    const bool layer3 = e >= n2;
+    if (layer3) {
+        e -= n2;
+        if (!w3 || e >= win3_records(tv.K1)) return;
+    }
+    PoseRec *out = (layer3 ? w3 : w2) + e;
+    const int64_t w = e / kWinLen;
+    const int m = (int)(e - w * kWinLen);
+    const int kb = (int)(layer3 ? w / kWin3Stride : w) - 1;
+    const int m2 = layer3 ? (int)(w % kWin3Stride) - 1 : -1;
+    double seed = (kb >= 0) ? tv.lat[kb] : 0.0;
+    double dt = 0.15;
+    dt *= 0.1;
+    if (m2 >= 0) {
+        double t = smaxd(0.0, seed - 10 * dt);
+        for (int i = 0; i < m2; ++i) t += dt;
+        seed = t;
+    }
+    if (layer3) dt *= 0.1;
+    double t = smaxd(0.0, seed - 10 * dt);
+    for (int i = 0; i < m; ++i) t += dt;
+    double x, y, yaw, sy, cy;
+    traj_pos(tv, t, x, y, yaw);
+    dev::sincos_portable(yaw, sy, cy);
+    out->x = x; out->y = y; out->c = cy; out->s = sy;
+}
 #if !defined(SVSDF_SCALED_UNIT) && !defined(SVSDF_MULTI_UNIT)
-__global__ void k_pose_table(double *blob) { pose_table_entry(blob, blockIdx.x * blockDim.x + threadIdx.x); }
+// one thread per layer-1 sample, then one per pose-window record
+__global__ void k_pose_table(double *blob, PoseRec *w2, PoseRec *w3) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int K1 = (int)blob[1];
+    if (e < K1) pose_table_entry(blob, (int)e);
+    else if (w2) pose_window_entry(blob, w2, w3, e - K1);
+}
 #endif
 
 // ------------------------------------------------------------------------------------------------
@@ -1083,7 +1160,7 @@ __device__ __forceinline__ void outer_body(const KernelArgs &A, const ShapeParam
         double m_seed = 0.0, m_min = 1e9, m_sdf = 0.0, m_ts = 0.0, m_gx = 0.0, m_gy = 0.0;
         if (BATCHED && batched) {
             int ev = 0;
-            if (my_valid) thread_choice_t_init<SHAPE, XFORM>(tv, S, mpx, mpy, m_seed, m_min, ev);
+            if (my_valid) thread_choice_t_init<SHAPE, XFORM>(tv, S, mpx, mpy, A.win2, A.win3, m_seed, m_min, ev);
             __syncwarp();
             unsigned ev2 = 0;
 #if SVSDF_ENGINE_ILP == 2
@@ -1104,7 +1181,7 @@ __device__ __forceinline__ void outer_body(const KernelArgs &A, const ShapeParam
 #pragma unroll 1
             for (int i = 0; i < nb; ++i) {
                 const double px = __shfl_sync(FULL, mpx, i), py = __shfl_sync(FULL, mpy, i);
-                const OuterResult R = solve_outer<SHAPE, XFORM, SCALED>(tv, S, px, py, false, 0.0, 1e9, Z);
+                const OuterResult R = solve_outer<SHAPE, XFORM, SCALED>(tv, S, px, py, A.win2, A.win3, false, 0.0, 1e9, Z);
                 my_evals += (unsigned long long)R.evals;
                 if (lane == i) { m_sdf = R.sdf; m_ts = R.tstar; }
                 double gx, gy;
@@ -1317,7 +1394,7 @@ __device__ __forceinline__ void gsip_body(const KernelArgs &A, const ShapeParams
                 double sn, cs;
                 dev::sincos_portable(th, sn, cs);
                 double yx = px + 1.0 * r * cs, yy = py + 1.0 * r * sn;  // CircleCoord2D::getPosition (:36-39)
-                OuterResult R = solve_outer<SHAPE, XFORM, SCALED>(tv, S, yx, yy, false, 0.0, 1e9, Z);
+                OuterResult R = solve_outer<SHAPE, XFORM, SCALED>(tv, S, yx, yy, A.win2, A.win3, false, 0.0, 1e9, Z);
                 my_evals += (unsigned long long)R.evals;
                 if (lane == 0) { s_val[k] = R.sdf; s_ts[k] = R.tstar; }
             }
@@ -1696,8 +1773,9 @@ cudaError_t launch_cost_kernels(const KernelArgs &A, const ShapeParams &S, const
 
 // the rigid units also bring the launchers every variant shares
 #ifndef SVSDF_SCALED_UNIT
-cudaError_t launch_pose_table(double *blob, int K1, cudaStream_t stream) {
-    k_pose_table<<<(K1 + 127) / 128, 128, 0, stream>>>(blob);
+cudaError_t launch_pose_table(double *blob, int K1, PoseRec *w2, PoseRec *w3, cudaStream_t stream) {
+    const int64_t n = K1 + (w2 ? win2_records(K1) : 0) + (w3 ? win3_records(K1) : 0);
+    k_pose_table<<<(unsigned)((n + 127) / 128), 128, 0, stream>>>(blob, w2, w3);
     return cudaGetLastError();
 }
 

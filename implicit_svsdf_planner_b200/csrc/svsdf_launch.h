@@ -31,7 +31,7 @@ SVSDF_DECLARE_LAUNCHERS(strict_scaled, strict_multi_scaled)
 // finalize of every multi launch.
 #define SVSDF_DECLARE_RIGID_LAUNCHERS(NS, MULTI)                                                                  \
     namespace NS {                                                                                               \
-    cudaError_t launch_pose_table(double *blob, int K1, cudaStream_t stream);                                    \
+    cudaError_t launch_pose_table(double *blob, int K1, PoseRec *w2, PoseRec *w3, cudaStream_t stream);          \
     cudaError_t launch_finalize(const double *partials, int n_blocks, int N, const int *n_inside,                \
                                 const double *gsip_contrib, const int *gsip_piece, double *tot,                  \
                                 unsigned int *ticket, double *out, cudaStream_t stream);                         \

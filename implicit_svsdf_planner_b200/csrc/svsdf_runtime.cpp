@@ -206,6 +206,9 @@ struct svsdf_ctx {
     bool scaled = false;
     ScaleSched sched{};
     int64_t last_n_inside = -1;  // interior points seen by the previous cost evaluation (picks the k_gsip variant)
+    // pose windows of choiceTInit layers 2 and 3 (svsdf_types.h:PoseRec), rebuilt with the layer-1 table: [layer 2 | layer 3]
+    DeviceBuffer<PoseRec> d_win;
+    int win_layers = 0;  // 0: none built, 1: layer 2, 2: layers 2 and 3
     // reduction
     DeviceBuffer<double> d_partials;
     DeviceBuffer<double> d_out;  // 1 + 19N + 1
@@ -257,6 +260,9 @@ struct svsdf_ctx {
     // test hook of the device A*, read ONCE at svsdf_create: SVSDF_FORCE_GRID_ASTAR = n > 0 sets k_astar_search's grid (1 = one
     // CTA runs every search on the same slot); -1 = not set
     int force_grid_astar = -1;
+    // test hook of the pose windows, read ONCE at svsdf_create: SVSDF_FORCE_POSE_WINDOWS = 0 (none: every layer evaluates the
+    // trajectory), 1 (layer 2 only) or 2 (layers 2 and 3), whatever pose_windows' rule says; -1 = not set
+    int force_pose_windows = -1;
     // svsdf_cost_grad_multi / svsdf_optimize_lockstep: packed inputs (one pinned stage mirrored by one device block, one copy in),
     // scratch, pinned outputs (one copy out)
     PinnedBuffer<unsigned char> h_multi_in;
@@ -416,10 +422,26 @@ int ensure_scratch(svsdf_ctx *ctx, int64_t P) {
     return SVSDF_OK;
 }
 
-// updateTraj (sw_manager.hpp:376-385) + the layer-1 lattice of choiceTInit (:538-581): builds the blob in
-// pinned memory, uploads it and launches the pose-table kernel.
-int pose_table(svsdf_ctx *ctx) {
-    CK(kernels(ctx).pose_table(ctx->d_blob, ctx->layout.K1, ctx->stream));
+// Which pose windows the evaluation of P points builds (0 / 1 / 2: none / layer 2 / layers 2 and 3).  The layer-2 windows are
+// always cheap: (K1 + 1) x 21 records, at most 42 k at D < 300 s.  The layer-3 windows hold (K1 + 1) x 22 x 21 records (0.9 M, 30 MB
+// at D near 300 s) and each replaces one trajectory evaluation of one point's layer-3 scan (21 per point): they are built when they
+// hold at most kWin3PerSample records per sample they serve.  Measured on an H100 (scripts/pose_windows_sweep.py, strict build):
+// they still pay at 3.0 records per sample (K1 = 134, P = 1 000: 3 % off the evaluation) and at 1.8 (K1 = 1999, P = 25 000: 1.5 %).
+constexpr int64_t kWin3PerSample = 2;
+int pose_windows(const svsdf_ctx *ctx, int K1, int64_t P) {
+    if (ctx->force_pose_windows >= 0) return std::min(ctx->force_pose_windows, 2);  // test hook
+    return win3_records(K1) <= kWin3PerSample * kWinLen * P ? 2 : 1;
+}
+
+// The layer-1 pose table of the uploaded blob and the pose windows for an evaluation of P points, in one launch.
+int pose_table(svsdf_ctx *ctx, int64_t P) {
+    const int K1 = ctx->layout.K1;
+    ctx->win_layers = 0;  // a failed reserve leaves no windows to read
+    const int layers = pose_windows(ctx, K1, P);
+    if (layers > 0) CK(ctx->d_win.reserve(win2_records(K1) + (layers > 1 ? win3_records(K1) : 0)));
+    PoseRec *w2 = layers > 0 ? ctx->d_win.get() : nullptr, *w3 = layers > 1 ? ctx->d_win + win2_records(K1) : nullptr;
+    CK(kernels(ctx).pose_table(ctx->d_blob, K1, w2, w3, ctx->stream));
+    ctx->win_layers = layers;
     ctx->launches += 1;
     return SVSDF_OK;
 }
@@ -469,7 +491,9 @@ void fill_blob(double *h, const BlobLayout &L, const double *T, const double *co
     }
 }
 
-int upload_traj(svsdf_ctx *ctx, int N, const double *T, const double *coeffs, bool launch_pose = true) {
+// updateTraj (sw_manager.hpp:376-385) + the layer-1 lattice of choiceTInit (:538-581): builds the blob in pinned memory, uploads it
+// and (launch_pose) launches the pose-table kernel for an evaluation of P points.
+int upload_traj(svsdf_ctx *ctx, int N, const double *T, const double *coeffs, int64_t P, bool launch_pose = true) {
     BlobLayout L;
     double D = 0.0;
     const char *msg = nullptr;
@@ -485,7 +509,7 @@ int upload_traj(svsdf_ctx *ctx, int N, const double *T, const double *coeffs, bo
     ctx->layout = L;
     ctx->traj_N = N;
     ctx->traj_D = D;
-    if (launch_pose) return pose_table(ctx);
+    if (launch_pose) return pose_table(ctx, P);
     return SVSDF_OK;
 }
 
@@ -610,6 +634,8 @@ int run_kernels(svsdf_ctx *ctx, const double *d_points, int64_t P, bool reduce, 
     A.gsip_contrib = ctx->d_gsip_contrib;
     A.gsip_piece = ctx->d_gsip_piece;
     A.eval_counter = ctx->count_evals ? ctx->d_eval_counter.get() : nullptr;
+    A.win2 = ctx->win_layers > 0 ? ctx->d_win.get() : nullptr;
+    A.win3 = ctx->win_layers > 1 ? ctx->d_win + win2_records(ctx->layout.K1) : nullptr;
     GsipPlan gp = gsip_plan(ctx, reduce ? ctx->last_n_inside : -1);
     if (gp.grid == 0) gp.grid = gp.wide ? ctx->sm_count : ctx->sm_count * occ.gsip;
     if (!gsip) CK(cudaMemsetAsync(ctx->d_n_inside, 0, sizeof(int), ctx->stream));
@@ -637,7 +663,7 @@ int cost_grad_raw(svsdf_ctx *ctx, int N, const double *T, const double *coeffs) 
         ctx->err = "svsdf: query points not set";
         return SVSDF_ERR_NOT_READY;
     }
-    int rc = upload_traj(ctx, N, T, coeffs);
+    int rc = upload_traj(ctx, N, T, coeffs, ctx->P);
     if (rc) return rc;
     if (ctx->time_kernels) CK(cudaEventRecord(ctx->ev0, ctx->stream));
     rc = run_kernels(ctx, ctx->points(), ctx->P, true, true, nullptr, nullptr, nullptr, nullptr);
@@ -1397,6 +1423,7 @@ int svsdf_create(const svsdf_config *cfg, svsdf_ctx **out) {
     if (const char *fw = std::getenv("SVSDF_FORCE_GSIP_WIDE")) ctx->force_gsip_wide = std::atoi(fw);
     if (const char *fg = std::getenv("SVSDF_FORCE_GRID_GSIP")) ctx->force_grid_gsip = std::atoi(fg);
     if (const char *fg = std::getenv("SVSDF_FORCE_GRID_ASTAR")) ctx->force_grid_astar = std::atoi(fg);
+    if (const char *fp = std::getenv("SVSDF_FORCE_POSE_WINDOWS")) ctx->force_pose_windows = std::atoi(fp);
     auto fail = [&](cudaError_t e) {
         std::fprintf(stderr, "svsdf_create: %s\n", cudaGetErrorString(e));
         svsdf_destroy(ctx);
@@ -1683,7 +1710,7 @@ int svsdf_scale_matrix(const svsdf_scale *scale, double t, double S_out[9], doub
 int svsdf_set_traj(svsdf_ctx *ctx, int N, const double *T, const double *coeffs) {
     if (!ctx) return SVSDF_ERR_INVALID;
     CK(cudaSetDevice(ctx->device));
-    int rc = upload_traj(ctx, N, T, coeffs);
+    int rc = upload_traj(ctx, N, T, coeffs, ctx->P);
     if (rc) return rc;
     CK(cudaStreamSynchronize(ctx->stream));
     return SVSDF_OK;
@@ -1693,7 +1720,7 @@ int svsdf_query(svsdf_ctx *ctx, int N, const double *T, const double *coeffs, in
                 double *sdf, double *tstar, double *grad3, int *rounds, int outer_only) {
     if (!ctx || P < 0 || (P > 0 && !pts)) return SVSDF_ERR_INVALID;
     CK(cudaSetDevice(ctx->device));
-    int rc = upload_traj(ctx, N, T, coeffs);
+    int rc = upload_traj(ctx, N, T, coeffs, P);
     if (rc) return rc;
     if (P == 0) { CK(cudaStreamSynchronize(ctx->stream)); return SVSDF_OK; }
     CK(ctx->d_q_points.reserve((size_t)P * 2));
@@ -1896,7 +1923,7 @@ int svsdf_swept_contour(svsdf_ctx *ctx, int N, const double *T, const double *co
     if (P > 0) {
         // the outer solve of svsdf_query (outer_only = 1) on the mesher's own points: the same kernels, so the same bits per point
         CK(launch_swept(1, A, st));
-        int rc = upload_traj(ctx, N, T, coeffs);
+        int rc = upload_traj(ctx, N, T, coeffs, P);
         if (rc) return rc;
         rc = run_kernels(ctx, A.pts, P, false, false, const_cast<double *>(A.val), nullptr, nullptr, nullptr);
         if (rc) return rc;
@@ -2120,7 +2147,7 @@ int svsdf_map_clearance(svsdf_ctx *ctx, int N, const double *T, const double *co
         CK(launch_clearance(1, A, st));
         ctx->launches += 1;
         // svsdf_query's path (outer solve, then the interior branch) on the band: the same kernels, so the same bits per point
-        int rc = upload_traj(ctx, N, T, coeffs);
+        int rc = upload_traj(ctx, N, T, coeffs, P);
         if (rc) return rc;
         rc = run_kernels(ctx, A.pts, P, false, true, d_sdf, d_ts, nullptr, nullptr);
         if (rc) return rc;
@@ -2287,14 +2314,14 @@ int svsdf_cost_grad_device(svsdf_ctx *ctx, int N, const double *T, const double 
     if (!ctx || repeats < 1) return SVSDF_ERR_INVALID;
     if (!ctx->points()) { ctx->err = "svsdf: query points not set"; return SVSDF_ERR_NOT_READY; }
     CK(cudaSetDevice(ctx->device));
-    int rc = upload_traj(ctx, N, T, coeffs, false);
+    int rc = upload_traj(ctx, N, T, coeffs, ctx->P, false);
     if (rc) return rc;
     CK(cudaStreamSynchronize(ctx->stream));
     CK(cudaEventRecord(ctx->ev0, ctx->stream));
     for (int r = 0; r < repeats; ++r) {
         ctx->mark_kernels = (r == repeats - 1);
         if (ctx->mark_kernels) CK(cudaEventRecord(ctx->evk[0], ctx->stream));
-        rc = pose_table(ctx);
+        rc = pose_table(ctx, ctx->P);
         if (rc) return rc;
         if (ctx->mark_kernels) CK(cudaEventRecord(ctx->evk[1], ctx->stream));
         rc = run_kernels(ctx, ctx->points(), ctx->P, true, true, nullptr, nullptr, nullptr, nullptr);

@@ -113,6 +113,19 @@ SVSDF_HD inline BlobLayout blob_layout(int N, int K1) {
     return L;
 }
 
+// Pose windows of choiceTInit layers 2 and 3 (k_pose_windows): the samples of a layer-2 window depend only on the layer-1 winner kb
+// (seed lat[kb], or 0 for kb = -1), those of a layer-3 window only on (kb, m2), m2 the layer-2 sample that set the minimum (-1: none,
+// the seed stays lat[kb]).  Window w holds kWinLen records, sample m at [kWinLen w + m]; the records past a window's last sample
+// (t > term) are computed but never read.  Layer 2: window kb + 1, (K1 + 1) windows; layer 3: window kWin3Stride (kb + 1) + m2 + 1.
+// One 32-byte record per sample: a lane's read is one sector.
+constexpr int kWinLen = 21;
+constexpr int kWin3Stride = kWinLen + 1;
+struct alignas(32) PoseRec {
+    double x, y, c, s;  // position and cos / sin of the yaw
+};
+SVSDF_HD inline int64_t win2_records(int K1) { return (int64_t)(K1 + 1) * kWinLen; }
+SVSDF_HD inline int64_t win3_records(int K1) { return (int64_t)(K1 + 1) * kWin3Stride * kWinLen; }
+
 // dynamic shared memory of k_outer in doubles: [ blob | 8 warps x (19N + 1) accumulators | 8 warps x 32 x 4 work area ]
 SVSDF_HD inline size_t outer_smem_doubles(int blob_doubles, int N) {
     return (size_t)blob_doubles + (size_t)kWarpsPerBlock * (19 * N + 1) + (size_t)kWarpsPerBlock * 128;
@@ -148,6 +161,8 @@ struct KernelArgs {
     double *gsip_contrib;        // [n_inside][20]: cost, 18 gdC entries ([d][q]), gdT
     int *gsip_piece;             // [n_inside]
     unsigned long long *eval_counter;  // optional: executed lane-evaluations (profiling builds)
+    // pose windows of choiceTInit layers 2 / 3 (k_pose_windows); null: the layer evaluates the trajectory at every sample
+    const PoseRec *win2, *win3;
 };
 
 // svsdf_cost_grad_multi (svsdf_kernels_multi.cuh): n problems in one set of launches.  The KernelArgs of a multi launch hold the
