@@ -2,17 +2,17 @@
 // Compiled with -fmad=false: a cell centre is ((i + 0.5) res + ox, (j + 0.5) res + oy) rounded as k_extract_write rounds it, so the
 // points are bit for bit the ones svsdf_extract_points[3d] hands the back end.
 //
-// Pipeline (the host side is svsdf_map_clearance in svsdf_runtime.cpp):
-//   k_cl_count   one item per 32-cell map word, 256 per CTA, row-major (the CTA order is the map order).  The path samples whose reach
-//                touches the CTA's cell-centre box go to a shared list; each item ORs its word over the z layers (a column is occupied
-//                when any layer is) and keeps the set bits whose centre lies within some listed sample's reach.  Writes the band bits,
-//                the CTA's band count and adds its occupied columns to the map's total.
+// Pipeline (the host side is clearance_bands in svsdf_runtime.cpp; svsdf_map_clearance is its one-trajectory case):
+//   k_cl_count   the words of every problem's reach rectangle, one item per 32-cell word, row-major, padded to whole CTAs of 256
+//                (the CTAs of problem k follow those of problem k - 1, so the CTA order is problem order, then map order).  The
+//                problem's samples whose reach touches the CTA's cell-centre box go to a shared list; each item ORs its word over
+//                the z layers (a column is occupied when any layer is) and keeps the set bits whose centre lies within some listed
+//                sample's reach.  Writes the band bits and the CTA's band count.  A last segment covers the whole map and only
+//                counts its occupied columns.
 //   k_sw_scan    exclusive prefix of the per-CTA counts (svsdf_swept.cu, one CTA).
-//   k_cl_write   the band's cells (i, j) and centres, in map order, into the clearance's own point buffer.
-//   (svsdf_query's kernels, outer solve and interior branch, run on that buffer)
-// svsdf_map_clearance_multi runs the same per-CTA test over each problem's reach rectangle (k_cl_count_multi, k_sw_scan,
-// k_cl_write_multi: the bands of all problems, concatenated in problem order, each in map order); the multi-problem kernels of
-// svsdf_kernels_multi.cuh evaluate them.
+//   k_cl_write   the band's cells (i, j) and centres, concatenated in problem order, each in map order, into the clearance's own
+//                point buffer.
+//   (then svsdf_query's kernels for one trajectory, the multi-problem kernels of svsdf_kernels_multi.cuh for n)
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -72,15 +72,12 @@ __device__ __forceinline__ unsigned column_word(const ClearanceArgs &A, int i, i
     return w & interval_mask(A.h - 32 * wy, A.h + A.Y - 1 - 32 * wy);
 }
 
-// The items of one CTA: item t = t0 + threadIdx.x (< n_items) is word wy0 + t % nW of map row i0 + t / nW.  Returns the item's band bits
-// (its occupied columns whose centre lies within some sample's reach; all of them when `all`) and its occupied bits in *occ.
-struct CtaItems {
-    int64_t t0, n_items;
-    int i0, wy0, nW, all, n_samp;
-    const double *samp;
-};
-__device__ __forceinline__ unsigned cta_band(const ClearanceArgs &A, const CtaItems &C, int *s_list, int *s_n, unsigned *occ_out) {
-    const int64_t first = C.t0;
+// The items of this CTA in problem C's rectangle: item t = first + threadIdx.x (< n_items) is word wy0 + t % nW of row i0 + t / nW.
+// Returns the item's band bits (its occupied columns whose centre lies within some sample's reach; all of them when `all`) and its
+// occupied bits in *occ.
+__device__ __forceinline__ unsigned cta_band(const ClearanceArgs &A, const ClearanceProblem &C, int64_t first, int *s_list, int *s_n,
+                                             unsigned *occ_out) {
+    const double *samp = A.samp + 3 * (int64_t)C.samp0;
     const int64_t last = min(first + (int64_t)blockDim.x - 1, C.n_items - 1);
     const int64_t t = first + threadIdx.x;
     int i = 0, wy = 0;
@@ -106,7 +103,7 @@ __device__ __forceinline__ unsigned cta_band(const ClearanceArgs &A, const CtaIt
         // a sample that reaches a centre of the CTA reaches its box: the centres are monotone in the index and the rounded differences
         // and squares are monotone, so the box distance is never larger than the centre distance computed below (k_sw_classify's test)
         for (int k = threadIdx.x; k < C.n_samp; k += blockDim.x) {
-            const double sx = C.samp[3 * k], sy = C.samp[3 * k + 1], r = C.samp[3 * k + 2];
+            const double sx = samp[3 * k], sy = samp[3 * k + 1], r = samp[3 * k + 2];
             const double dx = fmax(fmax(bx0 - sx, sx - bx1), 0.0), dy = fmax(fmax(by0 - sy, sy - by1), 0.0);
             if (dx * dx + dy * dy <= r * r) s_list[atomicAdd(s_n, 1)] = k;
         }
@@ -121,7 +118,7 @@ __device__ __forceinline__ unsigned cta_band(const ClearanceArgs &A, const CtaIt
                 bool in = false;
                 for (int q = 0; q < n && !in; ++q) {
                     const int s = s_list[q];
-                    const double dx = cx - C.samp[3 * s], dy = cy - C.samp[3 * s + 1], r = C.samp[3 * s + 2];
+                    const double dx = cx - samp[3 * s], dy = cy - samp[3 * s + 1], r = samp[3 * s + 2];
                     in = dx * dx + dy * dy <= r * r;
                 }
                 if (in) band |= 1u << k;
@@ -145,36 +142,8 @@ __device__ __forceinline__ void write_cells(const ClearanceArgs &A, unsigned ban
     }
 }
 
-__global__ void __launch_bounds__(256) k_cl_count(const __grid_constant__ ClearanceArgs A) {
-    __shared__ int s_list[kSweptMaxSamples];
-    __shared__ int s_n;
-    __shared__ int s_w[2][8];
-    const CtaItems C{(int64_t)blockIdx.x * blockDim.x, A.n_items, 0, A.wy0, A.nW, A.all, A.n_samp, A.samp};
-    unsigned occ;
-    const unsigned band = cta_band(A, C, s_list, &s_n, &occ);
-    const int64_t item = C.t0 + threadIdx.x;
-    if (item < A.n_items) A.band[item] = band;
-    int n_band, n_occ;
-    block_scan256(__popc(band), s_w[0], &n_band);
-    block_scan256(__popc(occ), s_w[1], &n_occ);
-    if (threadIdx.x == 0) {
-        A.blk[blockIdx.x] = n_band;
-        if (n_occ) atomicAdd(A.n_occ, (unsigned long long)n_occ);  // integer sum: the same total in any order
-    }
-}
-
-__global__ void __launch_bounds__(256) k_cl_write(const __grid_constant__ ClearanceArgs A) {
-    __shared__ int s_w[8];
-    const int64_t item = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const unsigned band = item < A.n_items ? A.band[item] : 0u;
-    int total;
-    const int64_t pos = (int64_t)A.blk[blockIdx.x] + block_scan256(__popc(band), s_w, &total);
-    if (!band) return;
-    write_cells(A, band, (int)(item / A.nW), A.wy0 + (int)(item % A.nW), pos);
-}
-
-// ---- svsdf_map_clearance_multi: the CTAs of problem k are cta0[k] .. cta0[k + 1] - 1, in problem order; the last segment counts the
-// occupied columns of the whole map and has no band.  Items: one per (CTA, thread), so band[] is indexed by blockIdx.x * 256 + threadIdx.x.
+// The CTAs of problem k are cta0[k] .. cta0[k + 1] - 1, in problem order; the last segment counts the occupied columns of the whole
+// map and has no band.  Items: one per (CTA, thread), so band[] is indexed by blockIdx.x * 256 + threadIdx.x.
 __device__ __forceinline__ const ClearanceProblem &cta_problem(const ClearanceArgs &A) {
     int lo = 0, hi = A.n_prob - 1;  // the last k with cta0 <= blockIdx.x (a problem without CTAs shares cta0 with the next one)
     while (lo < hi) {
@@ -185,15 +154,13 @@ __device__ __forceinline__ const ClearanceProblem &cta_problem(const ClearanceAr
     return A.prob[lo];
 }
 
-__global__ void __launch_bounds__(256) k_cl_count_multi(const __grid_constant__ ClearanceArgs A) {
+__global__ void __launch_bounds__(256) k_cl_count(const __grid_constant__ ClearanceArgs A) {
     __shared__ int s_list[kSweptMaxSamples];
     __shared__ int s_n;
     __shared__ int s_w[2][8];
     const ClearanceProblem &pr = cta_problem(A);
-    const CtaItems C{((int64_t)blockIdx.x - pr.cta0) * blockDim.x, pr.n_items, pr.i0, pr.wy0, pr.nW, pr.all, pr.n_samp,
-                     A.samp + 3 * (int64_t)pr.samp0};
     unsigned occ;
-    unsigned band = cta_band(A, C, s_list, &s_n, &occ);
+    unsigned band = cta_band(A, pr, ((int64_t)blockIdx.x - pr.cta0) * blockDim.x, s_list, &s_n, &occ);
     if (pr.occ_only) band = 0u;
     else occ = 0u;
     A.band[(int64_t)blockIdx.x * blockDim.x + threadIdx.x] = band;
@@ -202,11 +169,11 @@ __global__ void __launch_bounds__(256) k_cl_count_multi(const __grid_constant__ 
     block_scan256(__popc(occ), s_w[1], &n_occ);
     if (threadIdx.x == 0) {
         A.blk[blockIdx.x] = n_band;
-        if (n_occ) atomicAdd(A.n_occ, (unsigned long long)n_occ);
+        if (n_occ) atomicAdd(A.n_occ, (unsigned long long)n_occ);  // integer sum: the same total in any order
     }
 }
 
-__global__ void __launch_bounds__(256) k_cl_write_multi(const __grid_constant__ ClearanceArgs A) {
+__global__ void __launch_bounds__(256) k_cl_write(const __grid_constant__ ClearanceArgs A) {
     __shared__ int s_w[8];
     const unsigned band = A.band[(int64_t)blockIdx.x * blockDim.x + threadIdx.x];
     int total;
@@ -224,8 +191,6 @@ cudaError_t launch_clearance(int what, const ClearanceArgs &A, cudaStream_t st) 
     switch (what) {
         case 0: k_cl_count<<<nblk, 256, 0, st>>>(A); break;
         case 1: k_cl_write<<<nblk, 256, 0, st>>>(A); break;
-        case 2: k_cl_count_multi<<<nblk, 256, 0, st>>>(A); break;
-        case 3: k_cl_write_multi<<<nblk, 256, 0, st>>>(A); break;
         default: return cudaErrorInvalidValue;
     }
     return cudaGetLastError();

@@ -775,134 +775,33 @@ __device__ __forceinline__ void thread_grad_prel(const TrajView &tv, const Shape
 }
 
 // ------------------------------------------------------------------------------------------------
-// gradientDescent (sw_manager.hpp:1249-1325) for a BATCH of points, a quarter warp (8 lanes) per point, four points in
-// flight per warp — the batched path of k_outer and the interior-branch kernel.
+// gradientDescent (sw_manager.hpp:1249-1325) for a BATCH of points, a group of 4 lanes per point, each lane evaluating two
+// samples per round (8 points in flight per warp) — the batched path of k_outer.
 //
 // The reference's loop, per descent step: slope sign from the finite difference at x (2 evaluations, recomputed for every
 // halving in the reference but always at the same x, hence the same bits), then candidates x - sign * 0.01 * 2^-j for
 // j = 0, 1, ... until the first one that decreases f (29 failures end the descent).  Measured on configs 1-3 (oracle,
 // orc_descent_stats): ~8 steps per point, accepted j spread evenly over 7..20 (never 1..6), so a full warp per step
-// (29 candidates + slope, the round-1 design) spends most of its lanes on candidates beyond the accepted one, and one lane per
-// point (sequential, 155 +- 65 evaluations) leaves the warp waiting for its slowest lane.  Eight lanes per point in
-// rounds of one evaluation per lane:
-//   R1   lanes 0/1 of the quarter: the two finite-difference samples; lanes 2..7: candidates j = 0..5 in the PREDICTED
-//        direction (the slope flips after every non-full step because the accepted step is the largest decreasing one)
+// (29 candidates + slope) spends most of its lanes on candidates beyond the accepted one, and one lane per point
+// (sequential, 155 +- 65 evaluations) leaves the warp waiting for its slowest lane.  A group runs rounds of 8 samples,
+// lane q of the group evaluating samples s = q (slot A) and s = q + 4 (slot B):
+//   R1   samples 0/1: the two finite-difference samples; samples 2..7: candidates j = 0..5 in the PREDICTED direction (the
+//        slope flips after every non-full step because the accepted step is the largest decreasing one)
 //   RN   candidates j = jbase .. jbase + 7 in the known direction (jbase = 6, 14, 22 after R1; 0, 8, 16, 24 after a
 //        misprediction)
-//   F0   f(x0) when choiceTInit found nothing below 1e9 (degenerate input; the reference evaluates it at iter == 0)
-// => ~21 lane-evaluations per step instead of 31.  A quarter that finishes its point stores (sdf, t*) and takes the next
-// point of the batch (warp-uniform cursor), so the four quarters stay busy until the batch runs dry.  Every decision is
-// the sequential loop's decision given the same SDF values: the accepted halving is the FIRST j whose candidate
-// decreases f, the sign comes from the finite difference — bit-identical results (GPU parity tests, strict build).
-// In: lane i (< nb) holds point i of the batch (px, py, choiceTInit seed and minimum).  Out: res[2 i] = sdf, res[2 i + 1] = t*.
+//   F0   f(x0) when choiceTInit found nothing below 1e9 (degenerate input; the reference evaluates it at iter == 0), and
+//        always for a deformable robot (f(x0) of the scaled shape)
+// => ~21 sample evaluations per step instead of 31.  The two evaluations of a lane are independent instruction streams
+// (latency hiding inside the thread, on top of the resident warps) and the per-round bookkeeping is paid once per two
+// evaluations.  Every decision is the sequential loop's decision given the same SDF values: the accepted halving is the
+// FIRST j whose candidate decreases f, the sign comes from the finite difference — bit-identical results (GPU parity tests,
+// strict build).
+// The queue of prepared points is shared by the CTA's 8 warps (wk: 8 x 32 entries of 4 doubles in (px, py, choiceTInit
+// seed and minimum), entry (w, i) at wk[4 (32 w + i)], valid for i < nbw[w]; served in the order i-major, w-minor through
+// the shared cursor): a group that finishes its point writes (sdf, t*) over wk[4 (32 w + i)] and takes the next point of
+// the whole CTA, so the warps of a CTA finish together whatever the lengths of their own descents.  Which group solves a
+// point does not change its result; the reductions stay per warp, fixed order.
 // ------------------------------------------------------------------------------------------------
-template <int SHAPE, bool XFORM, bool SCALED = false>
-__device__ __forceinline__ void descent_engine(const TrajView &tv, const ShapeParams &S, int nb, double mpx, double mpy,
-                                               double mseed, double mmin, double *res, unsigned &evals,
-                                               const ScaleSched *Z = nullptr) {
-    enum { E_F0 = 0, E_R1 = 1, E_RN = 2 };
-    const int lane = threadIdx.x & 31, q = lane & 7, qbase = lane & 24;
-    const double D = tv.D;
-    const double INF = __longlong_as_double(0x7ff0000000000000LL);
-    const int hi001 = __double2hiint(0.01), lo001 = __double2loint(0.01);
-    // state of this lane's quarter (identical in its 8 lanes)
-    int pt = -1, mode = E_R1, iter = 0, pred = 1, sgn = 1, jbase = 0, hint = 0;
-    double px = 0.0, py = 0.0, x = 0.0, fx = 0.0, prev_x = 0.0, t_min = 0.0, t_max = 0.0;
-    bool need = true;   // the quarter wants a point
-    int next_i = 0;     // warp-uniform cursor into the batch
-#pragma unroll 1
-    for (;;) {
-        // ---- hand the next points of the batch to the quarters that are free ----
-        const unsigned want = __ballot_sync(FULL, need && q == 0);
-        if (want) {
-            const int cand = next_i + __popc(want & ((1u << qbase) - 1u));
-            next_i += __popc(want);
-            const bool take = need && cand < nb;
-            const int src = take ? cand : lane;
-            const double npx = __shfl_sync(FULL, mpx, src), npy = __shfl_sync(FULL, mpy, src);
-            const double nsd = __shfl_sync(FULL, mseed, src), nmn = __shfl_sync(FULL, mmin, src);
-            if (need) {
-                need = false;
-                pt = -1;
-                if (take) {
-                    pt = cand;
-                    px = npx; py = npy;
-                    x = nsd; fx = nmn; prev_x = nsd;   // `prev_x = x` after the (true) first loop test
-                    t_min = smaxd(0.0, nsd - 3.4);      // :856-857
-                    t_max = smind(nsd + 3.4, D);
-                    iter = 0; pred = 1; sgn = 1; jbase = 0; hint = 0;
-                    mode = (SCALED || nmn >= 1e9) ? E_F0 : E_R1;  // SCALED: f(x0) of the scaled shape
-                }
-            }
-        }
-        if (!__any_sync(FULL, pt >= 0)) break;
-
-        // ---- this lane's sample (straight-line code: the four quarters are in different modes) ----
-        const bool isR1 = mode == E_R1, isF0 = mode == E_F0;
-        const bool slope = isR1 && q < 2;
-        const int j = isR1 ? q - 2 : jbase + q;
-        const bool cand = !isF0 && !slope && j <= 28;
-        evals += (pt >= 0 && (cand || slope || (isF0 && q == 0))) ? 1u : 0u;
-        // candidate: tau = 0.01 halved j times (exact: subtract j from the exponent field); change = -tau * sign
-        const int dir = isR1 ? pred : sgn;
-        const int tau_hi = (hi001 - ((j & 31) << 20)) ^ ((dir > 0) ? (int)0x80000000 : 0);
-        // slope samples: t1 = max(0, x - 1e-6), t2 = min(D, x + 1e-6)   (:798-806)
-        const double off = slope ? ((q == 0) ? -0.000001 : 0.000001) : __hiloint2double(tau_hi, lo001);
-        const double lo_l = slope ? ((q == 0) ? 0.0 : -INF) : t_min;
-        const double hi_l = slope ? ((q == 0) ? INF : D) : t_max;
-        const double tc = smaxd(smind(x + off, hi_l), lo_l);
-        const double tq = (cand || slope) ? tc : x;
-        const double fq = eval_sdf<SHAPE, XFORM, SCALED>(tv, S, px, py, tq, hint, Z);
-
-        // ---- collectives (all lanes), then each quarter's decision, again without branches ----
-        const unsigned m8 = (__ballot_sync(FULL, (fq - fx) < 0) >> qbase) & 0xffu;
-        const double f0 = __shfl_sync(FULL, fq, qbase), f1 = __shfl_sync(FULL, fq, qbase + 1);
-        const double g = (f1 - f0) * 500000;
-        const int s_new = (int)(g > 0) - (int)(g < 0);
-        sgn = isR1 ? s_new : sgn;
-        const bool zero = isR1 && sgn == 0;              // all 29 candidates equal x: none decreases f
-        const bool mispred = isR1 && sgn != 0 && sgn != pred;
-        const int nvalid = max(0, min(8, 29 - jbase));   // (idle quarters keep counting jbase up)
-        const unsigned mc = isR1 ? (m8 >> 2) : (m8 & ((1u << nvalid) - 1u));
-        const bool hit = (pt >= 0) && !isF0 && !zero && !mispred && mc != 0u;   // first decreasing candidate found
-        const int k = __ffs(mc) - 1;
-        const int jacc = isR1 ? k : jbase + k;
-        const int src = hit ? qbase + (isR1 ? k + 2 : k) : lane;
-        const double xacc = __shfl_sync(FULL, tq, src), facc = __shfl_sync(FULL, fq, src);
-        // no decreasing candidate in this round: next chunk of halvings (R1: j = 6.., or j = 0.. after a misprediction)
-        const int jb_next = isR1 ? (mispred ? 0 : 6) : jbase + 8;
-        const bool failed = (pt >= 0) && !isF0 && (zero || (!hit && !mispred && jb_next > 28));
-        // a full, unclamped stride means we are still walking downhill: same slope sign next; otherwise the step overshot
-        // the minimiser (tau_j is the largest decreasing step) and the slope flips
-        const bool walking = (jacc == 0) && (xacc == x + (-0.01 * (double)sgn));
-        pred = hit ? (walking ? sgn : -sgn) : pred;
-        iter += hit ? jacc + 1 : (failed ? 29 : 0);
-        x = hit ? xacc : x;
-        fx = hit ? facc : (isF0 ? f0 : fx);
-        const bool step_end = hit || failed;
-        // while (iter < max_iter && !stop && abs(x - prev_x) > tol)   (:1288)
-        const bool running = (iter < 1000) && !failed && (fabs(x - prev_x) > 1e-16);
-        prev_x = step_end ? x : prev_x;
-        mode = (step_end || isF0) ? E_R1 : E_RN;
-        jbase = jb_next;
-        if (step_end && !running) {
-            if (q == 0) { res[2 * pt] = fx; res[2 * pt + 1] = x; }
-            pt = -1;
-            need = true;
-        }
-    }
-    __syncwarp();
-}
-
-// descent_engine with TWO samples per lane: a group of 4 lanes per point (8 points in flight per warp), each lane evaluates
-// samples s = q and s = q + 4 of its group's round (same rounds as above: R1 = 2 slope samples + candidates j = 0..5,
-// RN = candidates jbase..jbase + 7).  The two evaluations are independent instruction streams (latency hiding inside the
-// thread, on top of the resident warps) and the per-round bookkeeping is paid once per two evaluations.
-// wk: per-warp shared work area, 4 doubles per point in (px, py, seed, min), 2 doubles per point out (sdf, t*) at wk[4 i].
-// The queue of prepared points is shared by the CTA's 8 warps (wk: 8 x 32 entries of 4 doubles, entry (w, i) at
-// wk[4 (32 w + i)], valid for i < nbw[w]; served in the order i-major, w-minor through the shared cursor): a group that
-// finishes its point takes the next one of the whole CTA, so the warps of a CTA finish together whatever the lengths of
-// their own descents.  Which group solves a point does not change its result; the reductions stay per warp, fixed order.
 template <int SHAPE, bool XFORM, bool SCALED = false>
 __device__ __forceinline__ void descent_engine2(const TrajView &tv, const ShapeParams &S, double *wk, const int *nbw, int *cursor,
                                                 int limit, unsigned &evals, const ScaleSched *Z = nullptr) {
@@ -932,7 +831,7 @@ __device__ __forceinline__ void descent_engine2(const TrajView &tv, const ShapeP
                     const double *w = wk + 4 * pt;
                     px = w[0]; py = w[1];
                     const double nsd = w[2], nmn = w[3];
-                    x = nsd; fx = nmn; prev_x = nsd;
+                    x = nsd; fx = nmn; prev_x = nsd;   // `prev_x = x` after the (true) first loop test
                     t_min = smaxd(0.0, nsd - 3.4);
                     t_max = smind(nsd + 3.4, D);
                     iter = 0; pred = 1; sgn = 1; jbase = 0; hintA = 0; hintB = 0;
@@ -1100,9 +999,6 @@ __global__ void k_pose_table(double *blob, PoseRec *w2, PoseRec *w3) {
 // K1: outer solve for every point (+ penalty, chain rule and CTA reduction for outside points)
 // dynamic smem: [ blob | 8 warps x (19N + 1) accumulators ]
 // ------------------------------------------------------------------------------------------------
-#ifndef SVSDF_ENGINE_ILP
-#define SVSDF_ENGINE_ILP 2   // samples per lane and round in the batched descent (1: descent_engine, 2: descent_engine2)
-#endif
 #ifndef SVSDF_MESH_MIN_CTAS
 #define SVSDF_MESH_MIN_CTAS 4  // measured on config 4m: 2 -> 245 ms, 3 -> 206 ms, 4 -> 198 ms (the traversal is latency bound; spills stay in L1)
 #endif
@@ -1141,29 +1037,27 @@ __device__ __forceinline__ void outer_body(const KernelArgs &A, const ShapeParam
     //    (+-1; neighbouring map cells: the lanes of a warp then prune the same layer-1 samples and run descents of similar
     //    length), warp w owns batches w, w + W, ... (strided: a warp's batches come from different regions of the map, so
     //    hard regions are spread over the warps; static, hence deterministic).  choiceTInit and the FD gradient /
-    //    penalty / chain rule run one point per lane, gradientDescent one point per quarter warp (descent_engine).
+    //    penalty / chain rule run one point per lane, gradientDescent one point per group of 4 lanes, served from the CTA's
+    //    point queue (descent_engine2).
     //  * Sparse schedule (few points per warp, i.e. small problems): the warp owns points w, w + W, ...; everything one
     //    point per warp, as solve_outer / grad_prel do (lowest latency).
-    constexpr bool chunked = BATCHED;
-    const int64_t lstride = chunked ? 1 : wstride;  // distance between the points of neighbouring lanes
+    const int64_t lstride = BATCHED ? 1 : wstride;  // distance between the points of neighbouring lanes
     const int64_t nB = wstride * ((A.P + 32 * wstride - 1) / (32 * wstride));   // batches (batched schedule)
-    for (int64_t bi = first; chunked ? (bi < nB) : (bi < A.P); bi += chunked ? wstride : 32 * wstride) {
+    for (int64_t bi = first; BATCHED ? (bi < nB) : (bi < A.P); bi += BATCHED ? wstride : 32 * wstride) {
         // batched: batch bi covers [bi P / nB, (bi + 1) P / nB); sparse: points bi, bi + W, ...
-        const int64_t bfirst = chunked ? (bi * A.P) / nB : bi;
-        const int64_t bend = chunked ? ((bi + 1) * A.P) / nB : A.P;
+        const int64_t bfirst = BATCHED ? (bi * A.P) / nB : bi;
+        const int64_t bend = BATCHED ? ((bi + 1) * A.P) / nB : A.P;
         const int64_t my_pt = bfirst + (int64_t)lane * lstride;
         const int nb = (int)min((int64_t)32, (bend - bfirst + lstride - 1) / lstride);  // batch size (warp-uniform)
         const bool my_valid = lane < nb;
         const int64_t ld_pt = my_valid ? my_pt : bfirst;
         const double mpx = __ldg(A.points_xy + 2 * ld_pt), mpy = __ldg(A.points_xy + 2 * ld_pt + 1);
-        const bool batched = chunked;   // CTA-uniform: the batched schedule synchronises the CTA around its shared queue
         double m_seed = 0.0, m_min = 1e9, m_sdf = 0.0, m_ts = 0.0, m_gx = 0.0, m_gy = 0.0;
-        if (BATCHED && batched) {
+        if (BATCHED) {  // the whole CTA: the batched schedule synchronises the CTA around its shared queue
             int ev = 0;
             if (my_valid) thread_choice_t_init<SHAPE, XFORM>(tv, S, mpx, mpy, A.win2, A.win3, m_seed, m_min, ev);
             __syncwarp();
             unsigned ev2 = 0;
-#if SVSDF_ENGINE_ILP == 2
             if (my_valid) { res[4 * lane] = mpx; res[4 * lane + 1] = mpy; res[4 * lane + 2] = m_seed; res[4 * lane + 3] = m_min; }
             if (lane == 0) s_nb[warp] = nb;
             if (threadIdx.x == 0) s_cursor = 0;
@@ -1171,10 +1065,6 @@ __device__ __forceinline__ void outer_body(const KernelArgs &A, const ShapeParam
             descent_engine2<SHAPE, XFORM, SCALED>(tv, S, res - 128 * warp, s_nb, &s_cursor, kWarpsPerBlock * 32, ev2, Z);
             __syncthreads();
             if (my_valid) { m_sdf = res[4 * lane]; m_ts = res[4 * lane + 1]; }
-#else
-            descent_engine<SHAPE, XFORM, SCALED>(tv, S, nb, mpx, mpy, m_seed, m_min, res, ev2, Z);
-            if (my_valid) { m_sdf = res[2 * lane]; m_ts = res[2 * lane + 1]; }
-#endif
             my_evals += (unsigned long long)__reduce_add_sync(FULL, (unsigned)ev + ev2);
             __syncwarp();
         } else {
@@ -1190,7 +1080,7 @@ __device__ __forceinline__ void outer_body(const KernelArgs &A, const ShapeParam
             }
         }
         my_evals += 4ull * (unsigned long long)nb;
-        if (BATCHED && batched && my_valid) thread_grad_prel<SHAPE, XFORM, SCALED>(tv, S, mpx, mpy, m_ts, m_gx, m_gy, Z);
+        if (BATCHED && my_valid) thread_grad_prel<SHAPE, XFORM, SCALED>(tv, S, mpx, mpy, m_ts, m_gx, m_gy, Z);
         // ---- per-lane epilogue: outputs, interior flag, penalty + chain rule (one point per lane) ----
         const bool inside = my_valid && A.want_gsip && !(m_sdf > 0);  // getTrueSDFofSweptVolume: `if (argmin_dis > 0) return`
         if (my_valid) {

@@ -1997,18 +1997,6 @@ void clearance_empty(svsdf_clearance *out) {
     out->argmin = -1;
 }
 
-// svsdf_map_clearance's checks of one trajectory (D: its duration); on failure the message is in *err
-int clearance_traj(int N, const double *T, const double *coeffs, double &D, const char **err) {
-    BlobLayout L;
-    if (traj_layout(N, T, coeffs, L, D, err) != SVSDF_OK) return SVSDF_ERR_INVALID;
-    for (int64_t e = 0; e < 18 * (int64_t)N; ++e)
-        if (!std::isfinite(coeffs[e])) {
-            *err = "svsdf_map_clearance: non-finite trajectory coefficient";
-            return SVSDF_ERR_INVALID;
-        }
-    return SVSDF_OK;
-}
-
 // the band's samples: rho and the samples of svsdf_swept_contour with iso = d_max.  Returns `all` (every occupied column is in the band,
 // no samples): d_max = +inf or a shape without a far-field bound.
 bool clearance_samples(const svsdf_ctx *ctx, int N, const double *T, const double *coeffs, double D, double d_max, std::vector<double> &samp) {
@@ -2064,19 +2052,6 @@ int clearance_list(svsdf_ctx *ctx, int64_t P, const int32_t *h_ij, const double 
     return SVSDF_OK;
 }
 
-// the map fields of the clearance kernels' arguments
-ClearanceArgs clearance_args(const svsdf_ctx *ctx) {
-    ClearanceArgs A;
-    std::memset(&A, 0, sizeof(A));
-    A.map = ctx->map();
-    A.X = ctx->map_X; A.Y = ctx->map_Y; A.h = ctx->map_h; A.row_bytes = ctx->map_row_bytes; A.Z = ctx->map_Z;
-    A.layer = (int64_t)(A.X + 2 * A.h) * A.row_bytes;
-    A.ox = ctx->map_ox; A.oy = ctx->map_oy; A.res = ctx->map_res;
-    A.wy0 = A.h / 32;
-    A.nW = (A.h + A.Y - 1) / 32 - A.wy0 + 1;
-    return A;
-}
-
 // cell index range [lo, hi] of the map axis (n cells, origin o, resolution res) whose centres may lie in [a, b]: outward by one cell
 // beyond the rounding of the centres, clipped to the map (lo > hi: none)
 void cell_range(double a, double b, double o, double res, int n, int &lo, int &hi) {
@@ -2084,110 +2059,52 @@ void cell_range(double a, double b, double o, double res, int n, int &lo, int &h
     lo = (int)std::min(std::max(l, 0.0), (double)n);
     hi = (int)std::max(std::min(h, (double)n - 1.0), -1.0);
 }
-}  // namespace
 
-int svsdf_map_clearance(svsdf_ctx *ctx, int N, const double *T, const double *coeffs, double d_max, svsdf_clearance *out) {
-    if (!ctx || !out) return SVSDF_ERR_INVALID;
-    clearance_empty(out);
-    auto invalid = [&](const char *msg) {
-        ctx->err = msg;
-        return SVSDF_ERR_INVALID;
-    };
-    // the band proves only "outer value > d_max"; for d_max >= 0 that value is the whole answer (no interior branch), below 0 it is not
-    if (!(d_max >= 0.0)) return invalid("svsdf_map_clearance: d_max must be >= 0 or +INFINITY");
-    double D = 0.0;
-    const char *msg = nullptr;
-    if (clearance_traj(N, T, coeffs, D, &msg) != SVSDF_OK) return invalid(msg);
-    if (!ctx->map()) {
-        ctx->err = "svsdf_map_clearance: map not set";
-        return SVSDF_ERR_NOT_READY;
-    }
-    if ((int64_t)ctx->map_X * ctx->map_Y > 2000000000LL) return invalid("svsdf_map_clearance: map has more than 2e9 columns");
-    std::vector<double> samp;
-    const bool all = clearance_samples(ctx, N, T, coeffs, D, d_max, samp);
-    if ((int)(samp.size() / 3) > kSweptMaxSamples) return invalid("svsdf_map_clearance: too many path samples");
-    CK(cudaSetDevice(ctx->device));
-    ClearanceArgs A = clearance_args(ctx);
-    A.n_items = (int64_t)A.X * A.nW;
-    A.all = all ? 1 : 0;
-    A.n_samp = (int)(samp.size() / 3);
-    const int nblk = (int)((A.n_items + 255) / 256);
-    // small: header [0] occupied columns (u64), [8] band cells (int); samples; per-CTA counts
-    const size_t off_samp = 64, off_blk = off_samp + align16(samp.size() * 8);
-    CK(ctx->d_cl_small.reserve(off_blk + (size_t)(nblk + 1) * 4));
-    CK(ctx->d_cl_band.reserve((size_t)A.n_items * 4));
-    A.n_occ = reinterpret_cast<unsigned long long *>(ctx->d_cl_small.get());
-    int *d_total = reinterpret_cast<int *>(ctx->d_cl_small + 8);
-    A.samp = reinterpret_cast<double *>(ctx->d_cl_small + off_samp);
-    A.blk = reinterpret_cast<int *>(ctx->d_cl_small + off_blk);
-    A.band = reinterpret_cast<unsigned *>(ctx->d_cl_band.get());
-    CK(ctx->h_stage.reserve(64 + samp.size() * 8));
-    unsigned char *hs = ctx->h_stage;
-    std::memset(hs, 0, 64);
-    if (!samp.empty()) std::memcpy(hs + 64, samp.data(), samp.size() * 8);
-    cudaStream_t st = ctx->stream;
-    CK(cudaMemcpyAsync(ctx->d_cl_small, hs, 64 + samp.size() * 8, cudaMemcpyHostToDevice, st));
-    CK(launch_clearance(0, A, st));
-    CK(launch_swept_scan(A.blk, nblk, 1, d_total, st));
-    CK(cudaMemcpyAsync(hs, ctx->d_cl_small, 16, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    ctx->launches += 2;
-    unsigned long long n_occ;
-    int P32;
-    std::memcpy(&n_occ, hs, 8);
-    std::memcpy(&P32, hs + 8, 4);
-    const int64_t P = P32;
-    // band cells: (i, j) int32 pairs, centres, values, t* — contiguous, so one download brings them all
-    const size_t o_pts = align16((size_t)P * 8), o_sdf = o_pts + (size_t)P * 16, o_ts = o_sdf + (size_t)P * 8, o_end = o_ts + (size_t)P * 8;
-    CK(ctx->d_cl_point.reserve(o_end + 16));
-    A.ij = reinterpret_cast<int *>(ctx->d_cl_point.get());
-    A.pts = reinterpret_cast<double *>(ctx->d_cl_point + o_pts);
-    double *d_sdf = reinterpret_cast<double *>(ctx->d_cl_point + o_sdf), *d_ts = reinterpret_cast<double *>(ctx->d_cl_point + o_ts);
-    if (P > 0) {
-        CK(launch_clearance(1, A, st));
-        ctx->launches += 1;
-        // svsdf_query's path (outer solve, then the interior branch) on the band: the same kernels, so the same bits per point
-        int rc = upload_traj(ctx, N, T, coeffs, P);
-        if (rc) return rc;
-        rc = run_kernels(ctx, A.pts, P, false, true, d_sdf, d_ts, nullptr, nullptr);
-        if (rc) return rc;
-        CK(ctx->h_stage.reserve(o_end));
-        hs = ctx->h_stage;
-        CK(cudaMemcpyAsync(hs, ctx->d_cl_point, o_end, cudaMemcpyDeviceToHost, st));
-        CK(cudaStreamSynchronize(st));
-    }
-    return clearance_list(ctx, P, reinterpret_cast<const int32_t *>(hs), reinterpret_cast<const double *>(hs + o_pts),
-                          reinterpret_cast<const double *>(hs + o_sdf), reinterpret_cast<const double *>(hs + o_ts), n_occ, d_max, out);
-}
+// The bands of n trajectories, built in one count / scan / write (DESIGN.md §7).  Problem k's band is cells off[k] .. off[k + 1] - 1
+// of the concatenation in ctx->d_cl_point: (i, j) int32 pairs at 0, then centres, values and t* at o_pts, o_sdf, o_ts (contiguous, so
+// one download brings them all).
+struct ClearanceBands {
+    std::vector<int64_t> off;
+    unsigned long long n_occ = 0;  // occupied columns of the map
+    size_t o_pts = 0, o_sdf = 0, o_ts = 0, o_end = 0;
+};
 
-// The bands of all problems in one count / scan / write, then one multi-problem evaluation of the concatenated bands (DESIGN.md §7).
-int svsdf_map_clearance_multi(svsdf_ctx *ctx, int n, const svsdf_clearance_problem *problems, double d_max, svsdf_clearance *out,
-                              int *status_out) {
-    if (!ctx) return SVSDF_ERR_INVALID;
+// The checks of svsdf_map_clearance[_multi] (`multi`: messages name the call and the problem), then the bands.  Nothing is launched
+// for n = 0 or when a check fails.
+int clearance_bands(svsdf_ctx *ctx, bool multi, int n, const svsdf_clearance_problem *problems, double d_max, ClearanceBands &B) {
+    const std::string who = multi ? "svsdf_map_clearance_multi" : "svsdf_map_clearance";
     auto invalid = [&](const std::string &msg) {
         ctx->err = msg;
         return SVSDF_ERR_INVALID;
     };
-    if (n < 0 || n > kMaxMultiProblems || (n > 0 && (!problems || !out || !status_out)))
-        return invalid("svsdf_map_clearance_multi: needs 0 <= n <= 65535 and the problem, output and status arrays");
-    for (int k = 0; k < n; ++k) {
-        clearance_empty(&out[k]);
-        status_out[k] = SVSDF_ERR_INVALID;
-    }
-    if (!(d_max >= 0.0)) return invalid("svsdf_map_clearance_multi: d_max must be >= 0 or +INFINITY");
+    B.off.assign(n + 1, 0);
+    // the band proves only "outer value > d_max"; for d_max >= 0 that value is the whole answer (no interior branch), below 0 it is not
+    if (!(d_max >= 0.0)) return invalid(who + ": d_max must be >= 0 or +INFINITY");
     std::vector<double> dur(n);
     for (int k = 0; k < n; ++k) {
+        const svsdf_clearance_problem &p = problems[k];
         const char *msg = nullptr;
-        if (clearance_traj(problems[k].N, problems[k].T, problems[k].coeffs, dur[k], &msg) != SVSDF_OK)
-            return invalid(std::string("svsdf_map_clearance_multi: problem ") + std::to_string(k) + ": " + msg);
+        BlobLayout L;
+        bool ok = traj_layout(p.N, p.T, p.coeffs, L, dur[k], &msg) == SVSDF_OK;
+        for (int64_t e = 0; ok && e < 18 * (int64_t)p.N; ++e)
+            if (!std::isfinite(p.coeffs[e])) {
+                ok = false;
+                msg = "svsdf_map_clearance: non-finite trajectory coefficient";
+            }
+        if (!ok) return invalid(multi ? who + ": problem " + std::to_string(k) + ": " + msg : std::string(msg));
     }
     if (n == 0) return SVSDF_OK;
     if (!ctx->map()) {
-        ctx->err = "svsdf_map_clearance_multi: map not set";
+        ctx->err = who + ": map not set";
         return SVSDF_ERR_NOT_READY;
     }
-    if ((int64_t)ctx->map_X * ctx->map_Y > 2000000000LL) return invalid("svsdf_map_clearance_multi: map has more than 2e9 columns");
-    ClearanceArgs A = clearance_args(ctx);
+    if ((int64_t)ctx->map_X * ctx->map_Y > 2000000000LL) return invalid(who + ": map has more than 2e9 columns");
+    ClearanceArgs A;
+    std::memset(&A, 0, sizeof(A));
+    A.map = ctx->map();
+    A.X = ctx->map_X; A.Y = ctx->map_Y; A.h = ctx->map_h; A.row_bytes = ctx->map_row_bytes; A.Z = ctx->map_Z;
+    A.layer = (int64_t)(A.X + 2 * A.h) * A.row_bytes;
+    A.ox = ctx->map_ox; A.oy = ctx->map_oy; A.res = ctx->map_res;
     // per problem: its samples and its reach rectangle (the bounding box of the samples' discs, padded outwards by a relative margin far
     // above the rounding of the kernel's test dx*dx + dy*dy <= r*r, then by one cell; clipped to the map), padded to whole CTAs
     std::vector<ClearanceProblem> cp(n + 1);
@@ -2204,7 +2121,7 @@ int svsdf_map_clearance_multi(svsdf_ctx *ctx, int n, const svsdf_clearance_probl
             const svsdf_clearance_problem &p = problems[k];
             c.all = clearance_samples(ctx, p.N, p.T, p.coeffs, dur[k], d_max, samp) ? 1 : 0;
             c.n_samp = (int)(samp.size() / 3);
-            if (c.n_samp > kSweptMaxSamples) return invalid("svsdf_map_clearance_multi: too many path samples");
+            if (c.n_samp > kSweptMaxSamples) return invalid(who + ": too many path samples");
             c.samp0 = (int)(samp_all.size() / 3);
             samp_all.insert(samp_all.end(), samp.begin(), samp.end());
             if (!c.all) {
@@ -2224,14 +2141,19 @@ int svsdf_map_clearance_multi(svsdf_ctx *ctx, int n, const svsdf_clearance_probl
             c.wy0 = (j0 + A.h) / 32;
             c.nW = (j1 + A.h) / 32 - c.wy0 + 1;
             c.n_items = (int64_t)(i1 - i0 + 1) * c.nW;
-            if (k < n) cells += 32 * c.n_items;
+            // the map cells its words hold (its band is a subset of them): its rows times the map columns y0 .. y1 - 1 of its words
+            const int64_t y0 = std::max(32 * (int64_t)c.wy0 - A.h, (int64_t)0), y1 = std::min(32 * (int64_t)(c.wy0 + c.nW) - A.h, (int64_t)A.Y);
+            if (k < n) cells += (int64_t)(i1 - i0 + 1) * (y1 - y0);
         } else {
             c.nW = 1;
         }
         cta += (c.n_items + 255) / 256;
     }
-    if (cells > 2147483647LL || cta > 2147483647LL / 256)
-        return invalid("svsdf_map_clearance_multi: the problems' rectangles hold more than 2^31 - 1 cells");
+    // Band positions, the per-CTA prefix (k_sw_scan) and the band total are int32, and so are the CTA indices (grid x dimension).  The
+    // map cells of the rectangles' words bound the band total; one problem holds at most X Y <= 2e9 of them, so a single trajectory
+    // is never refused here.  A problem's words are no more than its cells, so its CTAs number at most cells / 256 + 1.
+    if (cells > 2147483647LL || cta > 2147483647LL)
+        return invalid(who + ": the problems' rectangles hold more than 2^31 - 1 cells");
     CK(cudaSetDevice(ctx->device));
     const int nblk = (int)cta;
     A.n_items = (int64_t)nblk * 256;
@@ -2253,47 +2175,104 @@ int svsdf_map_clearance_multi(svsdf_ctx *ctx, int n, const svsdf_clearance_probl
     A.band = reinterpret_cast<unsigned *>(ctx->d_cl_band.get());
     cudaStream_t st = ctx->stream;
     CK(cudaMemcpyAsync(ctx->d_cl_small, hs, small, cudaMemcpyHostToDevice, st));
-    CK(launch_clearance(2, A, st));
+    CK(launch_clearance(0, A, st));
     CK(launch_swept_scan(A.blk, nblk, 1, reinterpret_cast<int *>(ctx->d_cl_small + 8), st));
     CK(cudaMemcpyAsync(hs, ctx->d_cl_small, off_prob, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     ctx->launches += 2;
-    unsigned long long n_occ;
-    std::memcpy(&n_occ, hs, 8);
-    std::vector<int64_t> off(n + 1);  // problem k's band: cells off[k] .. off[k + 1] - 1 of the concatenation
-    for (int k = 0; k <= n; ++k) off[k] = reinterpret_cast<const int *>(hs + off_blk)[cp[k].cta0];
-    const int64_t P = off[n];
-    const size_t o_pts = align16((size_t)P * 8), o_sdf = o_pts + (size_t)P * 16, o_ts = o_sdf + (size_t)P * 8, o_end = o_ts + (size_t)P * 8;
+    std::memcpy(&B.n_occ, hs, 8);
+    for (int k = 0; k <= n; ++k) B.off[k] = reinterpret_cast<const int *>(hs + off_blk)[cp[k].cta0];
+    const int64_t P = B.off[n];
+    B.o_pts = align16((size_t)P * 8);
+    B.o_sdf = B.o_pts + (size_t)P * 16;
+    B.o_ts = B.o_sdf + (size_t)P * 8;
+    B.o_end = B.o_ts + (size_t)P * 8;
     if (P > 0) {
-        CK(ctx->d_cl_point.reserve(o_end + 16));
+        CK(ctx->d_cl_point.reserve(B.o_end + 16));
         A.ij = reinterpret_cast<int *>(ctx->d_cl_point.get());
-        A.pts = reinterpret_cast<double *>(ctx->d_cl_point + o_pts);
-        CK(launch_clearance(3, A, st));
+        A.pts = reinterpret_cast<double *>(ctx->d_cl_point + B.o_pts);
+        CK(launch_clearance(1, A, st));
         ctx->launches += 1;
+    }
+    return SVSDF_OK;
+}
+
+// the band cells (all problems) with their values and t*, from the device into the host stage
+int clearance_download(svsdf_ctx *ctx, const ClearanceBands &B) {
+    CK(ctx->h_stage.reserve(B.o_end));
+    CK(cudaMemcpyAsync(ctx->h_stage, ctx->d_cl_point, B.o_end, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    return SVSDF_OK;
+}
+
+// the list and summary of problem k from the host stage
+int clearance_out(svsdf_ctx *ctx, const ClearanceBands &B, int k, double d_max, svsdf_clearance *out) {
+    const unsigned char *hs = ctx->h_stage;
+    const int64_t o = B.off[k];
+    return clearance_list(ctx, B.off[k + 1] - o, reinterpret_cast<const int32_t *>(hs) + 2 * o, reinterpret_cast<const double *>(hs + B.o_pts) + 2 * o,
+                          reinterpret_cast<const double *>(hs + B.o_sdf) + o, reinterpret_cast<const double *>(hs + B.o_ts) + o, B.n_occ, d_max, out);
+}
+}  // namespace
+
+int svsdf_map_clearance(svsdf_ctx *ctx, int N, const double *T, const double *coeffs, double d_max, svsdf_clearance *out) {
+    if (!ctx || !out) return SVSDF_ERR_INVALID;
+    clearance_empty(out);
+    const svsdf_clearance_problem p{N, T, coeffs};
+    ClearanceBands B;
+    int rc = clearance_bands(ctx, false, 1, &p, d_max, B);
+    if (rc) return rc;
+    const int64_t P = B.off[1];
+    if (P > 0) {
+        // svsdf_query's path (outer solve, then the interior branch) on the band: the same kernels, so the same bits per point
+        rc = upload_traj(ctx, N, T, coeffs, P);
+        if (rc) return rc;
+        double *pts = reinterpret_cast<double *>(ctx->d_cl_point + B.o_pts);
+        rc = run_kernels(ctx, pts, P, false, true, reinterpret_cast<double *>(ctx->d_cl_point + B.o_sdf),
+                         reinterpret_cast<double *>(ctx->d_cl_point + B.o_ts), nullptr, nullptr);
+        if (rc) return rc;
+        rc = clearance_download(ctx, B);
+        if (rc) return rc;
+    }
+    return clearance_out(ctx, B, 0, d_max, out);
+}
+
+// The bands of all problems in one count / scan / write, then one multi-problem evaluation of the concatenated bands (DESIGN.md §7).
+int svsdf_map_clearance_multi(svsdf_ctx *ctx, int n, const svsdf_clearance_problem *problems, double d_max, svsdf_clearance *out,
+                              int *status_out) {
+    if (!ctx) return SVSDF_ERR_INVALID;
+    if (n < 0 || n > kMaxMultiProblems || (n > 0 && (!problems || !out || !status_out))) {
+        ctx->err = "svsdf_map_clearance_multi: needs 0 <= n <= 65535 and the problem, output and status arrays";
+        return SVSDF_ERR_INVALID;
+    }
+    for (int k = 0; k < n; ++k) {
+        clearance_empty(&out[k]);
+        status_out[k] = SVSDF_ERR_INVALID;
+    }
+    ClearanceBands B;
+    int rc = clearance_bands(ctx, true, n, problems, d_max, B);
+    if (rc || n == 0) return rc;
+    if (B.off[n] > 0) {
         // the problems with a band, in problem order: their points are the concatenation's, in the same order
         std::vector<MultiItem> items;
         for (int k = 0; k < n; ++k) {
-            if (off[k + 1] == off[k]) continue;
+            if (B.off[k + 1] == B.off[k]) continue;
             MultiItem it;
-            it.N = problems[k].N; it.T = problems[k].T; it.coeffs = problems[k].coeffs; it.P = off[k + 1] - off[k];
+            it.N = problems[k].N; it.T = problems[k].T; it.coeffs = problems[k].coeffs; it.P = B.off[k + 1] - B.off[k];
             items.push_back(it);
         }
-        const PointQuery pq{A.pts, reinterpret_cast<double *>(ctx->d_cl_point + o_sdf), reinterpret_cast<double *>(ctx->d_cl_point + o_ts)};
-        int rc = run_multi(ctx, items.data(), (int)items.size(), nullptr, &pq);
+        const PointQuery pq{reinterpret_cast<double *>(ctx->d_cl_point + B.o_pts), reinterpret_cast<double *>(ctx->d_cl_point + B.o_sdf),
+                            reinterpret_cast<double *>(ctx->d_cl_point + B.o_ts)};
+        rc = run_multi(ctx, items.data(), (int)items.size(), nullptr, &pq);
         if (rc) return rc;
         for (const MultiItem &it : items)
-            if (it.rc != SVSDF_OK) return invalid("svsdf_map_clearance_multi: a problem was refused by the evaluation");
-        CK(ctx->h_stage.reserve(o_end));
-        hs = ctx->h_stage;
-        CK(cudaMemcpyAsync(hs, ctx->d_cl_point, o_end, cudaMemcpyDeviceToHost, st));
-        CK(cudaStreamSynchronize(st));
+            if (it.rc != SVSDF_OK) {
+                ctx->err = "svsdf_map_clearance_multi: a problem was refused by the evaluation";
+                return SVSDF_ERR_INVALID;
+            }
+        rc = clearance_download(ctx, B);
+        if (rc) return rc;
     }
-    for (int k = 0; k < n; ++k) {
-        const int64_t o = off[k];
-        status_out[k] = clearance_list(ctx, off[k + 1] - o, reinterpret_cast<const int32_t *>(hs) + 2 * o, reinterpret_cast<const double *>(hs + o_pts) + 2 * o,
-                                       reinterpret_cast<const double *>(hs + o_sdf) + o, reinterpret_cast<const double *>(hs + o_ts) + o, n_occ,
-                                       d_max, &out[k]);
-    }
+    for (int k = 0; k < n; ++k) status_out[k] = clearance_out(ctx, B, k, d_max, &out[k]);
     return SVSDF_OK;
 }
 

@@ -237,14 +237,14 @@ struct SweptArgs {
     int *segs, *tris;          // [S][2], [F][3]
 };
 
-// svsdf_map_clearance (svsdf_clearance.cu): the occupied map columns near a trajectory.  One item per 32-cell word of a map row (the
-// words that hold real cells, rows 0 .. X - 1), 256 items per CTA, row-major: the CTA order is the map order.
-// svsdf_map_clearance_multi: problem k covers the words of its reach rectangle, row-major, padded to whole CTAs (cta0[k] ..).
+// svsdf_map_clearance[_multi] (svsdf_clearance.cu): the occupied map columns near n trajectories.  Problem k covers the words of its
+// reach rectangle (the 32-cell words of its rows that hold its columns), one item per word, row-major, padded to whole CTAs of 256
+// (cta0[k] ..); a last segment covers the whole map and counts its occupied columns.  The CTA order is problem order, then map order.
 struct ClearanceProblem {
     int64_t cta0;              // first CTA
     int64_t n_items;           // rows * nW (0: the rectangle misses the map)
     int i0, wy0, nW;           // first row, first word of a row, words per row
-    int all;                   // every occupied column of the rectangle is in the band
+    int all;                   // every occupied column of the rectangle is in the band (d_max = +inf or no far-field bound)
     int samp0, n_samp;         // its samples in ClearanceArgs::samp
     int occ_only;              // the last segment: the whole map, counts the occupied columns, no band
     int pad_;
@@ -254,17 +254,14 @@ struct ClearanceArgs {
     int X, Y, h, row_bytes, Z;
     int64_t layer;             // bytes per layer
     double ox, oy, res;        // boundary_xyzmin (x, y) and grid resolution
-    int wy0, nW;               // first word of a row that holds a real cell, words per row
-    int64_t n_items;           // X * nW
-    int all;                   // 1: every occupied column is in the band (d_max = +inf or a shape without a far-field bound)
-    int n_samp;
-    const double *samp;        // [n_samp][3]: sample x, y and its reach (a centre farther than reach from every sample is > d_max)
+    int64_t n_items;           // 256 x the CTAs of all segments
+    const double *samp;        // [..][3]: sample x, y and its reach (a centre farther than reach from every sample is > d_max)
     unsigned *band;            // [n_items] band bits of the word (k_cl_count)
     int *blk;                  // [n_blocks + 1] band cells per CTA, then their exclusive prefix (k_sw_scan)
     unsigned long long *n_occ; // occupied columns of the map
-    int *ij;                   // [P][2] band cells in map order: (i, j)
+    int *ij;                   // [P][2] band cells, problem by problem, each in map order: (i, j)
     double *pts;               // [P][2] their centres
-    int n_prob;                // svsdf_map_clearance_multi: problems + 1 (the occupied-column segment); 0 for the single call
+    int n_prob;                // problems + 1 (the occupied-column segment)
     const ClearanceProblem *prob;
 };
 

@@ -216,8 +216,8 @@ void svsdf_clearance_free(svsdf_clearance *c);
  * svsdf_map_clearance(ctx, N_k, T_k, coeffs_k, d_max, ...) on the same context bit for bit (counts, list and summary), and status_out[k]
  * is the status that call would return (SVSDF_OK or SVSDF_ERR_NONFINITE; a problem whose status is not OK has no arrays allocated).
  *   0 <= n <= 65535; n = 0 does nothing.  The call is refused before any work (SVSDF_ERR_INVALID, nothing allocated) for a bad d_max,
- *   any bad trajectory (N outside 1 .. 64, bad durations, non-finite coefficients), or when the problems' reach rectangles together hold
- *   more than 2^31 - 1 cells; SVSDF_ERR_NOT_READY without a map.
+ *   any bad trajectory (N outside 1 .. 64, bad durations, non-finite coefficients), or when the map cells in the 32-cell words of the
+ *   problems' reach rectangles number more than 2^31 - 1 together (never for n = 1); SVSDF_ERR_NOT_READY without a map.
  *   Each problem evaluates only the occupied columns of its reach rectangle (the bounding box of its samples' reach, padded outwards):
  *   the band is that of the single call.  The occupied columns of the map are counted once per call.  A fixed number of kernel
  *   launches, whatever n and the map size (none of the evaluation's when no problem has a band); the context's resident points,

@@ -1,6 +1,7 @@
 """GPU (-m gpu): svsdf_map_clearance — the band result against the dense alternative (svsdf_query(outer_only = 0) on the centre of every
 occupied column, filtered at d_max by oracle/clearance_oracle.py), bit for bit, over shapes, pre-transforms, the mesh functor, the scale
-schedule, both builds, N = 1 .. 64, d_max = 0 / safety_hor / 3 / +inf and 2-D and 3-D maps; the strict build against the CPU oracle; a
+schedule, both builds, N = 1 .. 64, d_max = 0 / safety_hor / 3 / +inf, 2-D and 3-D maps, reach rectangles clipped by the map's
+edges and paths outside the map; the strict build against the CPU oracle; a
 scene where the band bound decides; non-interference, determinism, launches, errors; certified plans."""
 import math
 import os
@@ -61,6 +62,13 @@ def path_xy(T, co):
         tp = t[:, None] ** np.arange(6)
         out.append(np.c_[tp @ c[0, 6 * i:6 * i + 6], tp @ c[1, 6 * i:6 * i + 6]])
     return np.concatenate(out)
+
+
+def far_x(T, co, dx=500.0):
+    """The trajectory moved by dx along x (every piece's constant term)."""
+    co = np.array(co, dtype=np.float64)
+    co[0:6 * len(T):6] += dx
+    return co
 
 
 def pack2d(occ, ks=KS, pad=True):
@@ -131,6 +139,12 @@ def test_band_equals_dense_every_shape(shape, pp):
     occ, origin, res = scene_map(T, co, 5)
     rs = check(ctx, T, co, occ, origin, res)
     assert rs[1].n_evaluated < rs[1].n_occupied and rs[3].n_within == rs[3].n_occupied
+    # the reach rectangle clipped by the map's edges (the middle third of the map in x, which the path crosses), and a path entirely
+    # outside the map (an empty rectangle below d_max = +inf)
+    X = occ.shape[0]
+    check(ctx, T, co, occ[X // 3:2 * X // 3], (origin[0] + (X // 3) * res, origin[1]), res)
+    rs = check(ctx, T, far_x(T, co), occ, origin, res)
+    assert rs[0].n_evaluated == rs[1].n_evaluated == rs[2].n_evaluated == 0
     ctx.close()
 
 
@@ -222,6 +236,9 @@ def test_non_interference_determinism_launches_and_manager():
         n0 = ctx.kernel_launches()
         res.append(ctx.map_clearance(T, co, 0.7))
         launches.append(ctx.kernel_launches() - n0)
+    n0 = ctx.kernel_launches()
+    r = ctx.map_clearance(T, far_x(T, co), 0.7)
+    assert ctx.kernel_launches() - n0 == 2 and r.n_evaluated == 0  # no column near the path: count and scan only
     after = ctx.cost_grad(T, co)
     for x, y in zip(ref, after):
         assert np.array_equal(bits(x), bits(y))
