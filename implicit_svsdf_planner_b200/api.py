@@ -240,7 +240,7 @@ EXPORTED_SYMBOLS = [
     "svsdf_lmbm_default_params", "svsdf_lmbm_open", "svsdf_lmbm_close", "svsdf_lmbm_last_error", "svsdf_lmbm_minimize", "svsdf_set_lmbm_library", "svsdf_read_obj", "svsdf_free", "svsdf_mesh_fwn_host",
     "svsdf_front_init", "svsdf_front_get_kernels", "svsdf_front_cspace", "svsdf_front_check_kernel_value", "svsdf_front_expand", "svsdf_front_astar",
     "svsdf_front_astar_device", "svsdf_set_scale", "svsdf_scale_matrix",
-    "svsdf_cost_grad_multi", "svsdf_optimize_lockstep", "svsdf_lockstep_rounds", "svsdf_swept_contour", "svsdf_swept_free",
+    "svsdf_cost_grad_multi", "svsdf_optimize_lockstep", "svsdf_lockstep_rounds", "svsdf_optimize_device", "svsdf_round_times", "svsdf_swept_contour", "svsdf_swept_free",
     "svsdf_map_clearance", "svsdf_clearance_free", "svsdf_map_clearance_multi",
 ]
 
@@ -322,6 +322,9 @@ def lib():
     L.svsdf_optimize_lockstep.argtypes = [vp, C.POINTER(LockstepProblem), C.c_int, C.POINTER(LbfgsParams), C.c_int, C.POINTER(OptStats),
                                           C.POINTER(C.c_int)]
     L.svsdf_lockstep_rounds.argtypes = [vp, C.POINTER(C.c_int64)]
+    L.svsdf_optimize_device.argtypes = [vp, C.POINTER(LockstepProblem), C.c_int, C.POINTER(LbfgsParams), C.c_int, C.POINTER(OptStats),
+                                        C.POINTER(C.c_int), C.POINTER(C.c_int64)]
+    L.svsdf_round_times.argtypes = [vp, dp, dp]
     L.svsdf_swept_contour.argtypes = [vp, C.c_int, dp, dp, C.POINTER(SweptParams), C.POINTER(SweptMesh)]
     L.svsdf_swept_free.argtypes = [C.POINTER(SweptMesh)]
     L.svsdf_swept_free.restype = None
@@ -802,9 +805,7 @@ class Context:
         self._ck(lib().svsdf_cost_grad_multi(self.h, n, arr), "svsdf_cost_grad_multi")
         return [(float(c[0]), gT, gC, int(ni[0])) for c, gT, gC, ni in res]
 
-    def optimize_lockstep(self, problems, params: LbfgsParams | None = None, max_in_flight: int = 0):
-        """svsdf_optimize_lockstep: problems = list of dicts with init_s, final_s (3x3), x0, N and points [P, >= 2].  Returns
-        (results, rounds): per problem a dict (status, x, T, coeffs, cost_at_start, and the stats of optimize) equal to optimize's bits."""
+    def _lockstep_call(self, fn, name, problems, params, max_in_flight):
         n = len(problems)
         arr = (LockstepProblem * max(n, 1))()
         keep, outs = [], []
@@ -823,8 +824,8 @@ class Context:
             outs.append((x, T, b, f0))
         stats = (OptStats * max(n, 1))()
         status = np.zeros(max(n, 1), dtype=np.int32)
-        self._ck(lib().svsdf_optimize_lockstep(self.h, arr, n, C.byref(params) if params is not None else None, int(max_in_flight), stats,
-                                               status.ctypes.data_as(C.POINTER(C.c_int))), "svsdf_optimize_lockstep")
+        self._ck(fn(self.h, arr, n, C.byref(params) if params is not None else None, int(max_in_flight), stats,
+                    status.ctypes.data_as(C.POINTER(C.c_int))), name)
         rounds = C.c_int64()
         lib().svsdf_lockstep_rounds(self.h, C.byref(rounds))
         res = []
@@ -834,6 +835,23 @@ class Context:
                             iterations=s.iterations, evaluations=s.evaluations, solver_status=s.status, seconds=s.seconds,
                             gpu_seconds=s.gpu_seconds))
         return res, rounds.value
+
+    def optimize_lockstep(self, problems, params: LbfgsParams | None = None, max_in_flight: int = 0):
+        """svsdf_optimize_lockstep: problems = list of dicts with init_s, final_s (3x3), x0, N and points [P, >= 2].  Returns
+        (results, rounds): per problem a dict (status, x, T, coeffs, cost_at_start, and the stats of optimize) equal to optimize's bits."""
+        return self._lockstep_call(lib().svsdf_optimize_lockstep, "svsdf_optimize_lockstep", problems, params, max_in_flight)
+
+    def optimize_device(self, problems, params: LbfgsParams | None = None, max_in_flight: int = 0):
+        """svsdf_optimize_device: optimize_lockstep with the L-BFGS and MINCO of every problem on the device.  Same problems, same
+        (results, rounds), the same bits."""
+        return self._lockstep_call(lambda h, arr, n, prm, mif, st, stt: lib().svsdf_optimize_device(h, arr, n, prm, mif, st, stt, None),
+                                   "svsdf_optimize_device", problems, params, max_in_flight)
+
+    def round_times(self):
+        """svsdf_round_times: device ms of the last lock-step / device back end's rounds: (evaluation kernels, back-end kernels)."""
+        e, b = C.c_double(), C.c_double()
+        self._ck(lib().svsdf_round_times(self.h, C.cast(C.byref(e), dp), C.cast(C.byref(b), dp)), "svsdf_round_times")
+        return e.value, b.value
 
     def shape_sdf(self, rel):
         rel = _f64(rel).reshape(-1, 3)

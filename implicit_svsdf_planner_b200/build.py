@@ -38,6 +38,7 @@ UNITS = [
     ("svsdf_frontend.cu", "svsdf_frontend.o", ["-fmad=false"]),  # shape kernels: same rounding as the strict functors
     ("svsdf_swept.cu", "svsdf_swept.o", ["-fmad=false"]),  # swept-volume mesher: vertices independent of the field's build
     ("svsdf_clearance.cu", "svsdf_clearance.o", ["-fmad=false"]),  # map clearance: cell centres round like svsdf_extract's
+    ("svsdf_backend.cu", "svsdf_backend.o", ["-fmad=false"]),  # device L-BFGS / MINCO: the host unit's bits (it has -ffp-contract=off)
     # host threads for the batch A* bookkeeping; no a*b+c contraction in the float winding-number builder (host/fwn_bvh.hpp)
     ("svsdf_runtime.cpp", "svsdf_runtime.o", ["-Xcompiler", "-fopenmp", "-Xcompiler", "-ffp-contract=off"]),
 ]
@@ -48,6 +49,7 @@ HEADERS = [
     "svsdf_sincos.cuh",
     "svsdf_types.h",
     "svsdf_launch.h",
+    "svsdf_backend.h",
     "host/minco.hpp",
     "host/lbfgs.hpp",
     "host/astar.hpp",

@@ -1,12 +1,19 @@
-// host/lbfgs.hpp — host outer optimiser of the drop-in: limited-memory BFGS with the Lewis–Overton weak-Wolfe
-// line search (suitable for the piecewise-smooth SVSDF cost).  Algorithm and return codes follow the clean
-// LBFGS-Lite the reference vendors (src/utils/include/utils/lbfgs_ref.hpp:276-395 line search, :434-716 driver);
-// re-implemented without Eigen on plain arrays and re-entrant (no static state, unlike the reference's LMBM
-// wrapper src/utils/include/utils/lmbm.cpp:4-6), so many problems can be optimised concurrently in batch mode.
+// host/lbfgs.hpp — outer optimiser of the drop-in: limited-memory BFGS with the Lewis–Overton weak-Wolfe line search (suitable for
+// the piecewise-smooth SVSDF cost).  Algorithm and return codes follow the clean LBFGS-Lite the reference vendors
+// (src/utils/include/utils/lbfgs_ref.hpp:276-395 line search, :434-716 driver); re-implemented without Eigen on plain arrays and
+// re-entrant (no static state, unlike the reference's LMBM wrapper src/utils/include/utils/lmbm.cpp:4-6).
+//
+// The solver is a machine that stops whenever it needs its caller (lbfgs_begin / lbfgs_step): to evaluate f and g at x, or to run
+// the progress hook.  Its state is one LbfgsMachine and caller-provided flat storage (LbfgsArrays), so the same code runs in a host
+// loop (Lbfgs::minimize) and, on one lane of each problem's warp, on the device (svsdf_backend.cu, svsdf_optimize_device).  Both builds keep
+// the operations in this order without contraction (host: -ffp-contract=off, device: -fmad=false); division and sqrt are
+// correctly rounded on both sides, so both give the same bits.
 #pragma once
-#include <algorithm>
 #include <cmath>
+#include <cstddef>
 #include <vector>
+
+#include "../svsdf_types.h"
 
 namespace svsdf {
 namespace host {
@@ -69,196 +76,330 @@ struct LbfgsResult {
     int status = 0;
 };
 
+// What the machine asks of its caller after lbfgs_begin / lbfgs_step.
+enum LbfgsAsk {
+    LBFGS_DONE = 0,      // finished: LbfgsMachine::R holds the result, x the returned iterate
+    LBFGS_EVAL = 1,      // evaluate f and g at x; g goes to lbfgs_eval_grad(M, A); then lbfgs_step(.., f, 0)
+    LBFGS_PROGRESS = 2,  // after an accepted line search: the progress hook at (x, M.k); then lbfgs_step(.., 0, cancel)
+};
+
+// Caller-provided storage of one run on n variables (lbfgs_doubles(P, n) doubles besides x; lbfgs_arrays carves it).
+struct LbfgsArrays {
+    double *x, *xp, *g, *gp, *d, *gs, *pf, *S, *Y, *ys_hist, *alpha;
+};
+
+struct LbfgsMachine {
+    int n, next, k, head, stored, restarts, count, ls, bracketed, touched, into_gs;
+    double fx, step, fx_before, olddnorm, lo, hi, finit, dgtest, dstest;
+    LbfgsResult R;
+};
+
+// the comparisons of std::max / std::min (not fmax / fmin, whose NaN rule differs)
+SVSDF_HD inline double lbfgs_max(double a, double b) { return a < b ? b : a; }
+SVSDF_HD inline int lbfgs_imax(int a, int b) { return a < b ? b : a; }
+SVSDF_HD inline int lbfgs_imin(int a, int b) { return b < a ? b : a; }
+
+SVSDF_HD inline size_t lbfgs_doubles(const LbfgsParams &P, int n) {
+    // xp, g, gp, d, gs | pf | S, Y | ys_hist, alpha  (P must pass lbfgs_check)
+    return (size_t)5 * n + (size_t)lbfgs_imax(1, P.past) + (size_t)2 * P.mem_size * n + (size_t)2 * P.mem_size;
+}
+SVSDF_HD inline LbfgsArrays lbfgs_arrays(double *x, double *base, const LbfgsParams &P, int n) {
+    LbfgsArrays A;
+    A.x = x;
+    A.xp = base;
+    A.g = A.xp + n;
+    A.gp = A.g + n;
+    A.d = A.gp + n;
+    A.gs = A.d + n;
+    A.pf = A.gs + n;
+    A.S = A.pf + lbfgs_imax(1, P.past);
+    A.Y = A.S + (size_t)P.mem_size * n;
+    A.ys_hist = A.Y + (size_t)P.mem_size * n;
+    A.alpha = A.ys_hist + P.mem_size;
+    return A;
+}
+// where the gradient of the evaluation the machine asks for goes
+SVSDF_HD inline double *lbfgs_eval_grad(const LbfgsMachine &M, const LbfgsArrays &A) { return M.into_gs ? A.gs : A.g; }
+
+SVSDF_HD inline int lbfgs_check(const LbfgsParams &P, int n) {
+    if (n <= 0) return LBFGSERR_INVALID_N;
+    if (P.mem_size <= 0) return LBFGSERR_INVALID_MEMSIZE;
+    if (P.g_epsilon < 0.0) return LBFGSERR_INVALID_GEPSILON;
+    if (P.past < 0) return LBFGSERR_INVALID_TESTPERIOD;
+    if (P.delta < 0.0) return LBFGSERR_INVALID_DELTA;
+    if (P.min_step < 0.0) return LBFGSERR_INVALID_MINSTEP;
+    if (P.max_step < P.min_step) return LBFGSERR_INVALID_MAXSTEP;
+    if (!(P.f_dec_coeff > 0.0 && P.f_dec_coeff < 1.0)) return LBFGSERR_INVALID_FDECCOEFF;
+    if (!(P.s_curv_coeff < 1.0 && P.s_curv_coeff > P.f_dec_coeff)) return LBFGSERR_INVALID_SCURVCOEFF;
+    if (!(P.machine_prec > 0.0)) return LBFGSERR_INVALID_MACHINEPREC;
+    if (P.max_linesearch <= 0) return LBFGSERR_INVALID_MAXLINESEARCH;
+    return 0;
+}
+SVSDF_HD inline double lbfgs_dot(const double *a, const double *b, int n) {
+    double s = 0.0;
+    for (int i = 0; i < n; ++i) s += a[i] * b[i];
+    return s;
+}
+SVSDF_HD inline void lbfgs_axpy(double a, const double *x, double *y, int n) {
+    for (int i = 0; i < n; ++i) y[i] += a * x[i];
+}
+SVSDF_HD inline double lbfgs_amax(const double *a, int n) {
+    double r = 0.0;
+    for (int i = 0; i < n; ++i) r = lbfgs_max(r, std::fabs(a[i]));
+    return r;
+}
+
+// Starts a run at A.x: checks the parameters, zeroes the storage and asks for the first evaluation (or ends at once with the check's
+// code).  The storage must hold lbfgs_doubles(P, n) doubles once the check has passed.
+SVSDF_HD inline int lbfgs_begin(const LbfgsParams &P, LbfgsMachine &M, const LbfgsArrays &A, int n) {
+    M = LbfgsMachine();
+    M.n = n;
+    if ((M.R.status = lbfgs_check(P, n)) != 0) return LBFGS_DONE;
+    for (double *p = A.xp; p != A.alpha + P.mem_size; ++p) *p = 0.0;
+    M.next = 0;
+    M.into_gs = 0;
+    return LBFGS_EVAL;
+}
+
+// Resumes the machine with the value the caller was asked for (f after LBFGS_EVAL, cancel after LBFGS_PROGRESS).
+SVSDF_HD inline int lbfgs_step(const LbfgsParams &P, LbfgsMachine &M, const LbfgsArrays &A, double f, int cancel) {
+    // resume points (M.next) and internal continuations
+    enum { FIRST, LS_EVAL, PROGRESS, STEEPEST_QN, STEEPEST_SKIP, ITERATE, LS_TRY, LS_DONE, DIRECTION, FINISH };
+    const int n = M.n, m = P.mem_size;
+    double *x = A.x, *xp = A.xp, *g = A.g, *gp = A.gp, *d = A.d;
+    int at = M.next;
+    for (;;) {
+        switch (at) {
+            case FIRST:
+                M.fx = f;
+                M.R.evaluations = 1;
+                if (!std::isfinite(M.fx)) {  // a failed first evaluation (NaN cost, g left at zero) must not read as convergence
+                    M.R.status = LBFGSERR_INVALID_FUNCVAL;
+                    M.R.f = M.fx;
+                    return LBFGS_DONE;
+                }
+                A.pf[0] = M.fx;
+                for (int i = 0; i < n; ++i) d[i] = -g[i];
+                M.k = 0;
+                if (lbfgs_amax(g, n) / lbfgs_max(1.0, lbfgs_amax(x, n)) <= P.g_epsilon) {
+                    M.R.status = LBFGS_CONVERGENCE;
+                    at = FINISH;
+                    break;
+                }
+                M.step = 1.0 / std::sqrt(lbfgs_dot(d, d, n));
+                M.head = M.stored = M.restarts = 0;
+                M.olddnorm = 1.0;
+                M.k = 1;
+                at = ITERATE;
+                break;
+            case ITERATE: {  // top of the iteration: save the point, then the line search's set-up
+                for (int i = 0; i < n; ++i) xp[i] = x[i];
+                for (int i = 0; i < n; ++i) gp[i] = g[i];
+                M.step = M.step < P.max_step ? M.step : 0.5 * P.max_step;
+                M.fx_before = M.fx;
+                if (!(M.step > 0.0)) {
+                    M.ls = LBFGSERR_INVALIDPARAMETERS;
+                    at = LS_DONE;
+                    break;
+                }
+                const double dginit = lbfgs_dot(gp, d, n);
+                if (0.0 < dginit) {
+                    M.ls = LBFGSERR_INCREASEGRADIENT;
+                    at = LS_DONE;
+                    break;
+                }
+                M.finit = M.fx;
+                M.dgtest = P.f_dec_coeff * dginit;
+                M.dstest = P.s_curv_coeff * dginit;
+                M.lo = 0.0;
+                M.hi = P.max_step;
+                M.bracketed = M.touched = 0;
+                M.count = 1;
+                at = LS_TRY;
+                break;
+            }
+            case LS_TRY:
+                for (int i = 0; i < n; ++i) x[i] = xp[i] + M.step * d[i];
+                M.next = LS_EVAL;
+                M.into_gs = 0;
+                return LBFGS_EVAL;
+            case LS_EVAL:  // Lewis–Overton: Armijo + weak Wolfe by bisection / doubling
+                M.fx = f;
+                ++M.R.evaluations;
+                at = LS_DONE;
+                if (std::isinf(M.fx) || std::isnan(M.fx)) {
+                    M.ls = LBFGSERR_INVALID_FUNCVAL;
+                    break;
+                }
+                if (M.fx > M.finit + M.step * M.dgtest) {
+                    M.hi = M.step;
+                    M.bracketed = 1;
+                } else if (!P.reference_patch && lbfgs_dot(g, d, n) < M.dstest) {
+                    M.lo = M.step;
+                } else {
+                    M.ls = M.count;
+                    break;
+                }
+                if (P.max_linesearch <= M.count) {
+                    M.ls = LBFGSERR_MAXIMUMLINESEARCH;
+                    break;
+                }
+                if (M.bracketed && (M.hi - M.lo) < P.machine_prec * M.hi) {
+                    M.ls = LBFGSERR_WIDTHTOOSMALL;
+                    break;
+                }
+                M.step = M.bracketed ? 0.5 * (M.lo + M.hi) : M.step * 2.0;
+                if (M.step < P.min_step) {
+                    M.ls = LBFGSERR_MINIMUMSTEP;
+                    break;
+                }
+                if (M.step > P.max_step) {
+                    if (M.touched) {
+                        M.ls = LBFGSERR_MAXIMUMSTEP;
+                        break;
+                    }
+                    M.touched = 1;
+                    M.step = P.max_step;
+                }
+                ++M.count;
+                at = LS_TRY;
+                break;
+            case LS_DONE:
+                if (M.ls < 0) {
+                    for (int i = 0; i < n; ++i) x[i] = xp[i];
+                    for (int i = 0; i < n; ++i) g[i] = gp[i];
+                    M.fx = M.fx_before;
+                    const int ls = M.ls;
+                    const bool recoverable = ls == LBFGSERR_MAXIMUMLINESEARCH || ls == LBFGSERR_MINIMUMSTEP || ls == LBFGSERR_WIDTHTOOSMALL ||
+                                             ls == LBFGSERR_INCREASEGRADIENT || ls == LBFGSERR_MAXIMUMSTEP;
+                    at = FINISH;
+                    if (P.nonsmooth_restarts > 0 && recoverable) {
+                        if (M.stored > 0 && M.restarts < P.nonsmooth_restarts) {
+                            // the quasi-Newton model is wrong across a kink: forget it and search along -g from here
+                            ++M.restarts;
+                            M.stored = 0;
+                            M.head = 0;
+                            for (int i = 0; i < n; ++i) d[i] = -g[i];
+                            M.step = 1.0 / std::sqrt(lbfgs_dot(d, d, n));
+                            at = ITERATE;
+                            break;
+                        }
+                        M.R.status = LBFGS_NOMOREPROGRESS;
+                        break;
+                    }
+                    M.R.status = ls;
+                    break;
+                }
+                M.restarts = 0;
+                M.next = PROGRESS;
+                return LBFGS_PROGRESS;
+            case PROGRESS: {
+                at = FINISH;
+                if (cancel) { M.R.status = LBFGS_CANCELED; break; }
+                if (lbfgs_amax(g, n) / lbfgs_max(1.0, lbfgs_amax(x, n)) < P.g_epsilon) { M.R.status = LBFGS_CONVERGENCE; break; }
+                if (P.past > 0) {
+                    if (P.past <= M.k) {
+                        const double rate = std::fabs(A.pf[M.k % P.past] - M.fx) / lbfgs_max(1.0, std::fabs(M.fx));
+                        if (rate < P.delta) { M.R.status = LBFGS_STOP; break; }
+                    }
+                    A.pf[M.k % P.past] = M.fx;
+                }
+                if (P.max_iterations != 0 && P.max_iterations <= M.k) { M.R.status = LBFGSERR_MAXIMUMITERATION; break; }
+                ++M.k;
+                double *s = A.S + (size_t)M.head * n, *y = A.Y + (size_t)M.head * n;
+                for (int i = 0; i < n; ++i) { s[i] = x[i] - xp[i]; y[i] = g[i] - gp[i]; }
+                const double ys = lbfgs_dot(y, s, n), yy = lbfgs_dot(y, y, n);
+                A.ys_hist[M.head] = ys;
+                for (int i = 0; i < n; ++i) d[i] = -g[i];
+                // cautious update (Li & Fukushima): skip the pair when curvature is too small
+                const double cau = lbfgs_dot(s, s, n) * std::sqrt(lbfgs_dot(gp, gp, n)) * P.cautious_factor;
+                at = DIRECTION;
+                if (ys > cau) {
+                    M.stored = lbfgs_imin(m, M.stored + 1);
+                    M.head = (M.head + 1) % m;
+                    int j = M.head;
+                    for (int i = 0; i < M.stored; ++i) {  // two-loop recursion, newest to oldest
+                        j = (j + m - 1) % m;
+                        A.alpha[j] = lbfgs_dot(A.S + (size_t)j * n, d, n) / A.ys_hist[j];
+                        lbfgs_axpy(-A.alpha[j], A.Y + (size_t)j * n, d, n);
+                    }
+                    const double scale = ys / yy;
+                    for (int i = 0; i < n; ++i) d[i] *= scale;
+                    for (int i = 0; i < M.stored; ++i) {  // oldest to newest
+                        const double beta = lbfgs_dot(A.Y + (size_t)j * n, d, n) / A.ys_hist[j];
+                        lbfgs_axpy(A.alpha[j] - beta, A.S + (size_t)j * n, d, n);
+                        j = (j + 1) % m;
+                    }
+                    // (`!(|d| < 0.04)` rather than the reference's `|d| >= 0.04`: a non-finite direction — a stored pair with y.s == 0
+                    // once the iterates stop moving — also takes the fallback instead of ending the run with a NaN cost)
+                    if (P.reference_patch && (!(std::sqrt(lbfgs_dot(d, d, n)) < 0.04) || lbfgs_dot(d, g, n) > 0)) M.next = STEEPEST_QN;
+                    else break;
+                } else if (P.reference_patch) {
+                    M.next = STEEPEST_SKIP;
+                } else {
+                    break;
+                }
+                // the reference's fallback direction: re-evaluate at x (its own callback returns the same gradient again),
+                // d = -g / |g| * |d_prev|
+                for (int i = 0; i < n; ++i) A.gs[i] = 0.0;
+                M.into_gs = 1;
+                return LBFGS_EVAL;
+            }
+            case STEEPEST_QN:
+            case STEEPEST_SKIP: {
+                ++M.R.evaluations;
+                for (int i = 0; i < n; ++i) g[i] = A.gs[i];
+                for (int i = 0; i < n; ++i) d[i] = -g[i];
+                const double z = lbfgs_dot(d, d, n);
+                if (z > 0) {
+                    const double nn = std::sqrt(z);
+                    for (int i = 0; i < n; ++i) d[i] /= nn;
+                }
+                for (int i = 0; i < n; ++i) d[i] *= M.olddnorm;
+                if (at == STEEPEST_SKIP) M.head = (M.head + 1) % m;  // the slot just written is skipped without counting as stored (lbfgs.hpp:776)
+                at = DIRECTION;
+                break;
+            }
+            case DIRECTION:
+                if (P.reference_patch) M.olddnorm = std::sqrt(lbfgs_dot(d, d, n));
+                M.step = 1.0;
+                at = ITERATE;
+                break;
+            default:  // FINISH
+                M.R.f = M.fx;
+                M.R.iterations = M.k;
+                return LBFGS_DONE;
+        }
+    }
+}
+
+// The host loop around the machine: the caller's callbacks evaluate, and the progress hook runs after every accepted line search.
 class Lbfgs {
    public:
     explicit Lbfgs(const LbfgsParams &p) : P(p) {}
 
     LbfgsResult minimize(double *x, int n, lbfgs_eval_fn eval, void *inst, lbfgs_progress_fn progress, void *puser) {
-        LbfgsResult R;
-        if ((R.status = check(n)) != 0) return R;
-        const int m = P.mem_size;
-        xp.assign(n, 0.0); g.assign(n, 0.0); gp.assign(n, 0.0); d.assign(n, 0.0);
-        pf.assign(std::max(1, P.past), 0.0);
-        S.assign((size_t)m * n, 0.0); Y.assign((size_t)m * n, 0.0);
-        ys_hist.assign(m, 0.0); alpha.assign(m, 0.0);
-
-        double fx = eval(inst, x, g.data(), n);
-        R.evaluations = 1;
-        if (!std::isfinite(fx)) {  // a failed first evaluation (NaN cost, g left at zero) must not read as convergence
-            R.status = LBFGSERR_INVALID_FUNCVAL;
-            R.f = fx;
-            return R;
+        LbfgsMachine M;
+        LbfgsArrays A{};
+        A.x = x;
+        if (lbfgs_check(P, n) == 0) {
+            store.assign(lbfgs_doubles(P, n), 0.0);
+            A = lbfgs_arrays(x, store.data(), P, n);
         }
-        pf[0] = fx;
-        for (int i = 0; i < n; ++i) d[i] = -g[i];
-        int k = 0;
-        if (amax(g.data(), n) / std::max(1.0, amax(x, n)) <= P.g_epsilon) {
-            R.status = LBFGS_CONVERGENCE;
-        } else {
-            double step = 1.0 / std::sqrt(dotp(d.data(), d.data(), n));
-            int head = 0, stored = 0, restarts = 0;
-            double olddnorm = 1.0;
-            k = 1;
-            for (;;) {
-                std::copy(x, x + n, xp.begin());
-                gp = g;
-                const double step_min = P.min_step, step_max = P.max_step;
-                step = step < step_max ? step : 0.5 * step_max;
-                const double fx_before = fx;
-                int ls = line_search(x, n, fx, step, step_min, step_max, eval, inst, R.evaluations);
-                if (ls < 0) {
-                    std::copy(xp.begin(), xp.end(), x);
-                    g = gp;
-                    fx = fx_before;
-                    const bool recoverable = ls == LBFGSERR_MAXIMUMLINESEARCH || ls == LBFGSERR_MINIMUMSTEP || ls == LBFGSERR_WIDTHTOOSMALL ||
-                                             ls == LBFGSERR_INCREASEGRADIENT || ls == LBFGSERR_MAXIMUMSTEP;
-                    if (P.nonsmooth_restarts > 0 && recoverable) {
-                        if (stored > 0 && restarts < P.nonsmooth_restarts) {
-                            // the quasi-Newton model is wrong across a kink: forget it and search along -g from here
-                            ++restarts;
-                            stored = 0;
-                            head = 0;
-                            for (int i = 0; i < n; ++i) d[i] = -g[i];
-                            step = 1.0 / std::sqrt(dotp(d.data(), d.data(), n));
-                            continue;
-                        }
-                        R.status = LBFGS_NOMOREPROGRESS;
-                        break;
-                    }
-                    R.status = ls;
-                    break;
-                }
-                restarts = 0;
-                if (progress && progress(puser, x, k)) { R.status = LBFGS_CANCELED; break; }
-                if (amax(g.data(), n) / std::max(1.0, amax(x, n)) < P.g_epsilon) { R.status = LBFGS_CONVERGENCE; break; }
-                if (P.past > 0) {
-                    if (P.past <= k) {
-                        const double rate = std::fabs(pf[k % P.past] - fx) / std::max(1.0, std::fabs(fx));
-                        if (rate < P.delta) { R.status = LBFGS_STOP; break; }
-                    }
-                    pf[k % P.past] = fx;
-                }
-                if (P.max_iterations != 0 && P.max_iterations <= k) { R.status = LBFGSERR_MAXIMUMITERATION; break; }
-                ++k;
-                double *s = &S[(size_t)head * n], *y = &Y[(size_t)head * n];
-                for (int i = 0; i < n; ++i) { s[i] = x[i] - xp[i]; y[i] = g[i] - gp[i]; }
-                const double ys = dotp(y, s, n), yy = dotp(y, y, n);
-                ys_hist[head] = ys;
-                for (int i = 0; i < n; ++i) d[i] = -g[i];
-                // cautious update (Li & Fukushima): skip the pair when curvature is too small
-                const double cau = dotp(s, s, n) * std::sqrt(dotp(gp.data(), gp.data(), n)) * P.cautious_factor;
-                if (ys > cau) {
-                    stored = std::min(m, stored + 1);
-                    head = (head + 1) % m;
-                    int j = head;
-                    for (int i = 0; i < stored; ++i) {  // two-loop recursion, newest to oldest
-                        j = (j + m - 1) % m;
-                        alpha[j] = dotp(&S[(size_t)j * n], d.data(), n) / ys_hist[j];
-                        axpy(-alpha[j], &Y[(size_t)j * n], d.data(), n);
-                    }
-                    const double scale = ys / yy;
-                    for (int i = 0; i < n; ++i) d[i] *= scale;
-                    for (int i = 0; i < stored; ++i) {  // oldest to newest
-                        const double beta = dotp(&Y[(size_t)j * n], d.data(), n) / ys_hist[j];
-                        axpy(alpha[j] - beta, &S[(size_t)j * n], d.data(), n);
-                        j = (j + 1) % m;
-                    }
-                    // (`!(|d| < 0.04)` rather than the reference's `|d| >= 0.04`: a non-finite direction — a stored pair with y.s == 0
-                    // once the iterates stop moving — also takes the fallback instead of ending the run with a NaN cost)
-                    if (P.reference_patch && (!(std::sqrt(dotp(d.data(), d.data(), n)) < 0.04) || dotp(d.data(), g.data(), n) > 0))
-                        steepest_with_old_norm(x, n, eval, inst, R.evaluations, olddnorm);
-                } else if (P.reference_patch) {
-                    steepest_with_old_norm(x, n, eval, inst, R.evaluations, olddnorm);
-                    head = (head + 1) % m;  // the slot just written is skipped without counting as stored (lbfgs.hpp:776)
-                }
-                if (P.reference_patch) olddnorm = std::sqrt(dotp(d.data(), d.data(), n));
-                step = 1.0;
+        for (int ask = lbfgs_begin(P, M, A, n); ask != LBFGS_DONE;) {
+            if (ask == LBFGS_EVAL) {
+                const double f = eval(inst, x, lbfgs_eval_grad(M, A), n);
+                ask = lbfgs_step(P, M, A, f, 0);
+            } else {
+                ask = lbfgs_step(P, M, A, 0.0, progress && progress(puser, x, M.k) ? 1 : 0);
             }
         }
-        R.f = fx;
-        R.iterations = k;
-        return R;
+        return M.R;
     }
 
    private:
-    int check(int n) const {
-        if (n <= 0) return LBFGSERR_INVALID_N;
-        if (P.mem_size <= 0) return LBFGSERR_INVALID_MEMSIZE;
-        if (P.g_epsilon < 0.0) return LBFGSERR_INVALID_GEPSILON;
-        if (P.past < 0) return LBFGSERR_INVALID_TESTPERIOD;
-        if (P.delta < 0.0) return LBFGSERR_INVALID_DELTA;
-        if (P.min_step < 0.0) return LBFGSERR_INVALID_MINSTEP;
-        if (P.max_step < P.min_step) return LBFGSERR_INVALID_MAXSTEP;
-        if (!(P.f_dec_coeff > 0.0 && P.f_dec_coeff < 1.0)) return LBFGSERR_INVALID_FDECCOEFF;
-        if (!(P.s_curv_coeff < 1.0 && P.s_curv_coeff > P.f_dec_coeff)) return LBFGSERR_INVALID_SCURVCOEFF;
-        if (!(P.machine_prec > 0.0)) return LBFGSERR_INVALID_MACHINEPREC;
-        if (P.max_linesearch <= 0) return LBFGSERR_INVALID_MAXLINESEARCH;
-        return 0;
-    }
-    static double dotp(const double *a, const double *b, int n) {
-        double s = 0.0;
-        for (int i = 0; i < n; ++i) s += a[i] * b[i];
-        return s;
-    }
-    static void axpy(double a, const double *x, double *y, int n) {
-        for (int i = 0; i < n; ++i) y[i] += a * x[i];
-    }
-    static double amax(const double *a, int n) {
-        double r = 0.0;
-        for (int i = 0; i < n; ++i) r = std::max(r, std::fabs(a[i]));
-        return r;
-    }
-    // the reference's fallback direction: re-evaluate at x (its own callback returns the same gradient again), d = -g / |g| * |d_prev|
-    void steepest_with_old_norm(const double *x, int n, lbfgs_eval_fn eval, void *inst, int &evals, double olddnorm) {
-        gp_scratch.assign(n, 0.0);
-        (void)eval(inst, x, gp_scratch.data(), n);
-        ++evals;
-        g = gp_scratch;
-        for (int i = 0; i < n; ++i) d[i] = -g[i];
-        const double z = dotp(d.data(), d.data(), n);
-        if (z > 0) {
-            const double nn = std::sqrt(z);
-            for (int i = 0; i < n; ++i) d[i] /= nn;
-        }
-        for (int i = 0; i < n; ++i) d[i] *= olddnorm;
-    }
-    // Lewis–Overton: Armijo + weak Wolfe by bisection / doubling.
-    int line_search(double *x, int n, double &f, double &stp, double stpmin, double stpmax, lbfgs_eval_fn eval,
-                    void *inst, int &evals) {
-        if (!(stp > 0.0)) return LBFGSERR_INVALIDPARAMETERS;
-        const double dginit = dotp(gp.data(), d.data(), n);
-        if (0.0 < dginit) return LBFGSERR_INCREASEGRADIENT;
-        const double finit = f, dgtest = P.f_dec_coeff * dginit, dstest = P.s_curv_coeff * dginit;
-        double lo = 0.0, hi = stpmax;
-        bool bracketed = false, touched = false;
-        for (int count = 1;; ++count) {
-            for (int i = 0; i < n; ++i) x[i] = xp[i] + stp * d[i];
-            f = eval(inst, x, g.data(), n);
-            ++evals;
-            if (std::isinf(f) || std::isnan(f)) return LBFGSERR_INVALID_FUNCVAL;
-            if (f > finit + stp * dgtest) {
-                hi = stp;
-                bracketed = true;
-            } else if (!P.reference_patch && dotp(g.data(), d.data(), n) < dstest) {
-                lo = stp;
-            } else {
-                return count;
-            }
-            if (P.max_linesearch <= count) return LBFGSERR_MAXIMUMLINESEARCH;
-            if (bracketed && (hi - lo) < P.machine_prec * hi) return LBFGSERR_WIDTHTOOSMALL;
-            stp = bracketed ? 0.5 * (lo + hi) : stp * 2.0;
-            if (stp < stpmin) return LBFGSERR_MINIMUMSTEP;
-            if (stp > stpmax) {
-                if (touched) return LBFGSERR_MAXIMUMSTEP;
-                touched = true;
-                stp = stpmax;
-            }
-        }
-    }
-
     LbfgsParams P;
-    std::vector<double> xp, g, gp, d, pf, S, Y, ys_hist, alpha, gp_scratch;
-
+    std::vector<double> store;
 };
 
 }  // namespace host

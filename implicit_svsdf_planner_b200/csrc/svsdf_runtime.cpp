@@ -33,6 +33,7 @@
 #include "host/lbfgs.hpp"
 #include "host/minco.hpp"
 #include "host/rendezvous.hpp"
+#include "svsdf_backend.h"
 #include "svsdf_launch.h"
 #include "svsdf_types.h"
 
@@ -44,7 +45,7 @@ using namespace svsdf;
 struct HostEval {
     host::MincoS3NU minco;
     int N = 0;
-    std::vector<double> times, gradByTimes, partialGradByTimes, partialGradByCoeffs, gradByPoints;
+    std::vector<double> times, gradByTimes, partialGradByTimes, partialGradByCoeffs, gradByPoints, adj;
     double energy = 0.0;
 
     void setup(const double *initS, const double *finalS, int n_pieces) {
@@ -55,33 +56,16 @@ struct HostEval {
         partialGradByTimes.assign(N, 0.0);
         partialGradByCoeffs.assign((size_t)18 * N, 0.0);
         gradByPoints.assign((size_t)3 * (N - 1), 0.0);
+        adj.assign((size_t)18 * N, 0.0);
     }
-    // forwardT / forwardP (back_end_optimizer.hpp:353-354)
-    void forward(const double *x) {
-        for (int i = 0; i < N; ++i) times[i] = host::forwardT(x[i]);
-        minco.setParameters(x + N, times.data());
-        energy = minco.getEnergy();
-        minco.getEnergyPartialGradByCoeffs(partialGradByCoeffs.data());
-        minco.getEnergyPartialGradByTimes(partialGradByTimes.data());
+    host::BackendEvalView view() {
+        return host::BackendEvalView{minco.view(),           times.data(),        gradByTimes.data(), partialGradByTimes.data(),
+                                     partialGradByCoeffs.data(), gradByPoints.data(), adj.data()};
     }
+    void forward(const double *x) { energy = host::backend_forward(view(), x); }
     // o: the device record [cost, gradC (18N), gradT (N), n_inside] of the trajectory forward() built
     double backward(const double *o, const double *x, double rho, double *g, double *pos_out, double *other_out) {
-        double cost = energy;
-        const double energy_cost = cost;
-        cost += o[0];
-        for (int e = 0; e < 18 * N; ++e) partialGradByCoeffs[e] += o[1 + e];
-        for (int i = 0; i < N; ++i) partialGradByTimes[i] += o[1 + 18 * N + i];
-        const double pos_cost = cost - energy_cost;
-        minco.propogateGrad(partialGradByCoeffs.data(), partialGradByTimes.data(), gradByPoints.data(), gradByTimes.data());
-        double tsum = 0.0;
-        for (int i = 0; i < N; ++i) tsum += times[i];
-        cost += rho * tsum;
-        for (int i = 0; i < N; ++i) gradByTimes[i] += rho;
-        *pos_out = pos_cost;
-        *other_out = cost - pos_cost;
-        for (int i = 0; i < N; ++i) g[i] = host::backwardGradT(x[i], gradByTimes[i]);
-        for (int i = 0; i < 3 * (N - 1); ++i) g[N + i] = gradByPoints[i];
-        return cost;
+        return host::backend_backward(view(), energy, o, x, rho, g, pos_out, other_out);
     }
     // The final trajectory from the solver's returned iterate x (optimize_traj_lmbm does the same on success and failure,
     // back_end_optimizer.cpp:44-94) and the run's statistics.
@@ -271,7 +255,17 @@ struct svsdf_ctx {
     PinnedBuffer<double> h_multi_out;
     DeviceBuffer<unsigned int> d_multi_tickets;  // [0] k_compact_multi's, [1 + k] problem k's k_finalize_multi ticket; zero between calls
     int64_t multi_last_inside = -1;  // inside points of the previous multi evaluation (picks the k_gsip_multi variant)
-    int64_t lockstep_rounds = 0;  // rounds of the last svsdf_optimize_lockstep
+    int64_t lockstep_rounds = 0;  // rounds of the last svsdf_optimize_lockstep / svsdf_optimize_device
+    double round_eval_ms = 0.0, round_backend_ms = 0.0;  // their device time: evaluation kernels, back-end kernels (svsdf_round_times)
+    // svsdf_optimize_device: slots (machine state, storage, status), the call's problems, results and resident points, the round's blobs
+    DeviceBuffer<BackendSlot> d_be_slots;
+    DeviceBuffer<double> d_be_mem, d_be_res, d_be_pts, d_be_blobs;
+    DeviceBuffer<BackendStatus> d_be_status;
+    PinnedBuffer<BackendStatus> h_be_status;
+    DeviceBuffer<BackendProblem> d_be_prob;
+    DeviceBuffer<BackendResult> d_be_result;
+    DeviceBuffer<unsigned char> d_be_round;
+    PinnedBuffer<unsigned char> h_be_round;
     // svsdf_swept_contour: device buffers (per corner, per needed corner, per CTA, outputs) and the samples' upload
     DeviceBuffer<unsigned char> d_sw_corner, d_sw_point, d_sw_small, d_sw_out;
     // svsdf_map_clearance: device buffers (header, samples and per-CTA counts; band bits per map word; band cells)
@@ -721,102 +715,82 @@ struct PointQuery {
     double *sdf, *tstar;
 };
 
-// One cost + gradient evaluation of every item with rc == SVSDF_OK, in one set of launches.  Items whose trajectory or points are
-// invalid get rc = SVSDF_ERR_INVALID and take no part; a CUDA error fails the call (and every item).  *ms: device time of the launches.
-// With pq: the per-point query of every item instead (no reduction, no finalize, nothing downloaded; multi_last_inside is kept).
-int run_multi(svsdf_ctx *ctx, MultiItem *items, int n, float *ms, const PointQuery *pq = nullptr) {
-    if (ms) *ms = 0.0f;
-    CK(cudaSetDevice(ctx->device));
+// The planning and launch sequence of one multi evaluation, shared by run_multi and svsdf_optimize_device.  The caller fills each
+// problem's blob_off, pt_off, P, blob_doubles, N and K1; plan_multi gives it the virtual grid and schedule of its single call (occupancy /
+// outer_plan: what gives it the single call's bits), the CTA maps and the scratch offsets.
+struct MultiPlan {
     std::vector<MultiProblem> pr;
-    std::vector<int> who, map_s, map_b;
-    std::vector<BlobLayout> lay;
-    std::vector<double> dur;
-    int64_t blob_tot = 0, pt_tot = 0, flag_tot = 0, part_tot = 0, out_tot = 0;
+    std::vector<int> map_s, map_b;
+    int64_t flag_tot = 0, part_tot = 0, out_tot = 0;
+    int64_t pt_round = 0;  // points of the round's problems (inside contributions)
+    int64_t pt_span = 0;   // points the pt_off values span (inside t* and lists are indexed by pt_off)
     int max_K1 = 1, max_N = 1, max_blob = 2;
     int smax_blob[2] = {0, 0}, smax_N[2] = {1, 1};  // per k_outer_multi launch (sparse, batched): the shared memory is sized by its largest
-    for (int k = 0; k < n; ++k) {
-        MultiItem &it = items[k];
-        if (it.rc != SVSDF_OK) continue;
-        BlobLayout L;
-        double D = 0.0;
-        const char *msg = nullptr;
-        if (it.P < 0 || it.P > 2000000000LL || (!pq && (it.stride < 2 || (it.P > 0 && !it.pts) || !it.out)) ||
-            traj_layout(it.N, it.T, it.coeffs, L, D, &msg) != SVSDF_OK) {
-            it.rc = SVSDF_ERR_INVALID;
-            continue;
-        }
-        // problem k's virtual grid is the grid svsdf_cost_grad would launch for it
+    size_t o_ms = 0, o_mb = 0, head_bytes = 0;        // packed head: problem table | CTA maps (sparse, batched)
+};
+
+int plan_multi(svsdf_ctx *ctx, MultiPlan &pl) {
+    for (size_t j = 0; j < pl.pr.size(); ++j) {
+        MultiProblem &m = pl.pr[j];
         Occupancy occ;
-        int rc = occupancy(ctx, it.N, L.total, &occ);
+        int rc = occupancy(ctx, m.N, m.blob_doubles, &occ);
         if (rc) return rc;
-        const OuterPlan plan = outer_plan(ctx, it.P, occ);
+        const OuterPlan plan = outer_plan(ctx, m.P, occ);
         const int G = plan.grid, batched = plan.batched;
-        MultiProblem m;
-        m.blob_off = blob_tot; m.pt_off = pt_tot; m.flag_off = flag_tot; m.part_off = part_tot; m.out_off = out_tot;
-        m.P = it.P; m.blob_doubles = L.total; m.N = it.N; m.K1 = L.K1; m.grid = G;
-        std::vector<int> &mp = batched ? map_b : map_s;
-        for (int v = 0; v < G; ++v) { mp.push_back((int)pr.size()); mp.push_back(v); }
-        pr.push_back(m);
-        who.push_back(k);
-        lay.push_back(L);
-        dur.push_back(D);
-        blob_tot += L.total;
-        pt_tot += it.P;
-        flag_tot += (it.P + 15) & ~(int64_t)15;
-        part_tot += (int64_t)G * (19 * it.N + 1);
-        out_tot += 19 * it.N + 2;
-        max_K1 = std::max(max_K1, L.K1);
-        max_N = std::max(max_N, it.N);
-        max_blob = std::max(max_blob, L.total);
-        smax_blob[batched] = std::max(smax_blob[batched], L.total);
-        smax_N[batched] = std::max(smax_N[batched], it.N);
+        m.flag_off = pl.flag_tot; m.part_off = pl.part_tot; m.out_off = pl.out_tot; m.grid = G;
+        std::vector<int> &mp = batched ? pl.map_b : pl.map_s;
+        for (int v = 0; v < G; ++v) { mp.push_back((int)j); mp.push_back(v); }
+        pl.pt_round += m.P;
+        pl.pt_span = std::max(pl.pt_span, m.pt_off + m.P);
+        pl.flag_tot += (m.P + 15) & ~(int64_t)15;
+        pl.part_tot += (int64_t)G * (19 * m.N + 1);
+        pl.out_tot += 19 * m.N + 2;
+        pl.max_K1 = std::max(pl.max_K1, m.K1);
+        pl.max_N = std::max(pl.max_N, m.N);
+        pl.max_blob = std::max(pl.max_blob, m.blob_doubles);
+        pl.smax_blob[batched] = std::max(pl.smax_blob[batched], m.blob_doubles);
+        pl.smax_N[batched] = std::max(pl.smax_N[batched], m.N);
     }
-    const int m = (int)pr.size();
-    if (m == 0) return SVSDF_OK;
     for (int b = 0; b < 2; ++b)
-        if (outer_smem_doubles(smax_blob[b], smax_N[b]) * sizeof(double) > 200 * 1024) {
+        if (outer_smem_doubles(pl.smax_blob[b], pl.smax_N[b]) * sizeof(double) > 200 * 1024) {
             ctx->err = "svsdf: trajectory blob does not fit in shared memory";
             return SVSDF_ERR_INVALID;
         }
-    // packed inputs: problem table | CTA maps (sparse, batched) | blobs | points (x, y; not with pq)
-    const size_t o_prob = 0, o_ms = align16(o_prob + m * sizeof(MultiProblem)), o_mb = align16(o_ms + map_s.size() * sizeof(int)),
-                 o_blob = align16(o_mb + map_b.size() * sizeof(int)), o_pts = align16(o_blob + (size_t)blob_tot * 8),
-                 in_bytes = align16(o_pts + (pq ? 0 : (size_t)pt_tot * 16));
-    CK(ctx->h_multi_in.reserve(in_bytes));
-    CK(ctx->d_multi_in.reserve(in_bytes));
-    // the previous call's copy has completed (every call ends with a stream synchronise)
-    unsigned char *h = ctx->h_multi_in, *d = ctx->d_multi_in;
-    std::memcpy(h + o_prob, pr.data(), m * sizeof(MultiProblem));
-    if (!map_s.empty()) std::memcpy(h + o_ms, map_s.data(), map_s.size() * sizeof(int));
-    if (!map_b.empty()) std::memcpy(h + o_mb, map_b.data(), map_b.size() * sizeof(int));
-    for (int j = 0; j < m; ++j) {
-        const MultiItem &it = items[who[j]];
-        fill_blob(reinterpret_cast<double *>(h + o_blob) + pr[j].blob_off, lay[j], it.T, it.coeffs, dur[j]);
-        if (pq) continue;
-        double *xy = reinterpret_cast<double *>(h + o_pts) + 2 * pr[j].pt_off;
-        if (it.stride == 2) {
-            if (it.P) std::memcpy(xy, it.pts, (size_t)it.P * 16);
-        } else {
-            for (int64_t i = 0; i < it.P; ++i) { xy[2 * i] = it.pts[i * it.stride]; xy[2 * i + 1] = it.pts[i * it.stride + 1]; }
-        }
-    }
+    pl.o_ms = align16(pl.pr.size() * sizeof(MultiProblem));
+    pl.o_mb = align16(pl.o_ms + pl.map_s.size() * sizeof(int));
+    pl.head_bytes = align16(pl.o_mb + pl.map_b.size() * sizeof(int));
+    return SVSDF_OK;
+}
+
+void pack_plan(const MultiPlan &pl, unsigned char *h) {
+    std::memcpy(h, pl.pr.data(), pl.pr.size() * sizeof(MultiProblem));
+    if (!pl.map_s.empty()) std::memcpy(h + pl.o_ms, pl.map_s.data(), pl.map_s.size() * sizeof(int));
+    if (!pl.map_b.empty()) std::memcpy(h + pl.o_mb, pl.map_b.data(), pl.map_b.size() * sizeof(int));
+}
+
+// The launches of a planned evaluation whose packed head is at d (device) and blobs at d_blobs: k_pose_table_multi, k_outer_multi per
+// schedule that occurs, k_compact_multi, k_gsip_multi and (not with pq) k_finalize_multi.  *records: the per-problem records [cost,
+// gradC (18N), gradT (N), n_inside] at out_off (device).
+int launch_plan(svsdf_ctx *ctx, const MultiPlan &pl, const unsigned char *d, double *d_blobs, const double *d_points, const PointQuery *pq,
+                double **records) {
+    const int m = (int)pl.pr.size();
+    const int64_t pt_span = pl.pt_span, pt_round = pl.pt_round;
     // scratch: flags | inside t* | inside lists | contributions | pieces | partials | out | tot | counts | slot offsets
-    const size_t s_flag = 0, s_ts = align16(s_flag + (size_t)flag_tot + 16), s_list = align16(s_ts + (size_t)pt_tot * 8),
-                 s_con = align16(s_list + (size_t)pt_tot * 4), s_pc = align16(s_con + (size_t)pt_tot * 160),
-                 s_part = align16(s_pc + (size_t)pt_tot * 4), s_out = align16(s_part + (size_t)part_tot * 8),
-                 s_tot = align16(s_out + (size_t)out_tot * 8), s_cnt = align16(s_tot + (size_t)out_tot * 8), s_off = align16(s_cnt + (size_t)m * 4),
+    const size_t s_flag = 0, s_ts = align16(s_flag + (size_t)pl.flag_tot + 16), s_list = align16(s_ts + (size_t)pt_span * 8),
+                 s_con = align16(s_list + (size_t)pt_span * 4), s_pc = align16(s_con + (size_t)pt_round * 160),
+                 s_part = align16(s_pc + (size_t)pt_round * 4), s_out = align16(s_part + (size_t)pl.part_tot * 8),
+                 s_tot = align16(s_out + (size_t)pl.out_tot * 8), s_cnt = align16(s_tot + (size_t)pl.out_tot * 8), s_off = align16(s_cnt + (size_t)m * 4),
                  s_bytes = align16(s_off + (size_t)(m + 1) * 4);
     CK(ctx->d_multi_scratch.reserve(s_bytes));
     if ((size_t)m + 1 > ctx->d_multi_tickets.capacity()) {  // a new block: its tickets start at zero
         CK(ctx->d_multi_tickets.reserve(m + 1));
         CK(cudaMemsetAsync(ctx->d_multi_tickets, 0, ctx->d_multi_tickets.capacity() * sizeof(unsigned int), ctx->stream));
     }
-    CK(ctx->h_multi_out.reserve(out_tot));
     unsigned char *sc = ctx->d_multi_scratch;
     KernelArgs A;
     std::memset(&A, 0, sizeof(A));
-    A.blob = reinterpret_cast<const double *>(d + o_blob);
-    A.points_xy = pq ? pq->pts : reinterpret_cast<const double *>(d + o_pts);
+    A.blob = d_blobs;
+    A.points_xy = d_points;
     A.cp = ctx->cp;
     A.partials = reinterpret_cast<double *>(sc + s_part);
     A.want_reduce = pq ? 0 : 1;
@@ -831,7 +805,7 @@ int run_multi(svsdf_ctx *ctx, MultiItem *items, int n, float *ms, const PointQue
     MultiArgs M;
     std::memset(&M, 0, sizeof(M));
     M.n = m;
-    M.prob = reinterpret_cast<const MultiProblem *>(d + o_prob);
+    M.prob = reinterpret_cast<const MultiProblem *>(d);
     M.ins_count = reinterpret_cast<int *>(sc + s_cnt);
     M.ins_off = reinterpret_cast<int *>(sc + s_off);
     M.compact_ticket = ctx->d_multi_tickets;
@@ -840,38 +814,102 @@ int run_multi(svsdf_ctx *ctx, MultiItem *items, int n, float *ms, const PointQue
     M.tot = reinterpret_cast<double *>(sc + s_tot);
     const ScaleSched *Z = ctx->scaled ? &ctx->sched : nullptr;
     const Kernels &K = kernels(ctx);
-    CK(cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, ctx->stream));
-    if (ms) CK(cudaEventRecord(ctx->ev0, ctx->stream));
-    CK(K.pose_multi(reinterpret_cast<double *>(d + o_blob), M, max_K1, ctx->stream));
+    CK(K.pose_multi(d_blobs, M, pl.max_K1, ctx->stream));
     int launches = 1;
     for (int b = 0; b < 2; ++b) {
-        const std::vector<int> &mp = b ? map_b : map_s;
+        const std::vector<int> &mp = b ? pl.map_b : pl.map_s;
         if (mp.empty()) continue;
-        M.cta_map = reinterpret_cast<const int *>(d + (b ? o_mb : o_ms));
-        CK(K.multi(b, A, M, ctx->shape, Z, (int)(mp.size() / 2), outer_smem_doubles(smax_blob[b], smax_N[b]) * sizeof(double), 0,
+        M.cta_map = reinterpret_cast<const int *>(d + (b ? pl.o_mb : pl.o_ms));
+        CK(K.multi(b, A, M, ctx->shape, Z, (int)(mp.size() / 2), outer_smem_doubles(pl.smax_blob[b], pl.smax_N[b]) * sizeof(double), 0,
                    ctx->sm_count, ctx->stream));
         ++launches;
     }
     M.cta_map = nullptr;
     CK(K.compact_multi(A.inside_flag, A.inside_list, M, ctx->stream));
     const GsipPlan gp = gsip_plan(ctx, pq ? -1 : ctx->multi_last_inside);  // the variant svsdf_query would pick
-    CK(K.multi(2, A, M, ctx->shape, Z, gp.grid, (size_t)max_blob * sizeof(double), gp.wide, ctx->sm_count, ctx->stream));
+    CK(K.multi(2, A, M, ctx->shape, Z, gp.grid, (size_t)pl.max_blob * sizeof(double), gp.wide, ctx->sm_count, ctx->stream));
     launches += 2;
-    if (pq) {
-        ctx->launches += launches;
-        return SVSDF_OK;
+    if (!pq) {
+        CK(K.finalize_multi(A.partials, A.gsip_contrib, A.gsip_piece, M, pl.max_N, ctx->stream));
+        launches += 1;
     }
-    CK(K.finalize_multi(A.partials, A.gsip_contrib, A.gsip_piece, M, max_N, ctx->stream));
-    launches += 1;
-    if (ms) CK(cudaEventRecord(ctx->ev1, ctx->stream));
-    CK(cudaMemcpyAsync(ctx->h_multi_out, M.out, (size_t)out_tot * 8, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
     ctx->launches += launches;
+    if (records) *records = M.out;
+    return SVSDF_OK;
+}
+
+// One cost + gradient evaluation of every item with rc == SVSDF_OK, in one set of launches.  Items whose trajectory or points are
+// invalid get rc = SVSDF_ERR_INVALID and take no part; a CUDA error fails the call (and every item).  *ms: device time of the launches.
+// With pq: the per-point query of every item instead (no reduction, no finalize, nothing downloaded; multi_last_inside is kept).
+int run_multi(svsdf_ctx *ctx, MultiItem *items, int n, float *ms, const PointQuery *pq = nullptr) {
+    if (ms) *ms = 0.0f;
+    CK(cudaSetDevice(ctx->device));
+    MultiPlan pl;
+    std::vector<int> who;
+    std::vector<BlobLayout> lay;
+    std::vector<double> dur;
+    int64_t blob_tot = 0, pt_tot = 0;
+    for (int k = 0; k < n; ++k) {
+        MultiItem &it = items[k];
+        if (it.rc != SVSDF_OK) continue;
+        BlobLayout L;
+        double D = 0.0;
+        const char *msg = nullptr;
+        if (it.P < 0 || it.P > 2000000000LL || (!pq && (it.stride < 2 || (it.P > 0 && !it.pts) || !it.out)) ||
+            traj_layout(it.N, it.T, it.coeffs, L, D, &msg) != SVSDF_OK) {
+            it.rc = SVSDF_ERR_INVALID;
+            continue;
+        }
+        MultiProblem m;
+        std::memset(&m, 0, sizeof(m));
+        m.blob_off = blob_tot; m.pt_off = pt_tot;
+        m.P = it.P; m.blob_doubles = L.total; m.N = it.N; m.K1 = L.K1;
+        pl.pr.push_back(m);
+        who.push_back(k);
+        lay.push_back(L);
+        dur.push_back(D);
+        blob_tot += L.total;
+        pt_tot += it.P;
+    }
+    const int m = (int)pl.pr.size();
+    if (m == 0) return SVSDF_OK;
+    int rc = plan_multi(ctx, pl);
+    if (rc) return rc;
+    // packed inputs: problem table | CTA maps (sparse, batched) | blobs | points (x, y; not with pq)
+    const size_t o_blob = pl.head_bytes, o_pts = align16(o_blob + (size_t)blob_tot * 8),
+                 in_bytes = align16(o_pts + (pq ? 0 : (size_t)pt_tot * 16));
+    CK(ctx->h_multi_in.reserve(in_bytes));
+    CK(ctx->d_multi_in.reserve(in_bytes));
+    // the previous call's copy has completed (every call ends with a stream synchronise)
+    unsigned char *h = ctx->h_multi_in, *d = ctx->d_multi_in;
+    pack_plan(pl, h);
+    for (int j = 0; j < m; ++j) {
+        const MultiItem &it = items[who[j]];
+        fill_blob(reinterpret_cast<double *>(h + o_blob) + pl.pr[j].blob_off, lay[j], it.T, it.coeffs, dur[j]);
+        if (pq) continue;
+        double *xy = reinterpret_cast<double *>(h + o_pts) + 2 * pl.pr[j].pt_off;
+        if (it.stride == 2) {
+            if (it.P) std::memcpy(xy, it.pts, (size_t)it.P * 16);
+        } else {
+            for (int64_t i = 0; i < it.P; ++i) { xy[2 * i] = it.pts[i * it.stride]; xy[2 * i + 1] = it.pts[i * it.stride + 1]; }
+        }
+    }
+    CK(ctx->h_multi_out.reserve(pl.out_tot));
+    CK(cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, ctx->stream));
+    if (ms) CK(cudaEventRecord(ctx->ev0, ctx->stream));
+    double *records = nullptr;
+    rc = launch_plan(ctx, pl, d, reinterpret_cast<double *>(d + o_blob), pq ? pq->pts : reinterpret_cast<const double *>(d + o_pts), pq,
+                     &records);
+    if (rc) return rc;
+    if (pq) return SVSDF_OK;
+    if (ms) CK(cudaEventRecord(ctx->ev1, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->h_multi_out, records, (size_t)pl.out_tot * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
     if (ms) CK(cudaEventElapsedTime(ms, ctx->ev0, ctx->ev1));
     int64_t inside = 0;
     for (int j = 0; j < m; ++j) {
-        const int nout = 19 * pr[j].N + 2;
-        const double *o = ctx->h_multi_out + pr[j].out_off;
+        const int nout = 19 * pl.pr[j].N + 2;
+        const double *o = ctx->h_multi_out + pl.pr[j].out_off;
         std::memcpy(items[who[j]].out, o, (size_t)nout * sizeof(double));
         inside += (int64_t)o[nout - 1];
     }
@@ -2572,6 +2610,7 @@ int svsdf_optimize_lockstep(svsdf_ctx *ctx, const svsdf_lockstep_problem *proble
         }
     }
     ctx->lockstep_rounds = 0;
+    ctx->round_eval_ms = ctx->round_backend_ms = 0.0;
     if (n == 0) return SVSDF_OK;
     CK(cudaSetDevice(ctx->device));
     const host::LbfgsParams hp = to_host_params(params);
@@ -2590,6 +2629,7 @@ int svsdf_optimize_lockstep(svsdf_ctx *ctx, const svsdf_lockstep_problem *proble
         for (int s : ready) items.push_back(slots[s].item);
         float ms = 0.0f;
         int rc = run_multi(ctx, items.data(), (int)items.size(), ctx->time_kernels ? &ms : nullptr);
+        ctx->round_eval_ms += ms;
         for (size_t j = 0; j < ready.size(); ++j) {
             LockstepSlot &s = slots[ready[j]];
             s.item.rc = rc != SVSDF_OK ? rc : items[j].rc;
@@ -2655,6 +2695,310 @@ int svsdf_optimize_lockstep(svsdf_ctx *ctx, const svsdf_lockstep_problem *proble
     ctx->time_kernels = false;
     ctx->lockstep_rounds = rv.rounds();
     if (round_err != SVSDF_OK) return round_err;
+    return SVSDF_OK;
+}
+
+int svsdf_optimize_device(svsdf_ctx *ctx, const svsdf_lockstep_problem *problems, int n, const svsdf_lbfgs_params *params, int max_in_flight,
+                          svsdf_opt_stats *stats_out, int *status_out, int64_t *rounds_out) {
+    if (!ctx) return SVSDF_ERR_INVALID;
+    if (ctx->lmbm) {
+        ctx->err = "svsdf_optimize_device: runs the built-in L-BFGS only; this context has an LMBM library set";
+        return SVSDF_ERR_INVALID;
+    }
+    if (n < 0 || (n > 0 && !problems)) {
+        ctx->err = "svsdf_optimize_device: needs n >= 0 and the problem array";
+        return SVSDF_ERR_INVALID;
+    }
+    if (max_in_flight > kMaxMultiProblems) {
+        ctx->err = "svsdf_optimize_device: max_in_flight above 65535";
+        return SVSDF_ERR_INVALID;
+    }
+    int Nmax = 2;
+    for (int k = 0; k < n; ++k) {  // svsdf_optimize_lockstep's checks
+        const svsdf_lockstep_problem &p = problems[k];
+        if (!p.initS || !p.finalS || !p.opt_x || p.N < 2 || p.N > kMaxPieces || p.P < 0 || p.P > 2000000000LL || p.stride < 2 ||
+            (p.P > 0 && !p.points)) {
+            ctx->err = std::string("svsdf_optimize_device: problem ") + std::to_string(k) +
+                       ": needs initS, finalS, opt_x, 2 <= N <= 64, P >= 0, stride >= 2 and points when P > 0";
+            return SVSDF_ERR_INVALID;
+        }
+        Nmax = std::max(Nmax, p.N);
+    }
+    ctx->lockstep_rounds = 0;
+    ctx->round_eval_ms = ctx->round_backend_ms = 0.0;
+    if (rounds_out) *rounds_out = 0;
+    if (n == 0) return SVSDF_OK;
+    CK(cudaSetDevice(ctx->device));
+    const auto t0 = std::chrono::steady_clock::now();
+    const host::LbfgsParams hp = to_host_params(params);
+    if (const int bad = host::lbfgs_check(hp, 1)) {
+        // parameters the solver refuses: every problem ends at once with the check's code, as svsdf_optimize ends (no evaluation; T
+        // and the coefficients of the start point), and nothing is sized or launched
+        for (int k = 0; k < n; ++k) {
+            const svsdf_lockstep_problem &p = problems[k];
+            HostEval he;
+            he.setup(p.initS, p.finalS, p.N);
+            host::LbfgsResult R;
+            R.status = bad;
+            he.finish(p.opt_x, R, 0.0, 0.0, p.T_out, p.coeffs_out, stats_out ? &stats_out[k] : nullptr);
+            if (status_out) status_out[k] = bad;
+        }
+        return SVSDF_OK;
+    }
+    const int M = std::min(n, max_in_flight > 0 ? max_in_flight : 1024);
+    const int64_t slot_doubles = backend_slot_doubles(hp, Nmax);
+    // the call's problems, their result block (x0 in, then x, T, coeffs) and their resident points
+    std::vector<BackendProblem> bp(n);
+    std::vector<int64_t> pt_off(n);
+    int64_t res_tot = 0, pts_tot = 0;
+    for (int k = 0; k < n; ++k) {
+        const svsdf_lockstep_problem &p = problems[k];
+        std::memset(&bp[k], 0, sizeof(BackendProblem));
+        bp[k].N = p.N;
+        bp[k].res_off = res_tot;
+        std::memcpy(bp[k].initS, p.initS, sizeof(bp[k].initS));
+        std::memcpy(bp[k].finalS, p.finalS, sizeof(bp[k].finalS));
+        res_tot += (4 * p.N - 3) + 19 * p.N;
+        pt_off[k] = pts_tot;
+        pts_tot += p.P;
+    }
+    if (pts_tot > INT32_MAX) {  // the resident points of the call share one index space (the multi kernels' int point index)
+        ctx->err = "svsdf_optimize_device: more than 2^31 - 1 query points in one call";
+        return SVSDF_ERR_INVALID;
+    }
+    CK(ctx->d_be_slots.reserve(M));
+    CK(ctx->d_be_mem.reserve((size_t)M * slot_doubles));
+    CK(ctx->d_be_status.reserve(M));
+    CK(ctx->h_be_status.reserve(M));
+    CK(ctx->d_be_prob.reserve(n));
+    CK(ctx->d_be_result.reserve(n));
+    CK(ctx->d_be_res.reserve(res_tot));
+    CK(ctx->d_be_pts.reserve((size_t)2 * pts_tot));
+    {
+        std::vector<double> res(res_tot, 0.0);
+        for (int k = 0; k < n; ++k) std::memcpy(res.data() + bp[k].res_off, problems[k].opt_x, sizeof(double) * (4 * bp[k].N - 3));
+        CK(cudaMemcpyAsync(ctx->d_be_prob, bp.data(), n * sizeof(BackendProblem), cudaMemcpyHostToDevice, ctx->stream));
+        CK(cudaMemcpyAsync(ctx->d_be_res, res.data(), res_tot * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    }
+    BackendArgs B;
+    std::memset(&B, 0, sizeof(B));
+    B.P = hp;
+    B.rho = ctx->rho;
+    B.Nmax = Nmax;
+    B.slot_doubles = slot_doubles;
+    B.slots = ctx->d_be_slots;
+    B.mem = ctx->d_be_mem;
+    B.status = ctx->d_be_status;
+    B.prob = ctx->d_be_prob;
+    B.result = ctx->d_be_result;
+    B.res = ctx->d_be_res;
+    std::vector<int> in_slot(M, -1), round_probs, entered;
+    std::vector<double> seconds(n, 0.0), gpu_ms(n, 0.0);
+    std::vector<char> finished(n, 0);
+    std::vector<int64_t> round_valid_slots;
+    int next = 0, round_err = SVSDF_OK;
+    int64_t rounds = 0;
+    bool timed = false, timed_init = false;
+    // a CUDA error ends the call with that error in status_out of every problem not finished; the other outputs are then not written
+    auto fail = [&](int rc) {
+        if (status_out)
+            for (int k = 0; k < n; ++k)
+                if (!finished[k]) status_out[k] = rc;
+        ctx->lockstep_rounds = rounds;
+        if (rounds_out) *rounds_out = rounds;
+        return rc;
+    };
+#define CKB(call)                                                                       \
+    do {                                                                                \
+        cudaError_t e__ = (call);                                                       \
+        if (e__ != cudaSuccess) {                                                       \
+            ctx->err = std::string(#call) + ": " + cudaGetErrorString(e__);             \
+            return fail(SVSDF_ERR_CUDA);                                                \
+        }                                                                               \
+    } while (0)
+    // the round stage: [problems entering slots (pairs) | round items | problem table and CTA maps], each region rewritten only after
+    // the stream synchronise that follows its last copy
+    const size_t o_items = align16((size_t)2 * M * sizeof(int)), o_head0 = align16(o_items + (size_t)M * sizeof(BackendRoundItem));
+    CKB(ctx->h_be_round.reserve(o_head0));
+    CKB(ctx->d_be_round.reserve(o_head0));
+    for (;;) {
+        // problems enter the free slots: their points go up once, the machine starts and asks for its first evaluation
+        int entering = 0;
+        entered.clear();
+        int *enter = reinterpret_cast<int *>(ctx->h_be_round.get());
+        for (int s = 0; s < M && next < n; ++s) {
+            if (in_slot[s] >= 0) continue;
+            const svsdf_lockstep_problem &p = problems[next];
+            if (p.P > 0) {
+                double *dst = ctx->d_be_pts + 2 * pt_off[next];
+                if (p.stride == 2) {
+                    CKB(cudaMemcpyAsync(dst, p.points, (size_t)p.P * 16, cudaMemcpyHostToDevice, ctx->stream));
+                } else {
+                    std::vector<double> xy((size_t)2 * p.P);
+                    for (int64_t i = 0; i < p.P; ++i) { xy[2 * i] = p.points[i * p.stride]; xy[2 * i + 1] = p.points[i * p.stride + 1]; }
+                    CKB(cudaMemcpyAsync(dst, xy.data(), (size_t)p.P * 16, cudaMemcpyHostToDevice, ctx->stream));
+                    CKB(cudaStreamSynchronize(ctx->stream));  // xy is about to go
+                }
+            }
+            in_slot[s] = next;
+            entered.push_back(next);
+            enter[2 * entering] = s;
+            enter[2 * entering + 1] = next;
+            ++entering;
+            ++next;
+        }
+        if (entering) {
+            int *d_enter = reinterpret_cast<int *>(ctx->d_be_round.get());
+            CKB(cudaMemcpyAsync(d_enter, enter, (size_t)2 * entering * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+            CKB(cudaEventRecord(ctx->evk[2], ctx->stream));
+            CKB(launch_backend_init(B, d_enter, entering, ctx->stream));
+            CKB(cudaEventRecord(ctx->evk[3], ctx->stream));
+            ctx->launches += 1;
+            timed_init = true;
+        }
+        // 1. one small download: every slot's status
+        CKB(cudaMemcpyAsync(ctx->h_be_status, ctx->d_be_status, (size_t)M * sizeof(BackendStatus), cudaMemcpyDeviceToHost, ctx->stream));
+        CKB(cudaStreamSynchronize(ctx->stream));
+        const BackendStatus *st = ctx->h_be_status;
+        const double now = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+        if (timed_init) {  // the entering problems' first forward half
+            float a = 0.0f;
+            CKB(cudaEventElapsedTime(&a, ctx->evk[2], ctx->evk[3]));
+            ctx->round_backend_ms += a;
+            for (int k : entered) gpu_ms[k] += a;
+            timed_init = false;
+        }
+        if (timed) {  // the previous round's device time
+            float a = 0.0f, b = 0.0f, c = 0.0f;
+            CKB(cudaEventElapsedTime(&a, ctx->ev0, ctx->evk[0]));
+            CKB(cudaEventElapsedTime(&b, ctx->evk[0], ctx->evk[1]));
+            CKB(cudaEventElapsedTime(&c, ctx->evk[1], ctx->ev1));
+            ctx->round_eval_ms += b;
+            ctx->round_backend_ms += a + c;
+            for (int k : round_probs) gpu_ms[k] += a + b + c;
+            int64_t inside = 0;
+            for (int64_t s : round_valid_slots) inside += st[s].n_inside;
+            if (!round_valid_slots.empty()) ctx->multi_last_inside = inside;
+            timed = false;
+        }
+        bool freed = false;
+        for (int s = 0; s < M; ++s)
+            if (in_slot[s] >= 0 && st[s].ask == host::LBFGS_DONE) {
+                seconds[in_slot[s]] = now;
+                finished[in_slot[s]] = 1;
+                in_slot[s] = -1;
+                freed = true;
+            }
+        if (freed && next < n) continue;
+        // 2. the round: every slot asking for an evaluation, planned as run_multi plans (each problem keeps its single call's grid)
+        MultiPlan pl;
+        std::vector<BackendRoundItem> items;
+        int64_t blob_tot = 0;
+        round_probs.clear();
+        round_valid_slots.clear();
+        for (int s = 0; s < M; ++s) {
+            if (in_slot[s] < 0 || st[s].ask != host::LBFGS_EVAL) continue;
+            const int k = in_slot[s];
+            BackendRoundItem it;
+            it.slot = s;
+            it.rc = st[s].valid ? SVSDF_OK : SVSDF_ERR_INVALID;
+            it.out_off = 0;
+            it.blob_off = 0;
+            round_probs.push_back(k);
+            if (it.rc == SVSDF_OK) {
+                const BlobLayout L = blob_layout(st[s].N, st[s].K1);
+                MultiProblem m;
+                std::memset(&m, 0, sizeof(m));
+                m.blob_off = blob_tot;
+                m.pt_off = pt_off[k];
+                m.P = problems[k].P;
+                m.blob_doubles = L.total;
+                m.N = st[s].N;
+                m.K1 = L.K1;
+                it.blob_off = blob_tot;
+                blob_tot += L.total;
+                pl.pr.push_back(m);
+                round_valid_slots.push_back(s);
+            }
+            items.push_back(it);
+        }
+        const int count = (int)items.size();
+        if (count == 0) break;  // nothing in flight and nothing left
+        ++rounds;
+        int rc = pl.pr.empty() ? SVSDF_OK : plan_multi(ctx, pl);
+        if (rc == SVSDF_ERR_CUDA) return fail(rc);
+        if (rc != SVSDF_OK) {  // the round fails: its error goes to every problem in it
+            for (BackendRoundItem &it : items) it.rc = rc;
+            if (round_err == SVSDF_OK) round_err = rc;
+            pl = MultiPlan();
+            round_valid_slots.clear();
+        } else {
+            for (int j = 0, v = 0; j < count; ++j)
+                if (items[j].rc == SVSDF_OK) items[j].out_off = pl.pr[v++].out_off;
+        }
+        // 3. one small upload: the round items, the problem table and the CTA maps (the stage's earlier copies have completed)
+        const size_t bytes = o_head0 + pl.head_bytes;
+        CKB(ctx->h_be_round.reserve(bytes));
+        CKB(ctx->d_be_round.reserve(bytes));
+        std::memcpy(ctx->h_be_round + o_items, items.data(), (size_t)count * sizeof(BackendRoundItem));
+        if (!pl.pr.empty()) pack_plan(pl, ctx->h_be_round + o_head0);
+        CKB(cudaMemcpyAsync(ctx->d_be_round + o_items, ctx->h_be_round + o_items, o_head0 - o_items + pl.head_bytes, cudaMemcpyHostToDevice,
+                            ctx->stream));
+        const BackendRoundItem *d_items = reinterpret_cast<const BackendRoundItem *>(ctx->d_be_round + o_items);
+        // 4. the launches: blobs, the evaluation, the records into the machines
+        CKB(cudaEventRecord(ctx->ev0, ctx->stream));
+        if (!pl.pr.empty()) {
+            CKB(ctx->d_be_blobs.reserve(blob_tot));
+            CKB(launch_backend_blob(B, d_items, count, ctx->d_be_blobs, ctx->stream));
+            ctx->launches += 1;
+        }
+        CKB(cudaEventRecord(ctx->evk[0], ctx->stream));
+        double *records = nullptr;
+        if (!pl.pr.empty()) {
+            rc = launch_plan(ctx, pl, ctx->d_be_round + o_head0, ctx->d_be_blobs, ctx->d_be_pts, nullptr, &records);
+            if (rc) return fail(rc);
+        }
+        CKB(cudaEventRecord(ctx->evk[1], ctx->stream));
+        CKB(launch_backend_backward(B, d_items, count, records, ctx->stream));
+        ctx->launches += 1;
+        CKB(cudaEventRecord(ctx->ev1, ctx->stream));
+        timed = true;
+    }
+#undef CKB
+    // the results: one download
+    std::vector<BackendResult> R(n);
+    std::vector<double> res(res_tot);
+    CK(cudaMemcpyAsync(R.data(), ctx->d_be_result, n * sizeof(BackendResult), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(res.data(), ctx->d_be_res, res_tot * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    for (int k = 0; k < n; ++k) {
+        const svsdf_lockstep_problem &p = problems[k];
+        const int N = p.N, nv = 4 * N - 3;
+        const double *x = res.data() + bp[k].res_off;
+        std::memcpy(p.opt_x, x, sizeof(double) * nv);
+        if (p.T_out) std::memcpy(p.T_out, x + nv, sizeof(double) * N);
+        if (p.coeffs_out) std::memcpy(p.coeffs_out, x + nv + N, sizeof(double) * 18 * N);
+        if (p.f0_out && R[k].f0_set) *p.f0_out = R[k].f0;
+        if (stats_out) {
+            svsdf_opt_stats &o = stats_out[k];
+            o.final_cost = R[k].f;
+            o.iterations = R[k].iterations;
+            o.evaluations = R[k].evaluations;
+            o.status = R[k].solver_status;
+            o.seconds = seconds[k];
+            o.gpu_seconds = gpu_ms[k] * 1e-3;
+        }
+        if (status_out) status_out[k] = R[k].status;
+    }
+    ctx->lockstep_rounds = rounds;
+    if (rounds_out) *rounds_out = rounds;
+    return round_err;
+}
+
+int svsdf_round_times(const svsdf_ctx *ctx, double *eval_ms, double *backend_ms) {
+    if (!ctx) return SVSDF_ERR_INVALID;
+    if (eval_ms) *eval_ms = ctx->round_eval_ms;
+    if (backend_ms) *backend_ms = ctx->round_backend_ms;
     return SVSDF_OK;
 }
 

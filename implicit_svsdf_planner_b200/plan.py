@@ -194,6 +194,16 @@ _ASTAR_REASON = {0: "start or goal outside the map", 2: "front end found no path
                  4: "path longer than max_path", -1: "front end internal guard"}
 
 
+# Problems from which the back end runs on the device (svsdf_optimize_device) rather than on host threads (svsdf_optimize_lockstep); both
+# give the same bits.  Measured on an H100 (tests/tools/run_optimize_device.py, DESIGN §7): the device wins at 427 and 843 problems
+# (1.9x, 1.3x) and loses at 216 (0.88x); at 109 the two are within the run-to-run spread.
+DEVICE_BACK_END_MIN_PROBLEMS = 256
+
+
+def _back_end(ctx: "api.Context", n_problems: int):
+    return ctx.optimize_device if n_problems >= DEVICE_BACK_END_MIN_PROBLEMS else ctx.optimize_lockstep
+
+
 def plan_batch(ctx: "api.Context", cmap: CloudMap, starts, goals, kernel_size: int = scenes.YAML["kernel_size"], kernel_yaw_num: int = 18,
                front_end_safeh: float = 0.0, traj_parlength: float = 3.0, inittime: float = scenes.YAML["inittime"],
                mid_cfg: Optional["api.MidConfig"] = None, lbfgs_params=None, max_path: int = 4096, max_in_flight: int = 0,
@@ -201,7 +211,8 @@ def plan_batch(ctx: "api.Context", cmap: CloudMap, starts, goals, kernel_size: i
                repair: int = 0) -> list:
     """generate_traj for n start / goal pairs on one map: one device A* launch for all searches (svsdf_front_astar_device), per problem the
     waypoints, the query points (extract_points3d, on the context) and the warm start (mid_get_ori_traj, on a thread pool: the mid end is
-    host code and ctypes releases the GIL), then ONE lock-step back end (svsdf_optimize_lockstep) for every problem whose mid end succeeded.
+    host code and ctypes releases the GIL), then ONE lock-step back end for every problem whose mid end succeeded (svsdf_optimize_device
+    from DEVICE_BACK_END_MIN_PROBLEMS problems, else svsdf_optimize_lockstep: the same bits).
     Returns one dict per problem with generate_traj's keys (except astar_rounds) and its bits, plus the query points (`points`);
     a failed problem has ok=False and the reason (an exception of one problem's extraction or mid end fails that problem only).
     stats (optional dict) receives the wall seconds of each stage, the back end's rounds and its kernel launches.  back_end=False stops
@@ -275,7 +286,7 @@ def plan_batch(ctx: "api.Context", cmap: CloudMap, starts, goals, kernel_size: i
         back = []
     params = lbfgs_params or api.default_lbfgs_params(mem_size=16, past=3, delta=1e-6, g_epsilon=0.0, max_iterations=0, min_step=1e-32)
     launches0 = ctx.kernel_launches()
-    results, rounds = ctx.optimize_lockstep([dict(N=p["N"], init_s=p["init_s"], final_s=p["final_s"], x0=p["x0"], points=p["points"])
+    results, rounds = _back_end(ctx, len(back))([dict(N=p["N"], init_s=p["init_s"], final_s=p["final_s"], x0=p["x0"], points=p["points"])
                                              for p in back], params, max_in_flight)
     t4 = time.perf_counter()
     if stats is not None:
@@ -301,7 +312,7 @@ def plan_batch(ctx: "api.Context", cmap: CloudMap, starts, goals, kernel_size: i
                 todo = [(p, pts) for p, pts in todo if pts is not None]
                 if not todo:
                     break
-                results, _ = ctx.optimize_lockstep([dict(N=p["N"], init_s=p["init_s"], final_s=p["final_s"], x0=out[p["q"]]["x"], points=pts)
+                results, _ = _back_end(ctx, len(todo))([dict(N=p["N"], init_s=p["init_s"], final_s=p["final_s"], x0=out[p["q"]]["x"], points=pts)
                                                     for p, pts in todo], params, max_in_flight)
                 for (p, _), r in zip(todo, results):
                     out[p["q"]].update(ok=r["status"] >= 0, status=r["status"], final_cost=float(r["final_cost"]), iterations=int(r["iterations"]),

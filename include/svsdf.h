@@ -454,6 +454,25 @@ int svsdf_optimize_lockstep(svsdf_ctx *ctx, const svsdf_lockstep_problem *proble
                             svsdf_opt_stats *stats_out, int *status_out);
 int svsdf_lockstep_rounds(const svsdf_ctx *ctx, int64_t *rounds);
 
+/* svsdf_optimize_device: svsdf_optimize_lockstep with the back end on the device.  Every problem in flight keeps its L-BFGS state, its
+ * MINCO spline and its query points (uploaded once, when it enters a slot) in device memory; one warp per problem runs the host's own
+ * solver and MINCO code (host/lbfgs.hpp, host/minco.hpp) between the evaluations, so no host thread per problem is needed.  A round is
+ * one small download of every slot's state, the host's launch plan (each problem keeps the grid of its single call), one small upload
+ * and the launches; the launches per round do not depend on n.  Same problems, checks, refusals and results as svsdf_optimize_lockstep
+ * (bit for bit svsdf_optimize per problem: opt_x, T_out, coeffs_out, f0_out, stats and status_out), plus: max_in_flight above 65535 is
+ * refused.  An invalid trajectory ends its problem with a NaN cost and SVSDF_ERR_INVALID; a round that fails gives its error to every
+ * problem in it and the call returns that error.  stats seconds: from the start of the call to the end of the problem's last round;
+ * gpu_seconds: device time of the rounds it took part in.  rounds_out (optional): the rounds of the call (also svsdf_lockstep_rounds).
+ * Solver parameters that svsdf_optimize refuses end every problem at once with that code, nothing launched.  At most 2^31 - 1 query points
+ * in one call.  After a CUDA error only the return value and status_out (that error for every problem not finished) are written.
+ * No progress hook. */
+int svsdf_optimize_device(svsdf_ctx *ctx, const svsdf_lockstep_problem *problems, int n, const svsdf_lbfgs_params *params, int max_in_flight,
+                          svsdf_opt_stats *stats_out, int *status_out, int64_t *rounds_out);
+/* svsdf_round_times: device time (ms) of the rounds of the last svsdf_optimize_lockstep / svsdf_optimize_device call: the evaluation
+ * kernels (pose table to finalize) and the back-end kernels (blobs and the device L-BFGS / MINCO; 0 for svsdf_optimize_lockstep, whose
+ * back end runs on host threads). */
+int svsdf_round_times(const svsdf_ctx *ctx, double *eval_ms, double *backend_ms);
+
 /* ---- "next" row (SURVEY.md §8f rank 1): query-point construction on the device --------------------------------------
  * R8  PlannerManager::generateTraj point collection  plan_manager/src/plan_manager.cpp:156-175
  *     PCSmapManager::getPointsInAABBOutOfLastOne       map_manager/include/map_manager/PCSmap_manager.h:184-219
