@@ -42,6 +42,19 @@ constexpr unsigned FULL = 0xffffffffu;
 using dev::smaxd;
 using dev::smind;
 
+// SVSDF_PHASE_STATS (scripts/outer_phase_stats.py builds the strict unit with it; never defined in the product): the batched
+// k_outer counts, per warp, the descent's issued and useful lane-evaluations and the clock64() cycles of its phases into
+// g_phase_stats[8 blockIdx.x + warp][6]: issued, useful, then cycles of the seed scan (up to the barrier that opens the queue), the
+// descent, the wait at the barrier after it, and the gradient + epilogue + accumulation.  Without the macro none of it exists.
+#ifdef SVSDF_PHASE_STATS
+#define SVSDF_STATS(...) __VA_ARGS__
+#define SVSDF_STATS_PARAM(...) , __VA_ARGS__
+__device__ unsigned long long *g_phase_stats = nullptr;
+#else
+#define SVSDF_STATS(...)
+#define SVSDF_STATS_PARAM(...)
+#endif
+
 // ------------------------------------------------------------------------------------------------
 // Trajectory view over the shared-memory copy of the blob
 // ------------------------------------------------------------------------------------------------
@@ -796,15 +809,17 @@ __device__ __forceinline__ void thread_grad_prel(const TrajView &tv, const Shape
 // evaluations.  Every decision is the sequential loop's decision given the same SDF values: the accepted halving is the
 // FIRST j whose candidate decreases f, the sign comes from the finite difference — bit-identical results (GPU parity tests,
 // strict build).
-// The queue of prepared points is shared by the CTA's 8 warps (wk: 8 x 32 entries of 4 doubles in (px, py, choiceTInit
-// seed and minimum), entry (w, i) at wk[4 (32 w + i)], valid for i < nbw[w]; served in the order i-major, w-minor through
-// the shared cursor): a group that finishes its point writes (sdf, t*) over wk[4 (32 w + i)] and takes the next point of
-// the whole CTA, so the warps of a CTA finish together whatever the lengths of their own descents.  Which group solves a
-// point does not change its result; the reductions stay per warp, fixed order.
+// The queue of prepared points is shared by the CTA's 8 warps and holds `limit` / 256 batches of each (wk: chunks of 8 x 32
+// entries of 4 doubles: px, py, choiceTInit seed and minimum; entry (c, w, i) at wk[4 (256 c + 32 w + i)], valid for
+// i < nbw[8 c + w]; served chunk by chunk, in a chunk i-major, w-minor, through the shared cursor): a group that finishes its
+// point writes (sdf, t*) over the entry's seed and minimum and takes the next point of the whole CTA, so the warps of a CTA
+// finish together whatever the lengths of their own descents, and the groups idle once per pass, when the queue is empty
+// and the longest descent still runs.  Which group solves a point does not change its result; the reductions stay per
+// warp, fixed order.
 // ------------------------------------------------------------------------------------------------
 template <int SHAPE, bool XFORM, bool SCALED = false>
 __device__ __forceinline__ void descent_engine2(const TrajView &tv, const ShapeParams &S, double *wk, const int *nbw, int *cursor,
-                                                int limit, unsigned &evals, const ScaleSched *Z = nullptr) {
+                                                int limit, unsigned &evals SVSDF_STATS_PARAM(unsigned &issued), const ScaleSched *Z = nullptr) {
     enum { E_F0 = 0, E_R1 = 1, E_RN = 2 };
     const int lane = threadIdx.x & 31, q = lane & 3, gbase = lane & 28;
     const double D = tv.D;
@@ -823,11 +838,11 @@ __device__ __forceinline__ void descent_engine2(const TrajView &tv, const ShapeP
             const int c = base + __popc(want & ((1u << gbase) - 1u));
             if (need) {
                 pt = -1;
-                const int cw = c & (kWarpsPerBlock - 1), ci = c >> 3;     // entry (warp cw, point ci)
-                need = c < limit;                                          // a hole (ci >= nbw[cw]): ask again
-                if (c < limit && ci < nbw[cw]) {
+                const int cc = c >> 8, cw = c & (kWarpsPerBlock - 1), ci = (c >> 3) & 31;  // entry (chunk cc, warp cw, point ci)
+                need = c < limit;                                          // a hole (ci >= nbw[8 cc + cw]): ask again
+                if (c < limit && ci < nbw[kWarpsPerBlock * cc + cw]) {
                     need = false;
-                    pt = 32 * cw + ci;
+                    pt = 256 * cc + 32 * cw + ci;
                     const double *w = wk + 4 * pt;
                     px = w[0]; py = w[1];
                     const double nsd = w[2], nmn = w[3];
@@ -858,6 +873,7 @@ __device__ __forceinline__ void descent_engine2(const TrajView &tv, const ShapeP
         const double loA = slopeA ? ((q == 0) ? 0.0 : -INF) : t_min, hiA = slopeA ? ((q == 0) ? INF : D) : t_max;
         const double tcA = smaxd(smind(x + offA, hiA), loA), tcB = smaxd(smind(x + offB, t_max), t_min);
         const double tA = (candA || slopeA) ? tcA : x, tB = candB ? tcB : x;
+        SVSDF_STATS(issued += 64u;)
         const double fA = eval_sdf<SHAPE, XFORM, SCALED>(tv, S, px, py, tA, hintA, Z);
         const double fB = eval_sdf<SHAPE, XFORM, SCALED>(tv, S, px, py, tB, hintB, Z);
 
@@ -892,7 +908,7 @@ __device__ __forceinline__ void descent_engine2(const TrajView &tv, const ShapeP
         mode = (step_end || isF0) ? E_R1 : E_RN;
         jbase = jb_next;
         if (step_end && !running) {
-            if (q == 0) { wk[4 * pt] = fx; wk[4 * pt + 1] = x; }
+            if (q == 0) { wk[4 * pt + 2] = fx; wk[4 * pt + 3] = x; }
             pt = -1;
             need = true;
         }
@@ -1016,7 +1032,7 @@ template <int SHAPE, bool XFORM, bool BATCHED, bool SCALED>
 __device__ __forceinline__ void outer_body(const KernelArgs &A, const ShapeParams &S, const ScaleSched *Z, int vblock, int vgrid) {
     extern __shared__ __align__(16) double smem[];
     __shared__ __align__(8) uint64_t bar;
-    __shared__ int s_nb[kWarpsPerBlock];
+    __shared__ int s_nb[kOuterChunkMax * kWarpsPerBlock];
     __shared__ int s_cursor;
     double *sblob = smem;
     tma_load_blob(sblob, A.blob, A.blob_doubles, &bar);
@@ -1038,88 +1054,126 @@ __device__ __forceinline__ void outer_body(const KernelArgs &A, const ShapeParam
     //    length), warp w owns batches w, w + W, ... (strided: a warp's batches come from different regions of the map, so
     //    hard regions are spread over the warps; static, hence deterministic).  choiceTInit and the FD gradient /
     //    penalty / chain rule run one point per lane, gradientDescent one point per group of 4 lanes, served from the CTA's
-    //    point queue (descent_engine2).
+    //    point queue (descent_engine2).  A pass takes up to A.outer_chunk batches of every warp: their seeds go into the queue
+    //    batch after batch, ONE descent pass drains it, then the warp finishes its batches in order.  The descents' lengths
+    //    vary by +-40 %, so every pass ends with groups idling until the longest one is done: fewer, longer passes idle less.
+    //    Nothing but the work area lives across the descent; the epilogue reads the point back from it.
     //  * Sparse schedule (few points per warp, i.e. small problems): the warp owns points w, w + W, ...; everything one
     //    point per warp, as solve_outer / grad_prel do (lowest latency).
     const int64_t lstride = BATCHED ? 1 : wstride;  // distance between the points of neighbouring lanes
     const int64_t nB = wstride * ((A.P + 32 * wstride - 1) / (32 * wstride));   // batches (batched schedule)
-    for (int64_t bi = first; BATCHED ? (bi < nB) : (bi < A.P); bi += BATCHED ? wstride : 32 * wstride) {
-        // batched: batch bi covers [bi P / nB, (bi + 1) P / nB); sparse: points bi, bi + W, ...
-        const int64_t bfirst = BATCHED ? (bi * A.P) / nB : bi;
-        const int64_t bend = BATCHED ? ((bi + 1) * A.P) / nB : A.P;
-        const int64_t my_pt = bfirst + (int64_t)lane * lstride;
-        const int nb = (int)min((int64_t)32, (bend - bfirst + lstride - 1) / lstride);  // batch size (warp-uniform)
-        const bool my_valid = lane < nb;
-        const int64_t ld_pt = my_valid ? my_pt : bfirst;
-        const double mpx = __ldg(A.points_xy + 2 * ld_pt), mpy = __ldg(A.points_xy + 2 * ld_pt + 1);
-        double m_seed = 0.0, m_min = 1e9, m_sdf = 0.0, m_ts = 0.0, m_gx = 0.0, m_gy = 0.0;
+    const int chunk = BATCHED ? A.outer_chunk : 1;  // batches of a warp per descent pass
+    SVSDF_STATS(unsigned long long st_issued = 0, st_useful = 0, st_seed = 0, st_desc = 0, st_wait = 0, st_epi = 0;)
+    for (int64_t bi = first; BATCHED ? (bi < nB) : (bi < A.P); bi += BATCHED ? chunk * wstride : 32 * wstride) {
+        int nc = 1;  // batches of this pass: bi, bi + W, ...  (nB is a multiple of W: the same for every warp of the CTA)
         if (BATCHED) {  // the whole CTA: the batched schedule synchronises the CTA around its shared queue
+            nc = (int)min((int64_t)chunk, (nB - bi + wstride - 1) / wstride);
+            SVSDF_STATS(const long long c0 = clock64();)
             int ev = 0;
-            if (my_valid) thread_choice_t_init<SHAPE, XFORM>(tv, S, mpx, mpy, A.win2, A.win3, m_seed, m_min, ev);
-            __syncwarp();
-            unsigned ev2 = 0;
-            if (my_valid) { res[4 * lane] = mpx; res[4 * lane + 1] = mpy; res[4 * lane + 2] = m_seed; res[4 * lane + 3] = m_min; }
-            if (lane == 0) s_nb[warp] = nb;
-            if (threadIdx.x == 0) s_cursor = 0;
-            __syncthreads();   // every warp has the same number of batches (nB is a multiple of the warp count)
-            descent_engine2<SHAPE, XFORM, SCALED>(tv, S, res - 128 * warp, s_nb, &s_cursor, kWarpsPerBlock * 32, ev2, Z);
-            __syncthreads();
-            if (my_valid) { m_sdf = res[4 * lane]; m_ts = res[4 * lane + 1]; }
-            my_evals += (unsigned long long)__reduce_add_sync(FULL, (unsigned)ev + ev2);
-            __syncwarp();
-        } else {
 #pragma unroll 1
-            for (int i = 0; i < nb; ++i) {
-                const double px = __shfl_sync(FULL, mpx, i), py = __shfl_sync(FULL, mpy, i);
-                const OuterResult R = solve_outer<SHAPE, XFORM, SCALED>(tv, S, px, py, A.win2, A.win3, false, 0.0, 1e9, Z);
-                my_evals += (unsigned long long)R.evals;
-                if (lane == i) { m_sdf = R.sdf; m_ts = R.tstar; }
-                double gx, gy;
-                grad_prel<SHAPE, XFORM, SCALED>(tv, S, px, py, R.tstar, gx, gy, Z);
-                if (lane == i) { m_gx = gx; m_gy = gy; }
-            }
-        }
-        my_evals += 4ull * (unsigned long long)nb;
-        if (BATCHED && my_valid) thread_grad_prel<SHAPE, XFORM, SCALED>(tv, S, mpx, mpy, m_ts, m_gx, m_gy, Z);
-        // ---- per-lane epilogue: outputs, interior flag, penalty + chain rule (one point per lane) ----
-        const bool inside = my_valid && A.want_gsip && !(m_sdf > 0);  // getTrueSDFofSweptVolume: `if (argmin_dis > 0) return`
-        if (my_valid) {
-            if (A.out_sdf) A.out_sdf[my_pt] = m_sdf;
-            if (A.out_tstar) A.out_tstar[my_pt] = m_ts;
-            if (A.out_grad) { A.out_grad[3 * my_pt] = m_gx; A.out_grad[3 * my_pt + 1] = m_gy; A.out_grad[3 * my_pt + 2] = 0.0; }
-            if (A.out_rounds) A.out_rounds[my_pt] = 0;
-            if (A.inside_flag) A.inside_flag[my_pt] = inside ? 1 : 0;
-            if (inside && A.inside_tstar) A.inside_tstar[my_pt] = m_ts;
-        }
-        if (A.want_reduce) {
-            Contribution C;
-            C.active = false;
-            if (my_valid && !inside) C = point_contribution<SCALED>(tv, A.cp, mpx, mpy, m_sdf, m_ts, m_gx, m_gy, Z);
-            // accumulate the active lanes' contributions in batch order (deterministic)
-            unsigned m = __ballot_sync(FULL, C.active);
-            while (m) {
-                const int src = __ffs(m) - 1;
-                m &= m - 1;
-                const int piece = __shfl_sync(FULL, C.piece, src);
-                const double s1 = __shfl_sync(FULL, C.s1, src);
-                const double g0 = __shfl_sync(FULL, C.G[0], src), g1 = __shfl_sync(FULL, C.G[1], src),
-                             g2 = __shfl_sync(FULL, C.G[2], src);
-                const double gdT = __shfl_sync(FULL, C.gdT, src), pena = __shfl_sync(FULL, C.pena, src);
-                if (lane < 18) {
-                    const int d = lane / 6, q = lane - 6 * d;
-                    const double s2 = s1 * s1, s3 = s2 * s1, s4 = s2 * s2, s5 = s4 * s1;
-                    const double beta = (q == 0) ? 1.0 : (q == 1) ? s1 : (q == 2) ? s2 : (q == 3) ? s3 : (q == 4) ? s4 : s5;
-                    const double gd = (d == 0) ? g0 : (d == 1) ? g1 : g2;
-                    acc[piece * 18 + lane] += beta * gd;
-                } else if (lane == 18) {
-                    acc[18 * tv.N + piece] += gdT;
-                } else if (lane == 19) {
-                    acc[19 * tv.N] += pena;
+            for (int c = 0; c < nc; ++c) {  // seeds of batch c, one point per lane, into work-area entry (c, warp, lane)
+                const int64_t b = bi + c * wstride;
+                const int64_t bfirst = (b * A.P) / nB;
+                const int nb = (int)min((int64_t)32, ((b + 1) * A.P) / nB - bfirst);
+                if (lane < nb) {
+                    const double px = __ldg(A.points_xy + 2 * (bfirst + lane)), py = __ldg(A.points_xy + 2 * (bfirst + lane) + 1);
+                    double seed = 0.0, mn = 1e9;
+                    thread_choice_t_init<SHAPE, XFORM>(tv, S, px, py, A.win2, A.win3, seed, mn, ev);
+                    double *e = res + 1024 * c + 4 * lane;
+                    e[0] = px; e[1] = py; e[2] = seed; e[3] = mn;
                 }
                 __syncwarp();
+                if (lane == 0) s_nb[kWarpsPerBlock * c + warp] = nb;
+            }
+            unsigned ev2 = 0;
+            SVSDF_STATS(unsigned issued = 0;)
+            if (threadIdx.x == 0) s_cursor = 0;
+            SVSDF_STATS(const long long c1 = clock64();)
+            __syncthreads();
+            SVSDF_STATS(const long long c2 = clock64();)
+            descent_engine2<SHAPE, XFORM, SCALED>(tv, S, res - 128 * warp, s_nb, &s_cursor, nc * kWarpsPerBlock * 32, ev2 SVSDF_STATS_PARAM(issued), Z);
+            SVSDF_STATS(const long long c3 = clock64();)
+            __syncthreads();
+            SVSDF_STATS(const long long c4 = clock64(); st_seed += c2 - c0; st_desc += c3 - c2; st_wait += c4 - c3;
+                        st_issued += issued; st_useful += __reduce_add_sync(FULL, ev2);)
+            my_evals += (unsigned long long)__reduce_add_sync(FULL, (unsigned)ev + ev2);
+            __syncwarp();
+        }
+        SVSDF_STATS(const long long c5 = clock64();)
+#pragma unroll 1
+        for (int c = 0; c < nc; ++c) {  // the batches of the pass in their own order: the warp's summation chain (sparse: one)
+            // batched: batch b covers [b P / nB, (b + 1) P / nB); sparse: points bi, bi + W, ...
+            const int64_t b = bi + c * wstride;
+            const int64_t bfirst = BATCHED ? (b * A.P) / nB : b;
+            const int64_t bend = BATCHED ? ((b + 1) * A.P) / nB : A.P;
+            const int64_t my_pt = bfirst + (int64_t)lane * lstride;
+            const int nb = (int)min((int64_t)32, (bend - bfirst + lstride - 1) / lstride);  // batch size (warp-uniform)
+            const bool my_valid = lane < nb;
+            double mpx = 0.0, mpy = 0.0, m_sdf = 0.0, m_ts = 0.0, m_gx = 0.0, m_gy = 0.0;
+            if (BATCHED) {
+                const double *e = res + 1024 * c + 4 * lane;
+                if (my_valid) { mpx = e[0]; mpy = e[1]; m_sdf = e[2]; m_ts = e[3]; }
+            } else {
+                const int64_t ld_pt = my_valid ? my_pt : bfirst;
+                mpx = __ldg(A.points_xy + 2 * ld_pt); mpy = __ldg(A.points_xy + 2 * ld_pt + 1);
+#pragma unroll 1
+                for (int i = 0; i < nb; ++i) {
+                    const double px = __shfl_sync(FULL, mpx, i), py = __shfl_sync(FULL, mpy, i);
+                    const OuterResult R = solve_outer<SHAPE, XFORM, SCALED>(tv, S, px, py, A.win2, A.win3, false, 0.0, 1e9, Z);
+                    my_evals += (unsigned long long)R.evals;
+                    if (lane == i) { m_sdf = R.sdf; m_ts = R.tstar; }
+                    double gx, gy;
+                    grad_prel<SHAPE, XFORM, SCALED>(tv, S, px, py, R.tstar, gx, gy, Z);
+                    if (lane == i) { m_gx = gx; m_gy = gy; }
+                }
+            }
+            my_evals += 4ull * (unsigned long long)nb;
+            if (BATCHED && my_valid) thread_grad_prel<SHAPE, XFORM, SCALED>(tv, S, mpx, mpy, m_ts, m_gx, m_gy, Z);
+            // ---- per-lane epilogue: outputs, interior flag, penalty + chain rule (one point per lane) ----
+            const bool inside = my_valid && A.want_gsip && !(m_sdf > 0);  // getTrueSDFofSweptVolume: `if (argmin_dis > 0) return`
+            if (my_valid) {
+                if (A.out_sdf) A.out_sdf[my_pt] = m_sdf;
+                if (A.out_tstar) A.out_tstar[my_pt] = m_ts;
+                if (A.out_grad) { A.out_grad[3 * my_pt] = m_gx; A.out_grad[3 * my_pt + 1] = m_gy; A.out_grad[3 * my_pt + 2] = 0.0; }
+                if (A.out_rounds) A.out_rounds[my_pt] = 0;
+                if (A.inside_flag) A.inside_flag[my_pt] = inside ? 1 : 0;
+                if (inside && A.inside_tstar) A.inside_tstar[my_pt] = m_ts;
+            }
+            if (A.want_reduce) {
+                Contribution C;
+                C.active = false;
+                if (my_valid && !inside) C = point_contribution<SCALED>(tv, A.cp, mpx, mpy, m_sdf, m_ts, m_gx, m_gy, Z);
+                // accumulate the active lanes' contributions in batch order (deterministic)
+                unsigned m = __ballot_sync(FULL, C.active);
+                while (m) {
+                    const int src = __ffs(m) - 1;
+                    m &= m - 1;
+                    const int piece = __shfl_sync(FULL, C.piece, src);
+                    const double s1 = __shfl_sync(FULL, C.s1, src);
+                    const double g0 = __shfl_sync(FULL, C.G[0], src), g1 = __shfl_sync(FULL, C.G[1], src),
+                                 g2 = __shfl_sync(FULL, C.G[2], src);
+                    const double gdT = __shfl_sync(FULL, C.gdT, src), pena = __shfl_sync(FULL, C.pena, src);
+                    if (lane < 18) {
+                        const int d = lane / 6, q = lane - 6 * d;
+                        const double s2 = s1 * s1, s3 = s2 * s1, s4 = s2 * s2, s5 = s4 * s1;
+                        const double beta = (q == 0) ? 1.0 : (q == 1) ? s1 : (q == 2) ? s2 : (q == 3) ? s3 : (q == 4) ? s4 : s5;
+                        const double gd = (d == 0) ? g0 : (d == 1) ? g1 : g2;
+                        acc[piece * 18 + lane] += beta * gd;
+                    } else if (lane == 18) {
+                        acc[18 * tv.N + piece] += gdT;
+                    } else if (lane == 19) {
+                        acc[19 * tv.N] += pena;
+                    }
+                    __syncwarp();
+                }
             }
         }
+        SVSDF_STATS(if (BATCHED) st_epi += clock64() - c5;)
     }
+    SVSDF_STATS(if (BATCHED && g_phase_stats && lane == 0) {
+        unsigned long long *st = g_phase_stats + 6 * ((size_t)blockIdx.x * kWarpsPerBlock + warp);
+        st[0] = st_issued; st[1] = st_useful; st[2] = st_seed; st[3] = st_desc; st[4] = st_wait; st[5] = st_epi;
+    })
     if (A.eval_counter && lane == 0) atomicAdd(A.eval_counter, my_evals);
     if (A.want_reduce) {
         __syncthreads();
@@ -1602,7 +1656,8 @@ static cudaError_t dispatch(const KernelArgs &A, const ShapeParams &S, const Sca
 }
 
 template <int SHAPE, bool XFORM>
-static cudaError_t occ_shape(size_t smem_outer, size_t smem_gsip, int *occ_outer, int *occ_gsip) {
+static cudaError_t occ_shape(int N, int blob_doubles, int *occ_outer, int *occ_gsip, int *chunk_outer) {
+    const size_t smem_outer = outer_smem_doubles(blob_doubles, N, 1) * sizeof(double), smem_gsip = (size_t)blob_doubles * sizeof(double);
     const void *k[4];
     cost_kernels<SHAPE, XFORM, kScaledUnit>(k);
     for (int i = 0; i < 3; ++i) {
@@ -1612,18 +1667,28 @@ static cudaError_t occ_shape(size_t smem_outer, size_t smem_gsip, int *occ_outer
     // the two schedules are compiled to the same register cap (launch bounds); the batched kernel sizes the full wave
     cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ_outer, k[1], kWarpsPerBlock * 32, smem_outer);
     if (e != cudaSuccess) return e;
+    // the largest chunk whose work area fits and leaves that residency alone (the grid is sized from it)
+    for (*chunk_outer = kOuterChunkMax; *chunk_outer > 1; --*chunk_outer) {
+        const size_t sc = outer_smem_doubles(blob_doubles, N, *chunk_outer) * sizeof(double);
+        int occ = 0;
+        if (sc > 200 * 1024) continue;
+        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k[1], kWarpsPerBlock * 32, sc);
+        if (e != cudaSuccess) return e;
+        if (occ == *occ_outer) break;
+    }
     return cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ_gsip, k[2], kWarpsPerBlock * 32, smem_gsip);
 }
 
 // Resident CTAs per SM of k_outer / k_gsip for this shape and trajectory size: the host sizes the grids as
-// SMs x occupancy so that the warp-stride loops run as exactly one full wave (no partial second wave).
-cudaError_t query_occupancy(const ShapeParams &S, int N, int blob_doubles, int *occ_outer, int *occ_gsip) {
-    const size_t so = outer_smem_doubles(blob_doubles, N) * sizeof(double);
-    const size_t sg = (size_t)blob_doubles * sizeof(double);
+// SMs x occupancy so that the warp-stride loops run as exactly one full wave (no partial second wave).  k_outer's is taken with a
+// chunk of 1; *chunk_outer is the largest chunk (<= kOuterChunkMax) at which it is still the same.
+cudaError_t query_occupancy(const ShapeParams &S, int N, int blob_doubles, int *occ_outer, int *occ_gsip, int *chunk_outer) {
     const bool xf = S.has_xform != 0;
     switch (S.id) {
 #define SVSDF_CASE(ID) \
-    case ID: return xf ? occ_shape<ID, true>(so, sg, occ_outer, occ_gsip) : occ_shape<ID, false>(so, sg, occ_outer, occ_gsip);
+    case ID:                 \
+        return xf ? occ_shape<ID, true>(N, blob_doubles, occ_outer, occ_gsip, chunk_outer) \
+                  : occ_shape<ID, false>(N, blob_doubles, occ_outer, occ_gsip, chunk_outer);
         SVSDF_CASE(SH_STAR)
         SVSDF_CASE(SH_HORSESHOE)
         SVSDF_CASE(SH_PIE)
@@ -1642,8 +1707,8 @@ cudaError_t query_occupancy(const ShapeParams &S, int N, int blob_doubles, int *
         SVSDF_CASE(SH_UNEVENCAPSULE)
         SVSDF_CASE(SH_CIRCLE)
 #undef SVSDF_CASE
-        case SH_POLYGON: return occ_shape<SH_POLYGON, false>(so, sg, occ_outer, occ_gsip);
-        case SH_MESH: return occ_shape<SH_MESH, false>(so, sg, occ_outer, occ_gsip);
+        case SH_POLYGON: return occ_shape<SH_POLYGON, false>(N, blob_doubles, occ_outer, occ_gsip, chunk_outer);
+        case SH_MESH: return occ_shape<SH_MESH, false>(N, blob_doubles, occ_outer, occ_gsip, chunk_outer);
         default: return cudaErrorInvalidValue;
     }
 }
@@ -1655,7 +1720,7 @@ cudaError_t launch_cost_kernels(const KernelArgs &A, const ShapeParams &S, const
     cfg.gsip_wide = gsip_wide != 0;
     cfg.grid_outer = grid_outer;
     cfg.grid_gsip = grid_gsip;
-    cfg.smem_outer = outer_smem_doubles(A.blob_doubles, N) * sizeof(double);
+    cfg.smem_outer = outer_smem_doubles(A.blob_doubles, N, A.batched ? A.outer_chunk : 1) * sizeof(double);
     cfg.smem_gsip = (size_t)A.blob_doubles * sizeof(double);
     cfg.stream = stream;
     return S.has_xform ? dispatch<true>(A, S, Z, cfg, N) : dispatch<false>(A, S, Z, cfg, N);

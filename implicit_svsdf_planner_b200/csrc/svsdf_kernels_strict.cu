@@ -2,3 +2,10 @@
 // CPU oracle / the reference's x86-64 build (SURVEY.md §7 "Hard parts").
 #define SVSDF_NS strict
 #include "svsdf_kernels.cuh"
+
+#ifdef SVSDF_PHASE_STATS
+// scripts/outer_phase_stats.py: where the batched k_outer of this unit writes its per-warp counters ([8 x grid][6] 64-bit words)
+extern "C" int svsdf_phase_stats_buffer(unsigned long long *buf) {
+    return (int)cudaMemcpyToSymbol(svsdf::strict::g_phase_stats, &buf, sizeof(buf));
+}
+#endif

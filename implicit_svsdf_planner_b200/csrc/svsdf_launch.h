@@ -12,7 +12,8 @@ namespace svsdf {
 // one full wave of the chosen variant).
 #define SVSDF_DECLARE_LAUNCHERS(NS, MULTI)                                                                        \
     namespace NS {                                                                                               \
-    cudaError_t query_occupancy(const ShapeParams &S, int N, int blob_doubles, int *occ_outer, int *occ_gsip);   \
+    cudaError_t query_occupancy(const ShapeParams &S, int N, int blob_doubles, int *occ_outer, int *occ_gsip,    \
+                                int *chunk_outer);                                                               \
     cudaError_t launch_cost_kernels(const KernelArgs &A, const ShapeParams &S, const ScaleSched *Z, int N,       \
                                     int grid_outer, int grid_gsip, cudaStream_t stream, cudaEvent_t after_outer, \
                                     int gsip_wide);                                                              \

@@ -129,9 +129,10 @@ using DeviceBuffer = Buffer<T>;
 template <class T>
 using PinnedBuffer = Buffer<T, true>;
 
-// (resident single-problem k_outer, k_gsip CTAs per SM) of one trajectory size
+// (resident single-problem k_outer, k_gsip CTAs per SM) of one trajectory size; chunk: the most batches per descent pass (<=
+// kOuterChunkMax) whose work area leaves k_outer's residency what it is with one
 struct Occupancy {
-    int outer, gsip;
+    int outer, gsip, chunk;
 };
 
 struct svsdf_ctx {
@@ -247,6 +248,9 @@ struct svsdf_ctx {
     // test hook of the pose windows, read ONCE at svsdf_create: SVSDF_FORCE_POSE_WINDOWS = 0 (none: every layer evaluates the
     // trajectory), 1 (layer 2 only) or 2 (layers 2 and 3), whatever pose_windows' rule says; -1 = not set
     int force_pose_windows = -1;
+    // test hook of the batched k_outer, read ONCE at svsdf_create: SVSDF_FORCE_OUTER_CHUNK = n > 0 sets the batches per descent pass
+    // (outer_chunk), whatever the rounds and the residency say; still clipped to kOuterChunkMax and the shared memory; -1 = not set
+    int force_outer_chunk = -1;
     // svsdf_cost_grad_multi / svsdf_optimize_lockstep: packed inputs (one pinned stage mirrored by one device block, one copy in),
     // scratch, pinned outputs (one copy out)
     PinnedBuffer<unsigned char> h_multi_in;
@@ -552,9 +556,9 @@ int occupancy(svsdf_ctx *ctx, int N, int blob, Occupancy *occ) {
     const auto key = std::make_tuple(N, blob, ctx->scaled ? 1 : 0);
     auto it = ctx->occ_cache.find(key);
     if (it == ctx->occ_cache.end()) {
-        int oo = 0, og = 0;
-        CK(kernels(ctx).query_occupancy(ctx->shape, N, blob, &oo, &og));
-        it = ctx->occ_cache.emplace(key, Occupancy{oo > 0 ? oo : 1, og > 0 ? og : 1}).first;
+        int oo = 0, og = 0, ch = 1;
+        CK(kernels(ctx).query_occupancy(ctx->shape, N, blob, &oo, &og, &ch));
+        it = ctx->occ_cache.emplace(key, Occupancy{oo > 0 ? oo : 1, og > 0 ? og : 1, ch}).first;
     }
     *occ = it->second;
     return SVSDF_OK;
@@ -576,6 +580,20 @@ OuterPlan outer_plan(const svsdf_ctx *ctx, int64_t P, const Occupancy &occ) {
     plan.batched = (P >= (int64_t)16 * plan.grid * kWarpsPerBlock) ? 1 : 0;
     if (ctx->force_batched >= 0) plan.batched = ctx->force_batched;  // test hook
     return plan;
+}
+
+// Batches of a warp per descent pass of a batched k_outer launch whose warps own up to `rounds` batches and whose shared memory is
+// sized by (blob, N): as many as there are rounds, up to what keeps the residency (occ.chunk).  The chunk changes who solves a point
+// and when, never a bit of the results, so a problem's may differ between its single and its multi call.
+int outer_chunk(const svsdf_ctx *ctx, const Occupancy &occ, int64_t rounds, int blob, int N) {
+    int64_t c = std::min<int64_t>(occ.chunk, rounds);
+    if (ctx->force_outer_chunk > 0) c = std::min(ctx->force_outer_chunk, kOuterChunkMax);  // test hook
+    while (c > 1 && outer_smem_doubles(blob, N, (int)c) * sizeof(double) > 200 * 1024) --c;
+    return (int)std::max<int64_t>(c, 1);
+}
+int64_t outer_rounds(int64_t P, int grid) {
+    const int64_t per = (int64_t)32 * grid * kWarpsPerBlock;
+    return (P + per - 1) / per;
 }
 
 // k_gsip's variant from the interior points of the previous evaluation (-1: none): few -> 22-warp CTAs (one warp per ring sample,
@@ -621,6 +639,7 @@ int run_kernels(svsdf_ctx *ctx, const double *d_points, int64_t P, bool reduce, 
     A.want_reduce = reduce ? 1 : 0;
     A.want_gsip = gsip ? 1 : 0;
     A.batched = plan.batched;
+    A.outer_chunk = outer_chunk(ctx, occ, outer_rounds(P, grid), A.blob_doubles, N);
     A.inside_flag = ctx->d_flag;
     A.inside_tstar = ctx->d_inside_tstar;
     A.inside_list = ctx->d_inside_list;
@@ -633,7 +652,7 @@ int run_kernels(svsdf_ctx *ctx, const double *d_points, int64_t P, bool reduce, 
     GsipPlan gp = gsip_plan(ctx, reduce ? ctx->last_n_inside : -1);
     if (gp.grid == 0) gp.grid = gp.wide ? ctx->sm_count : ctx->sm_count * occ.gsip;
     if (!gsip) CK(cudaMemsetAsync(ctx->d_n_inside, 0, sizeof(int), ctx->stream));
-    size_t smem = outer_smem_doubles(A.blob_doubles, N) * sizeof(double);
+    size_t smem = outer_smem_doubles(A.blob_doubles, N, 1) * sizeof(double);
     if (smem > 200 * 1024) {
         ctx->err = "svsdf: trajectory blob does not fit in shared memory";
         return SVSDF_ERR_INVALID;
@@ -726,6 +745,8 @@ struct MultiPlan {
     int64_t pt_span = 0;   // points the pt_off values span (inside t* and lists are indexed by pt_off)
     int max_K1 = 1, max_N = 1, max_blob = 2;
     int smax_blob[2] = {0, 0}, smax_N[2] = {1, 1};  // per k_outer_multi launch (sparse, batched): the shared memory is sized by its largest
+    int64_t max_rounds = 1;  // most batches a warp of the batched launch owns
+    int chunk = 1;           // the batched launch's batches per descent pass (outer_chunk at its largest blob and N)
     size_t o_ms = 0, o_mb = 0, head_bytes = 0;        // packed head: problem table | CTA maps (sparse, batched)
 };
 
@@ -750,12 +771,19 @@ int plan_multi(svsdf_ctx *ctx, MultiPlan &pl) {
         pl.max_blob = std::max(pl.max_blob, m.blob_doubles);
         pl.smax_blob[batched] = std::max(pl.smax_blob[batched], m.blob_doubles);
         pl.smax_N[batched] = std::max(pl.smax_N[batched], m.N);
+        if (batched) pl.max_rounds = std::max(pl.max_rounds, outer_rounds(m.P, G));
     }
     for (int b = 0; b < 2; ++b)
-        if (outer_smem_doubles(pl.smax_blob[b], pl.smax_N[b]) * sizeof(double) > 200 * 1024) {
+        if (outer_smem_doubles(pl.smax_blob[b], pl.smax_N[b], 1) * sizeof(double) > 200 * 1024) {
             ctx->err = "svsdf: trajectory blob does not fit in shared memory";
             return SVSDF_ERR_INVALID;
         }
+    if (!pl.map_b.empty()) {
+        Occupancy occ;
+        int rc = occupancy(ctx, pl.smax_N[1], pl.smax_blob[1], &occ);
+        if (rc) return rc;
+        pl.chunk = outer_chunk(ctx, occ, pl.max_rounds, pl.smax_blob[1], pl.smax_N[1]);
+    }
     pl.o_ms = align16(pl.pr.size() * sizeof(MultiProblem));
     pl.o_mb = align16(pl.o_ms + pl.map_s.size() * sizeof(int));
     pl.head_bytes = align16(pl.o_mb + pl.map_b.size() * sizeof(int));
@@ -820,8 +848,9 @@ int launch_plan(svsdf_ctx *ctx, const MultiPlan &pl, const unsigned char *d, dou
         const std::vector<int> &mp = b ? pl.map_b : pl.map_s;
         if (mp.empty()) continue;
         M.cta_map = reinterpret_cast<const int *>(d + (b ? pl.o_mb : pl.o_ms));
-        CK(K.multi(b, A, M, ctx->shape, Z, (int)(mp.size() / 2), outer_smem_doubles(pl.smax_blob[b], pl.smax_N[b]) * sizeof(double), 0,
-                   ctx->sm_count, ctx->stream));
+        A.outer_chunk = b ? pl.chunk : 1;
+        CK(K.multi(b, A, M, ctx->shape, Z, (int)(mp.size() / 2),
+                   outer_smem_doubles(pl.smax_blob[b], pl.smax_N[b], A.outer_chunk) * sizeof(double), 0, ctx->sm_count, ctx->stream));
         ++launches;
     }
     M.cta_map = nullptr;
@@ -1462,6 +1491,7 @@ int svsdf_create(const svsdf_config *cfg, svsdf_ctx **out) {
     if (const char *fg = std::getenv("SVSDF_FORCE_GRID_GSIP")) ctx->force_grid_gsip = std::atoi(fg);
     if (const char *fg = std::getenv("SVSDF_FORCE_GRID_ASTAR")) ctx->force_grid_astar = std::atoi(fg);
     if (const char *fp = std::getenv("SVSDF_FORCE_POSE_WINDOWS")) ctx->force_pose_windows = std::atoi(fp);
+    if (const char *fc = std::getenv("SVSDF_FORCE_OUTER_CHUNK")) ctx->force_outer_chunk = std::atoi(fc);
     auto fail = [&](cudaError_t e) {
         std::fprintf(stderr, "svsdf_create: %s\n", cudaGetErrorString(e));
         svsdf_destroy(ctx);

@@ -126,9 +126,12 @@ struct alignas(32) PoseRec {
 SVSDF_HD inline int64_t win2_records(int K1) { return (int64_t)(K1 + 1) * kWinLen; }
 SVSDF_HD inline int64_t win3_records(int K1) { return (int64_t)(K1 + 1) * kWin3Stride * kWinLen; }
 
-// dynamic shared memory of k_outer in doubles: [ blob | 8 warps x (19N + 1) accumulators | 8 warps x 32 x 4 work area ]
-SVSDF_HD inline size_t outer_smem_doubles(int blob_doubles, int N) {
-    return (size_t)blob_doubles + (size_t)kWarpsPerBlock * (19 * N + 1) + (size_t)kWarpsPerBlock * 128;
+// Batched k_outer: a warp's batches whose descents share one pass over the CTA's point queue (KernelArgs::outer_chunk).  The host
+// takes the largest chunk <= kOuterChunkMax that the launch has rounds for and that leaves the kernel's residency what it is at 1.
+constexpr int kOuterChunkMax = 4;
+// dynamic shared memory of k_outer in doubles: [ blob | 8 warps x (19N + 1) accumulators | chunk x 8 warps x 32 x 4 work area ]
+SVSDF_HD inline size_t outer_smem_doubles(int blob_doubles, int N, int chunk) {
+    return (size_t)blob_doubles + (size_t)kWarpsPerBlock * (19 * N + 1) + (size_t)chunk * kWarpsPerBlock * 128;
 }
 
 // Penalty parameters (star.yaml: weight_p 60, safety_hor 0.7; smoothedL1 mu = 0.01 is a literal in the
@@ -153,6 +156,7 @@ struct KernelArgs {
     int want_reduce;
     int want_gsip;             // 0: stop after the outer solve (getSDFofSweptVolume semantics)
     int batched;               // k_outer: run choiceTInit / gradient / chain rule one point per lane (large P)
+    int outer_chunk;           // batched k_outer: batches per warp that share one descent pass (1 .. kOuterChunkMax; sizes the work area)
     // inside-point bookkeeping
     unsigned char *inside_flag;  // P
     double *inside_tstar;        // P (sparse: written for inside points only)
