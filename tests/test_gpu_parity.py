@@ -68,14 +68,13 @@ def test_shape_functors_match_oracle(oracle_mod, strict):
 
 def test_strict_shape_functors_are_bitwise(oracle_mod):
     """The strict build uses only IEEE-exact operations in the shape functors (+, -, *, sqrt, and divisions either
-    native or by Markstein's corrected reciprocal for compile-time divisors), so it must reproduce the CPU bit for bit."""
+    native or by Markstein's corrected reciprocal for compile-time divisors), so it must reproduce the CPU bit for bit.
+    The Polygon fallback ("unknown_mesh_shape") included: its crossing test calls the same pinned atan2 on both sides."""
     rng = np.random.default_rng(77)
     rel = np.c_[rng.uniform(-8, 8, size=(200_000, 2)), np.zeros(200_000)]
     rel[:1000, :2] = rng.uniform(-0.05, 0.05, size=(1000, 2))  # near the origin / symmetry axes
     for pp in ((0.0, 0.0, 0.0), (0.6, -0.3, 25.0)):
         for name in ALL_SHAPES:
-            if name == "unknown_mesh_shape":
-                continue  # polygon uses atan2 (libm) for its inside test
             ctx = api.Context(name, poly_params=pp, strict_fp=True)
             s_gpu = ctx.shape_sdf(rel)
             s_cpu = oracle_mod.shape_sdf(name, rel, poly_params=pp)
