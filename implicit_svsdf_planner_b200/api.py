@@ -242,6 +242,7 @@ EXPORTED_SYMBOLS = [
     "svsdf_front_astar_device", "svsdf_set_scale", "svsdf_scale_matrix",
     "svsdf_cost_grad_multi", "svsdf_optimize_lockstep", "svsdf_lockstep_rounds", "svsdf_optimize_device", "svsdf_round_times", "svsdf_swept_contour", "svsdf_swept_free",
     "svsdf_map_clearance", "svsdf_clearance_free", "svsdf_map_clearance_multi",
+    "svsdf_default_dynamics", "svsdf_set_dynamics", "svsdf_dynamics_penalty",
 ]
 
 
@@ -318,6 +319,10 @@ def lib():
     L.svsdf_device_ptr_points.argtypes = [vp, C.POINTER(vp)]
     L.svsdf_set_scale.argtypes = [vp, C.POINTER(Scale)]
     L.svsdf_scale_matrix.argtypes = [C.POINTER(Scale), C.c_double, dp, dp]
+    L.svsdf_default_dynamics.argtypes = [C.POINTER(Dynamics)]
+    L.svsdf_default_dynamics.restype = None
+    L.svsdf_set_dynamics.argtypes = [vp, C.POINTER(Dynamics)]
+    L.svsdf_dynamics_penalty.argtypes = [C.POINTER(Dynamics), C.c_int, dp, dp, dp, dp, dp]
     L.svsdf_cost_grad_multi.argtypes = [vp, C.c_int, C.POINTER(MultiProblem)]
     L.svsdf_optimize_lockstep.argtypes = [vp, C.POINTER(LockstepProblem), C.c_int, C.POINTER(LbfgsParams), C.c_int, C.POINTER(OptStats),
                                           C.POINTER(C.c_int)]
@@ -372,6 +377,53 @@ def scale_matrix(t, a, b=(0.0, 0.0), w=(0.0, 0.0), phi=(0.0, 0.0)):
 
 def _p(a):
     return a.ctypes.data_as(dp) if a is not None else None
+
+
+class Dynamics(C.Structure):
+    """svsdf_dynamics: the back end's speed and yaw-rate limits and their penalty's weights (svsdf_set_dynamics)."""
+    _fields_ = [("vmax", C.c_double), ("omgmax", C.c_double), ("weight_v", C.c_double), ("weight_omg", C.c_double),
+                ("smoothingEps", C.c_double), ("integralIntervs", C.c_int)]
+
+    def as_dict(self) -> dict:
+        return {name: getattr(self, name) for name, _ in self._fields_}
+
+
+DYNAMICS_KEYS = ("vmax", "omgmax", "weight_v", "weight_omg", "smoothingEps", "integralIntervs")
+
+
+def dynamics(base=None, **kw) -> Dynamics:
+    """A Dynamics: star.yaml's values (svsdf_default_dynamics), then those of `base` (a Dynamics or a dict with DYNAMICS_KEYS), then kw."""
+    d = Dynamics()
+    lib().svsdf_default_dynamics(C.byref(d))
+    vals = dict(base.as_dict() if isinstance(base, Dynamics) else (base or {}))
+    vals.update(kw)
+    for k, v in vals.items():
+        if k not in DYNAMICS_KEYS:
+            raise ValueError(f"unknown dynamics key {k!r} (expected one of {DYNAMICS_KEYS})")
+        setattr(d, k, int(v) if k == "integralIntervs" else float(v))
+    return d
+
+
+def yaml_dynamics(yaml: dict) -> Dynamics:
+    """The dynamics block of a yaml dict such as scenes.YAML (its vmax, omgmax, weight_v, weight_omg, smoothingEps and
+    integralIntervs; keys it lacks keep star.yaml's values)."""
+    return dynamics({k: yaml[k] for k in DYNAMICS_KEYS if k in yaml})
+
+
+def dynamics_penalty(T, coeffs_colmajor, dyn=None, **kw):
+    """svsdf_dynamics_penalty on the host: the back end's speed and yaw-rate penalty of one trajectory (T [N], MINCO coefficients
+    18N column-major) under dynamics(dyn, **kw).  Returns (cost, gradT [N], gradC [18N column-major]), as cost_grad does."""
+    T = _f64(T).reshape(-1)
+    c = _f64(coeffs_colmajor).reshape(-1)
+    N = T.shape[0]
+    if c.shape[0] != 18 * N:
+        raise ValueError("coeffs must hold 18 N values (6N x 3 column-major)")
+    d = dynamics(dyn, **kw)
+    cost, gT, gC = np.zeros(1), np.zeros(N), np.zeros(18 * N)
+    rc = lib().svsdf_dynamics_penalty(C.byref(d), N, _p(T), _p(c), _p(cost), _p(gC), _p(gT))
+    if rc != 0:
+        raise SvsdfError(f"svsdf_dynamics_penalty: status {rc}: invalid limits or N < 1")
+    return float(cost[0]), gT, gC
 
 
 def _colmajor33(m):
@@ -620,6 +672,7 @@ class Context:
         self.h = h
         self.P = 0
         self.safety_hor = float(safety_hor)  # the penalty's horizon: plan's certification lists the cells within it
+        self.dynamics = None  # the limits set with set_dynamics (a dict with DYNAMICS_KEYS), or None
 
     def close(self):
         if getattr(self, "h", None):
@@ -661,6 +714,20 @@ class Context:
             return
         z = _scale(a, b, w, phi)
         self._ck(lib().svsdf_set_scale(self.h, C.byref(z)), "svsdf_set_scale")
+
+    def set_dynamics(self, dyn=..., **kw):
+        """Speed and yaw-rate limits for every later evaluation and optimisation of this context (svsdf_set_dynamics): e.g.
+        set_dynamics(vmax=1.0) (the other values star.yaml's), set_dynamics(yaml_dynamics(scenes.YAML)) or a dict.
+        set_dynamics(None): no dynamics penalty (the default).  Invalid limits raise and keep the previous setting."""
+        if dyn is None:
+            if kw:
+                raise ValueError("set_dynamics(None) takes no limits")
+            self._ck(lib().svsdf_set_dynamics(self.h, None), "svsdf_set_dynamics")
+            self.dynamics = None
+            return
+        d = dynamics(None if dyn is ... else dyn, **kw)
+        self._ck(lib().svsdf_set_dynamics(self.h, C.byref(d)), "svsdf_set_dynamics")
+        self.dynamics = d.as_dict()
 
     def set_traj(self, T, coeffs_colmajor):
         T = _f64(T)
@@ -1081,8 +1148,11 @@ class TrajOptimizer:
     """Mirror of the reference's TrajOptimizer for the back-end SVSDF cost (back_end_optimizer.hpp)."""
 
     def __init__(self, shape="star", poly_params=(0.0, 0.0, 0.0), weight_p=60.0, safety_hor=0.7, rho=3.8, device=0,
-                 strict_fp=True, polygon=None, mesh=None):
+                 strict_fp=True, polygon=None, mesh=None, dynamics=None):
+        """dynamics: the back end's speed and yaw-rate limits (Context.set_dynamics), or None (no dynamics penalty)."""
         self.ctx = Context(shape, poly_params, weight_p, safety_hor, rho, device, strict_fp, polygon, mesh)
+        if dynamics is not None:
+            self.ctx.set_dynamics(dynamics)
         self.sv_manager = SweptVolumeManager(self.ctx)
         self._points = None
         self.pieceN = 0
@@ -1102,6 +1172,9 @@ class TrajOptimizer:
 
     def addSaftyPenaOnSweptVolumeParallelTrueSDF(self, T, coeffs_colmajor, cost=0.0, gradT=None, gradC=None):
         return self.ctx.cost_grad(T, coeffs_colmajor, cost, gradT, gradC)
+
+    def setDynamics(self, dynamics=None):  # the vmax / omgmax / weight_v / weight_omg members of setParam (:884-896)
+        self.ctx.set_dynamics(dynamics)
 
     def setConditions(self, init_s, final_s, N):
         self.pieceN = N

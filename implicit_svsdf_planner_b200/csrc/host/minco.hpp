@@ -329,12 +329,101 @@ SVSDF_HD inline double backwardGradT(double tau, double gradT) {
     return gradT * (1.0 - tau) / (den * den);
 }
 
+// Speed and yaw-rate limits (svsdf_set_dynamics): the yaml's vmax, omgmax, weight_v, weight_omg, smoothingEps and integralIntervs.
+struct DynamicsParams {
+    double vmax, omgmax, weight_v, weight_omg, eps;
+    int res;  // integralIntervs: samples j = 0 .. res per piece
+};
+// smoothedL1 (back_end_optimizer.hpp:316-340): false below 0, the cubic on [0, mu], x - mu / 2 above
+SVSDF_HD inline bool smoothed_l1(double x, double mu, double &f, double &df) {
+    if (x < 0.0) return false;
+    if (x > mu) {
+        f = x - 0.5 * mu;
+        df = 1.0;
+        return true;
+    }
+    const double xdmu = x / mu;
+    const double sqrxdmu = xdmu * xdmu;
+    const double mumxd2 = mu - 0.5 * x;
+    f = mumxd2 * sqrxdmu * xdmu;
+    df = sqrxdmu * ((-0.5) * xdmu + 3.0 * mumxd2 / mu);
+    return true;
+}
+// The dynamics penalty: the reference's addTimeIntPenalty (back_end_optimizer.hpp:411-533) with the two violations it computes,
+// violaVel = |vel_xy|^2 - vmax^2 and violaOmg = vel_yaw^2 - omgmax^2, penalised through smoothed_l1 (the reference computes them and
+// penalises neither).  No St(t) term: the limits are on the body's path, not on its shape.  b: MINCO coefficients (6N x 3
+// column-major), T: durations.  Adds the partials to gradC (6N x 3) and gradT (N), writes each piece's cost to partial (N) and returns
+// the cost (every lane).  Per piece i: step = T_i * (1 / res) as the reference computes it; at s = j step, j = 0 .. res ascending,
+// vel = beta1(s)^T c_i and acc = beta2(s)^T c_i (each a left-to-right sum over k = 1 .. 5, resp. 2 .. 5), node = 0.5 at j = 0 and
+// j = res else 1, alpha = j * (1 / res).  A sample where neither violation is >= 0 adds nothing; otherwise gradVel = (w_v df_v 2 vel_x,
+// w_v df_v 2 vel_y, w_omg df_omg 2 vel_yaw) (a zero where its violation is below 0), pena = w_v f_v + w_omg f_omg, and
+//   gradC[d][k] += beta1_k gradVel_d node step  (k = 1 .. 5; beta1_0 = 0)
+//   gradT[i]    += (gradVel . acc) alpha node step + node (1 / res) pena
+//   partial[i]  += node step pena
+// Summation order: within a piece the samples in ascending j, into the piece's partial (from 0.0); the cost is then the sum of the
+// partials in ascending i.  One lane owns a piece's samples, so every team gives the same bits.
+template <class Team = SerialTeam>
+SVSDF_HD inline double dynamics_penalty(const DynamicsParams &p, int N, const double *T, const double *b, double *gradC, double *gradT,
+                                        double *partial, const Team &team = Team()) {
+    const int n = 6 * N, res = p.res;
+    const double velSqrMax = p.vmax * p.vmax, omgSqrMax = p.omgmax * p.omgmax, integralFrac = 1.0 / res;
+    for (int i = team.lane(); i < N; i += team.size()) {
+        const double step = T[i] * integralFrac;
+        double part = 0.0;
+        for (int j = 0; j <= res; ++j) {
+            // beta1 = (0, 1, 2 s1, 3 s2, 4 s3, 5 s4), beta2 = (0, 0, 2, 6 s1, 12 s2, 20 s3), formed where they are used
+            const double s1 = j * step, s2 = s1 * s1, s3 = s2 * s1, s4 = s2 * s2;
+            double vel[3];
+            for (int d = 0; d < 3; ++d) {
+                const double *c = b + (size_t)d * n + 6 * i;
+                vel[d] = c[1] + 2.0 * s1 * c[2] + 3.0 * s2 * c[3] + 4.0 * s3 * c[4] + 5.0 * s4 * c[5];
+            }
+            const double violaVel = vel[0] * vel[0] + vel[1] * vel[1] - velSqrMax;
+            const double violaOmg = vel[2] * vel[2] - omgSqrMax;
+            double f, df, pena = 0.0, gradVel[3] = {0.0, 0.0, 0.0};
+            bool active = false;
+            if (smoothed_l1(violaVel, p.eps, f, df)) {
+                gradVel[0] = p.weight_v * df * 2.0 * vel[0];
+                gradVel[1] = p.weight_v * df * 2.0 * vel[1];
+                pena += p.weight_v * f;
+                active = true;
+            }
+            if (smoothed_l1(violaOmg, p.eps, f, df)) {
+                gradVel[2] = p.weight_omg * df * 2.0 * vel[2];
+                pena += p.weight_omg * f;
+                active = true;
+            }
+            if (!active) continue;
+            const double node = (j == 0 || j == res) ? 0.5 : 1.0, alpha = j * integralFrac;
+            double dot = 0.0;
+            for (int d = 0; d < 3; ++d) {
+                const double *c = b + (size_t)d * n + 6 * i;
+                double *g = gradC + (size_t)d * n + 6 * i;
+                const double acc = 2.0 * c[2] + 6.0 * s1 * c[3] + 12.0 * s2 * c[4] + 20.0 * s3 * c[5];
+                dot = d == 0 ? gradVel[0] * acc : dot + gradVel[d] * acc;
+                g[1] += 1.0 * gradVel[d] * node * step;
+                g[2] += 2.0 * s1 * gradVel[d] * node * step;
+                g[3] += 3.0 * s2 * gradVel[d] * node * step;
+                g[4] += 4.0 * s3 * gradVel[d] * node * step;
+                g[5] += 5.0 * s4 * gradVel[d] * node * step;
+            }
+            gradT[i] += dot * alpha * node * step + node * integralFrac * pena;
+            part += node * step * pena;
+        }
+        partial[i] = part;
+    }
+    team.sync();
+    double cost = 0.0;
+    for (int i = 0; i < N; ++i) cost += partial[i];
+    return cost;
+}
+
 // The host half of one back-end evaluation (back_end_optimizer.hpp:353-398) on flat storage of N pieces: times, gradByTimes,
-// partialGradByTimes (N each), partialGradByCoeffs and adj (18N each), gradByPoints (3 (N - 1)).  Shared by the host evaluation
-// (svsdf_runtime.cpp: HostEval) and the device back end (svsdf_backend.cu).
+// partialGradByTimes (N each), partialGradByCoeffs and adj (18N each), gradByPoints (3 (N - 1)), dynPartial (N: the dynamics
+// penalty's per-piece costs).  Shared by the host evaluation (svsdf_runtime.cpp: HostEval) and the device back end (svsdf_backend.cu).
 struct BackendEvalView {
     MincoView m;
-    double *times, *gradByTimes, *partialGradByTimes, *partialGradByCoeffs, *gradByPoints, *adj;
+    double *times, *gradByTimes, *partialGradByTimes, *partialGradByCoeffs, *gradByPoints, *adj, *dynPartial;
 };
 // forwardT / forwardP (back_end_optimizer.hpp:353-354): tau -> T, MINCO, its energy (returned) and partial gradients
 // (every lane returns the energy)
@@ -350,11 +439,12 @@ SVSDF_HD inline double backend_forward(const BackendEvalView &E, const double *x
     team.sync();
     return energy;
 }
-// o: the device record [cost, gradC (18N), gradT (N), n_inside] of the trajectory backend_forward built; adds it, propagates through
-// MINCO and adds rho * sum(T).  Returns the cost (every lane), g the gradient w.r.t. x.
+// o: the device record [cost, gradC (18N), gradT (N), n_inside] of the trajectory backend_forward built; adds it, then the dynamics
+// penalty when dyn is not null (the reference's dyn_cost slot, back_end_optimizer.hpp:358, :387), propagates through MINCO and adds
+// rho * sum(T).  Returns the cost (every lane), g the gradient w.r.t. x.  pos_out: the safety term alone; other_out the rest.
 template <class Team = SerialTeam>
-SVSDF_HD inline double backend_backward(const BackendEvalView &E, double energy, const double *o, const double *x, double rho, double *g,
-                                        double *pos_out, double *other_out, const Team &team = Team()) {
+SVSDF_HD inline double backend_backward(const BackendEvalView &E, double energy, const double *o, const double *x, double rho,
+                                        const DynamicsParams *dyn, double *g, double *pos_out, double *other_out, const Team &team = Team()) {
     const int N = E.m.N;
     double cost = energy;
     const double energy_cost = cost;
@@ -363,6 +453,7 @@ SVSDF_HD inline double backend_backward(const BackendEvalView &E, double energy,
     for (int i = team.lane(); i < N; i += team.size()) E.partialGradByTimes[i] += o[1 + 18 * N + i];
     const double pos_cost = cost - energy_cost;
     team.sync();
+    if (dyn) cost += dynamics_penalty(*dyn, N, E.times, E.m.b, E.partialGradByCoeffs, E.partialGradByTimes, E.dynPartial, team);
     minco_propagate(E.m, E.partialGradByCoeffs, E.partialGradByTimes, E.adj, E.gradByPoints, E.gradByTimes, team);
     double tsum = 0.0;
     for (int i = 0; i < N; ++i) tsum += E.times[i];

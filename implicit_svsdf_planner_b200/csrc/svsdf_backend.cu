@@ -4,7 +4,8 @@
 // no contraction on either side, correctly rounded division and sqrt on both, so every problem gets svsdf_optimize's bits.
 //   k_backend_init:     problems enter slots; the machine starts and asks for its first evaluation
 //   k_backend_blob:     the round's trajectory blobs, byte for byte fill_blob's (the layer-1 lattice accumulated on one thread)
-//   k_backend_backward: the round's records through MINCO's adjoint into the machines, which ask for the next evaluation or finish
+//   k_backend_backward: the round's records (and the dynamics penalty, when it is on) through MINCO's adjoint into the machines,
+//                       which ask for the next evaluation or finish
 // Asking for an evaluation runs its forward half (tau -> T, MINCO, energy, partial gradients) and traj_layout's checks at once.
 #include <cmath>
 
@@ -47,6 +48,8 @@ __device__ SlotView carve(const BackendArgs &B, int s) {
     V.E.gradByPoints = p;
     p += 3 * (N - 1);
     V.E.adj = p;
+    p += 18 * N;
+    V.E.dynPartial = p;
     return V;
 }
 
@@ -174,7 +177,8 @@ __global__ void k_backend_blob(const BackendArgs B, const BackendRoundItem *item
     }
 }
 
-__global__ void __launch_bounds__(kBackendWarps * 32) k_backend_backward(const BackendArgs B, const BackendRoundItem *items, int count,
+// (kBackendWarps * 32, 1): lets ptxas hold the machine and the dynamics penalty in registers (162, no spills; three CTAs per SM)
+__global__ void __launch_bounds__(kBackendWarps * 32, 1) k_backend_backward(const BackendArgs B, const BackendRoundItem *items, int count,
                                                                          const double *records) {
     const int j = blockIdx.x * kBackendWarps + threadIdx.x / 32;
     if (j >= count) return;
@@ -187,7 +191,8 @@ __global__ void __launch_bounds__(kBackendWarps * 32) k_backend_backward(const B
     if (it.rc == 0) {
         const double *o = records + it.out_off;
         double pos = 0.0, other = 0.0;
-        f = host::backend_backward(V.E, sl.energy, o, V.L.x, B.rho, host::lbfgs_eval_grad(sl.M, V.L), &pos, &other, team);
+        f = host::backend_backward(V.E, sl.energy, o, V.L.x, B.rho, B.dyn_on ? &B.dyn : nullptr, host::lbfgs_eval_grad(sl.M, V.L), &pos,
+                                   &other, team);
         if (team.lane() == 0) {
             if (sl.good_evals++ == 0) {
                 B.result[sl.problem].f0 = f;

@@ -48,6 +48,8 @@ struct BackendRoundItem {
 struct BackendArgs {
     host::LbfgsParams P;
     double rho;
+    host::DynamicsParams dyn;     // the context's speed and yaw-rate limits (svsdf_set_dynamics), used when dyn_on
+    int dyn_on;
     int Nmax;
     int64_t slot_doubles;
     BackendSlot *slots;
@@ -61,9 +63,9 @@ struct BackendArgs {
 // Doubles of one slot's storage for trajectories of up to Nmax pieces.
 inline int64_t backend_slot_doubles(const host::LbfgsParams &P, int Nmax) {
     const int nv = 4 * Nmax - 3;
-    // lbfgs | head, tail | band | b | t | times, gradByTimes, partialGradByTimes | partialGradByCoeffs | gradByPoints | adj
+    // lbfgs | head, tail | band | b | t | times, gradByTimes, partialGradByTimes | partialGradByCoeffs | gradByPoints | adj | dynPartial
     return (int64_t)host::lbfgs_doubles(P, nv) + 18 + (int64_t)host::minco_band_doubles(Nmax) + 18 * Nmax + 5 * Nmax + 3 * Nmax +
-           18 * Nmax + 3 * (Nmax - 1) + 18 * Nmax;
+           18 * Nmax + 3 * (Nmax - 1) + 18 * Nmax + Nmax;
 }
 
 // launchers (svsdf_backend.cu).  init: problems enter slots (pairs [slot, problem]); blob: the round's blobs; backward: the round's

@@ -41,11 +41,11 @@ using namespace svsdf;
 
 // The host half of one back-end evaluation (back_end_optimizer.hpp:353-398), shared by svsdf_evaluate and the lock-step back end
 // (svsdf_optimize_lockstep).  forward(): tau -> T and MINCO (coefficients, energy and its partial gradients), before the device
-// evaluation; backward(): adds the device record, propagates through MINCO and adds rho * sum(T).
+// evaluation; backward(): adds the device record and the dynamics penalty (dyn not null), propagates through MINCO and adds rho * sum(T).
 struct HostEval {
     host::MincoS3NU minco;
     int N = 0;
-    std::vector<double> times, gradByTimes, partialGradByTimes, partialGradByCoeffs, gradByPoints, adj;
+    std::vector<double> times, gradByTimes, partialGradByTimes, partialGradByCoeffs, gradByPoints, adj, dynPartial;
     double energy = 0.0;
 
     void setup(const double *initS, const double *finalS, int n_pieces) {
@@ -57,15 +57,17 @@ struct HostEval {
         partialGradByCoeffs.assign((size_t)18 * N, 0.0);
         gradByPoints.assign((size_t)3 * (N - 1), 0.0);
         adj.assign((size_t)18 * N, 0.0);
+        dynPartial.assign(N, 0.0);
     }
     host::BackendEvalView view() {
         return host::BackendEvalView{minco.view(),           times.data(),        gradByTimes.data(), partialGradByTimes.data(),
-                                     partialGradByCoeffs.data(), gradByPoints.data(), adj.data()};
+                                     partialGradByCoeffs.data(), gradByPoints.data(), adj.data(), dynPartial.data()};
     }
     void forward(const double *x) { energy = host::backend_forward(view(), x); }
     // o: the device record [cost, gradC (18N), gradT (N), n_inside] of the trajectory forward() built
-    double backward(const double *o, const double *x, double rho, double *g, double *pos_out, double *other_out) {
-        return host::backend_backward(view(), energy, o, x, rho, g, pos_out, other_out);
+    double backward(const double *o, const double *x, double rho, const host::DynamicsParams *dyn, double *g, double *pos_out,
+                    double *other_out) {
+        return host::backend_backward(view(), energy, o, x, rho, dyn, g, pos_out, other_out);
     }
     // The final trajectory from the solver's returned iterate x (optimize_traj_lmbm does the same on success and failure,
     // back_end_optimizer.cpp:44-94) and the run's statistics.
@@ -230,6 +232,10 @@ struct svsdf_ctx {
     bool have_boundary = false;
     double cost_pos = 0, cost_other = 0, cost_total = 0;
     int n_evaluate = 0;
+    // speed and yaw-rate limits (svsdf_set_dynamics): every back-end evaluation of this context adds their penalty when dyn_on
+    bool dyn_on = false;
+    host::DynamicsParams dyn{};
+    const host::DynamicsParams *dynamics() const { return dyn_on ? &dyn : nullptr; }
     double gpu_ms_total = 0.0;
     bool time_kernels = false;
     int last_status = 0;
@@ -708,7 +714,7 @@ double evaluate_impl(svsdf_ctx *ctx, const double *x, double *g, int n) {
         ctx->last_status = rc;
         return NAN;
     }
-    const double cost = ctx->he.backward(ctx->h_out, x, ctx->rho, g, &ctx->cost_pos, &ctx->cost_other);
+    const double cost = ctx->he.backward(ctx->h_out, x, ctx->rho, ctx->dynamics(), g, &ctx->cost_pos, &ctx->cost_other);
     ctx->cost_total = cost;
     ctx->last_status = SVSDF_OK;
     return cost;
@@ -1758,6 +1764,52 @@ int svsdf_set_scale(svsdf_ctx *ctx, const svsdf_scale *scale) {
     return SVSDF_OK;
 }
 
+static bool dynamics_valid(const svsdf_dynamics &d) {
+    const double v[5] = {d.vmax, d.omgmax, d.weight_v, d.weight_omg, d.smoothingEps};
+    for (double e : v)
+        if (!std::isfinite(e)) return false;
+    return d.vmax > 0.0 && d.omgmax > 0.0 && d.weight_v >= 0.0 && d.weight_omg >= 0.0 && d.smoothingEps > 0.0 && d.integralIntervs >= 1 &&
+           d.integralIntervs <= 64;
+}
+static host::DynamicsParams to_host_dynamics(const svsdf_dynamics &d) {
+    host::DynamicsParams p;
+    p.vmax = d.vmax; p.omgmax = d.omgmax; p.weight_v = d.weight_v; p.weight_omg = d.weight_omg; p.eps = d.smoothingEps;
+    p.res = d.integralIntervs;
+    return p;
+}
+
+void svsdf_default_dynamics(svsdf_dynamics *dyn) {
+    if (!dyn) return;
+    dyn->vmax = 10.0; dyn->omgmax = 10.0; dyn->weight_v = 10.0; dyn->weight_omg = 10.0; dyn->smoothingEps = 1.0e-2;
+    dyn->integralIntervs = 4;
+}
+
+int svsdf_set_dynamics(svsdf_ctx *ctx, const svsdf_dynamics *dyn) {
+    if (!ctx) return SVSDF_ERR_INVALID;
+    if (!dyn) {
+        ctx->dyn_on = false;
+        return SVSDF_OK;
+    }
+    if (!dynamics_valid(*dyn)) {
+        ctx->err = "svsdf_set_dynamics: needs finite values, vmax > 0, omgmax > 0, weights >= 0, smoothingEps > 0 and 1 <= integralIntervs <= 64";
+        return SVSDF_ERR_INVALID;
+    }
+    ctx->dyn = to_host_dynamics(*dyn);
+    ctx->dyn_on = true;
+    return SVSDF_OK;
+}
+
+int svsdf_dynamics_penalty(const svsdf_dynamics *dyn, int N, const double *T, const double *coeffs, double *cost, double *gradC,
+                           double *gradT) {
+    if (!dyn || !dynamics_valid(*dyn) || N < 1 || !T || !coeffs || !cost || !gradC || !gradT) return SVSDF_ERR_INVALID;
+    std::vector<double> gc((size_t)18 * N, 0.0), gt(N, 0.0), partial(N, 0.0);
+    const double c = host::dynamics_penalty(to_host_dynamics(*dyn), N, T, coeffs, gc.data(), gt.data(), partial.data());
+    *cost = c;
+    std::memcpy(gradC, gc.data(), sizeof(double) * 18 * N);
+    std::memcpy(gradT, gt.data(), sizeof(double) * N);
+    return SVSDF_OK;
+}
+
 int svsdf_scale_matrix(const svsdf_scale *scale, double t, double S_out[9], double Sinv_out[9]) {
     if (!scale || !scale_valid(*scale) || !std::isfinite(t)) return SVSDF_ERR_INVALID;
     // the arithmetic of scale_inv (svsdf_kernels.cuh) and Eigen 3.3's size-3 inverse of diag(sx, sy, 1)
@@ -2612,7 +2664,7 @@ static double lockstep_evaluate(void *inst, const double *x, double *g, const in
         return NAN;
     }
     double pos = 0.0, other = 0.0;
-    const double cost = s.he.backward(s.out.data(), x, s.ctx->rho, g, &pos, &other);
+    const double cost = s.he.backward(s.out.data(), x, s.ctx->rho, s.ctx->dynamics(), g, &pos, &other);
     if (s.evals++ == 0 && s.pr->f0_out) *s.pr->f0_out = cost;
     s.last_status = SVSDF_OK;
     return cost;
@@ -2814,6 +2866,8 @@ int svsdf_optimize_device(svsdf_ctx *ctx, const svsdf_lockstep_problem *problems
     std::memset(&B, 0, sizeof(B));
     B.P = hp;
     B.rho = ctx->rho;
+    B.dyn_on = ctx->dyn_on ? 1 : 0;
+    B.dyn = ctx->dyn;
     B.Nmax = Nmax;
     B.slot_doubles = slot_doubles;
     B.slots = ctx->d_be_slots;

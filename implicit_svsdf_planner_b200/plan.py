@@ -81,7 +81,8 @@ def generate_traj(ctx: "api.Context", cmap: CloudMap, start_xy, goal_xy, kernel_
     """generatePath + generateTraj for one start / goal on the map `cmap` (the context's shape is the robot).  certify=True adds
     `clearance` (see certificate) to a result that reached the back end.  repair=R > 0 (implies certify) then runs up to R repair rounds
     (see Repair): the top-level trajectory keys and `clearance` describe the final trajectory, `repair` what the rounds did, and
-    the context's resident points are the last query set."""
+    the context's resident points are the last query set.  When the context has dynamics set (Context.set_dynamics), the back end
+    penalises them and a result that reached it gains `dynamics` (dynamics_report of the final trajectory)."""
     X, Y, Z = cmap.occ.shape
     res = cmap.res
     ctx.set_map3d(pack_map_kernel3d(cmap.occ, kernel_size), X, Y, Z, kernel_size, cmap.boundary_min, res)
@@ -119,7 +120,34 @@ def generate_traj(ctx: "api.Context", cmap: CloudMap, start_xy, goal_xy, kernel_
         out["clearance"], out["repair"] = certificate_of(cl), rp.summary()
     elif certify:
         out["clearance"] = certificate(ctx, T, b)
+    if ctx.dynamics is not None:
+        out["dynamics"] = dynamics_report(ctx.dynamics, T, b)
     return out
+
+
+# samples per piece of dynamics_report's lattice
+DYNAMICS_SAMPLES = 1000
+
+
+def sampled_rates(T, coeffs, samples: int = DYNAMICS_SAMPLES):
+    """The body's speed |v_xy| and yaw rate at `samples` evenly spaced times s = T_i k / (samples - 1), k = 0 .. samples - 1, of every
+    piece (coeffs: MINCO b, 18N column-major).  Returns (s, speed, yaw_rate), each [N, samples]."""
+    T = np.asarray(T, dtype=np.float64).reshape(-1)
+    N = T.shape[0]
+    c = np.asarray(coeffs, dtype=np.float64).reshape(3, N, 6)  # [dim, piece, power]
+    s = T[:, None] * (np.arange(samples) / (samples - 1))[None, :]
+    k = np.arange(1, 6)
+    pw = k[None, None, :] * s[:, :, None] ** (k - 1)[None, None, :]  # d/ds s^k
+    vel = np.einsum("nmk,dnk->dnm", pw, c[:, :, 1:])
+    return s, np.hypot(vel[0], vel[1]), vel[2]
+
+
+def dynamics_report(dyn: dict, T, coeffs) -> dict:
+    """The peaks of a trajectory's speed and |yaw rate| on sampled_rates' lattice (sampled: a peak between two samples can be missed)
+    and within_limits = v_peak <= vmax and omg_peak <= omgmax.  The back end's penalty is soft, so a plan can exceed its limits."""
+    _, v, w = sampled_rates(T, coeffs)
+    v_peak, omg_peak = float(v.max()), float(np.abs(w).max())
+    return dict(v_peak=v_peak, omg_peak=omg_peak, within_limits=bool(v_peak <= dyn["vmax"] and omg_peak <= dyn["omgmax"]))
 
 
 def _xy(points) -> np.ndarray:
@@ -217,6 +245,8 @@ def plan_batch(ctx: "api.Context", cmap: CloudMap, starts, goals, kernel_size: i
     a failed problem has ok=False and the reason (an exception of one problem's extraction or mid end fails that problem only).
     stats (optional dict) receives the wall seconds of each stage, the back end's rounds and its kernel launches.  back_end=False stops
     before the back end: the problems that would enter it are returned with its inputs (init_s, final_s, x0, points) instead.
+    When the context has dynamics set (Context.set_dynamics), every problem that went through the back end also gains generate_traj's
+    `dynamics` (dynamics_report of its final trajectory).
     certify=True adds generate_traj's `clearance` to every problem that went through the back end (one svsdf_map_clearance_multi for
     all of them, after the back end; stats then also holds its wall seconds, certify_s).  repair=R > 0 (implies certify) adds
     generate_traj(repair=R)'s keys and bits: each round is one lock-step back end over the problems that gained cells and one
@@ -326,6 +356,10 @@ def plan_batch(ctx: "api.Context", cmap: CloudMap, starts, goals, kernel_size: i
                 stats.update(repair_s=time.perf_counter() - t6, repair_rounds=n_rounds)
         for q, c in final.items():
             out[q]["clearance"] = certificate_of(c)
+    if ctx.dynamics is not None:
+        for p in back:
+            r = out[p["q"]]
+            r["dynamics"] = dynamics_report(ctx.dynamics, r["T"], r["coeffs"])
     return out
 
 

@@ -25,7 +25,9 @@ START_GOAL = {
 }
 
 # src/plan_manager/config/star.yaml
-YAML = dict(weight_p=60.0, safety_hor=0.7, rho=3.8, inittime=2.5, kernel_size=17, occupancy_resolution=1.0)
+YAML = dict(weight_p=60.0, safety_hor=0.7, rho=3.8, inittime=2.5, kernel_size=17, occupancy_resolution=1.0,
+            # the back end's speed and yaw-rate limits (api.yaml_dynamics; off unless a context sets them)
+            vmax=10.0, omgmax=10.0, weight_v=10.0, weight_omg=10.0, smoothingEps=1.0e-2, integralIntervs=4)
 
 SEED_TRAJ = 20240501
 SEED_MAP = 20240502

@@ -124,6 +124,31 @@ int svsdf_set_scale(svsdf_ctx *ctx, const svsdf_scale *scale);
  * Either output may be NULL.  No context and no GPU needed. */
 int svsdf_scale_matrix(const svsdf_scale *scale, double t, double S_out[9], double Sinv_out[9]);
 
+/* ---- Speed and yaw-rate limits: the back end's dynamics penalty ------------------------------------------------------------
+ * The yaml's back-end limits (vmax, omgmax, weight_v, weight_omg, smoothingEps, integralIntervs), which the reference reads
+ * (back_end_optimizer.hpp:72-79, :884-896) and never penalises: addTimeIntPenalty (:411-533) computes violaVel = |vel_xy|^2 - vmax^2
+ * and violaOmg = vel_yaw^2 - omgmax^2, and nothing uses them.  Here the penalty fills the callback's dyn_cost slot (:358, :387):
+ *   cost = sum over pieces i and samples j = 0 .. integralIntervs of node step (weight_v smoothedL1(violaVel) + weight_omg
+ *          smoothedL1(violaOmg)), node = 1/2 at both ends of a piece, step = T_i / integralIntervs; smoothedL1 as :316-340.
+ * The exact arithmetic and summation order are those of host::dynamics_penalty (csrc/host/minco.hpp).  The penalty is soft. */
+typedef struct {
+    double vmax, omgmax, weight_v, weight_omg, smoothingEps;
+    int integralIntervs;
+} svsdf_dynamics;
+/* star.yaml's values: vmax 10, omgmax 10, weight_v 10, weight_omg 10, smoothingEps 1e-2, integralIntervs 4. */
+void svsdf_default_dynamics(svsdf_dynamics *dyn);
+/* NULL: no dynamics penalty (the default).  Otherwise every later svsdf_evaluate, svsdf_optimize, svsdf_optimize_batch (each context
+ * of the pool with its own setting), svsdf_optimize_lockstep and svsdf_optimize_device of this context adds the penalty after the
+ * safety term and before the MINCO adjoint and rho * sum(T); svsdf_last_costs counts it in cost_other.  The limits are copied.
+ * Returns SVSDF_ERR_INVALID, and keeps the previous setting, for a non-finite value, vmax or omgmax <= 0, a negative weight,
+ * smoothingEps <= 0 or integralIntervs outside 1 .. 64. */
+int svsdf_set_dynamics(svsdf_ctx *ctx, const svsdf_dynamics *dyn);
+/* The penalty of one trajectory (N >= 1 pieces, T[N], coeffs: MINCO b, 6N x 3 column-major) on the host: writes (not adds) the cost,
+ * gradC[18N] (column-major like coeffs) and gradT[N], with the bits both back ends add.  No context and no GPU needed.  Returns
+ * SVSDF_ERR_INVALID, writing nothing, for invalid limits (as svsdf_set_dynamics), N < 1 or a NULL pointer. */
+int svsdf_dynamics_penalty(const svsdf_dynamics *dyn, int N, const double *T, const double *coeffs, double *cost, double *gradC,
+                           double *gradT);
+
 /* ---- Swept-volume outline and mesh: the planner's own field contoured on the GPU ---------------------------------------------
  * svsdf_swept_contour meshes the level set f(p) = iso of f = getSDFofSweptVolume<false,true> (exactly what svsdf_query(...,
  * outer_only = 1) returns, bit for bit per point) on the z = 0 plane, for the trajectory (N, T, coeffs) as svsdf_query takes it and

@@ -253,6 +253,9 @@ class TrajOptimizer {
         if (svsdf_last_costs(obj.sv_manager->handle(), c3) == SVSDF_OK) { obj.cost_pos = c3[0]; obj.cost_other = c3[1]; obj.cost_total = c3[2]; }
         return f;
     }
+    // the vmax / omgmax / weight_v / weight_omg / smoothingEps / integralIntervs members setParam reads (:884-896), penalised in the
+    // callback's dyn_cost slot (svsdf_set_dynamics; nullptr: no dynamics penalty, the default)
+    int setDynamics(const svsdf_dynamics *dyn) { return svsdf_set_dynamics(sv_manager->handle(), dyn); }
     int setConditions(const double *initS, const double *finalS, int N) {
         pieceN = N; temporalDim = N; spatialDim = 3 * (N - 1);
         return svsdf_set_boundary(sv_manager->handle(), initS, finalS, N);
