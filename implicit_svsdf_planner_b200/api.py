@@ -243,6 +243,7 @@ EXPORTED_SYMBOLS = [
     "svsdf_cost_grad_multi", "svsdf_optimize_lockstep", "svsdf_lockstep_rounds", "svsdf_optimize_device", "svsdf_round_times", "svsdf_swept_contour", "svsdf_swept_free",
     "svsdf_map_clearance", "svsdf_clearance_free", "svsdf_map_clearance_multi",
     "svsdf_default_dynamics", "svsdf_set_dynamics", "svsdf_dynamics_penalty",
+    "svsdf_default_pose_penalty", "svsdf_set_pose_penalty", "svsdf_pose_penalty_eval",
 ]
 
 
@@ -323,6 +324,10 @@ def lib():
     L.svsdf_default_dynamics.restype = None
     L.svsdf_set_dynamics.argtypes = [vp, C.POINTER(Dynamics)]
     L.svsdf_dynamics_penalty.argtypes = [C.POINTER(Dynamics), C.c_int, dp, dp, dp, dp, dp]
+    L.svsdf_default_pose_penalty.argtypes = [C.POINTER(PosePenalty)]
+    L.svsdf_default_pose_penalty.restype = None
+    L.svsdf_set_pose_penalty.argtypes = [vp, C.POINTER(PosePenalty)]
+    L.svsdf_pose_penalty_eval.argtypes = [vp, C.c_int, dp, dp, C.POINTER(PosePenalty), dp, dp, dp, dp]
     L.svsdf_cost_grad_multi.argtypes = [vp, C.c_int, C.POINTER(MultiProblem)]
     L.svsdf_optimize_lockstep.argtypes = [vp, C.POINTER(LockstepProblem), C.c_int, C.POINTER(LbfgsParams), C.c_int, C.POINTER(OptStats),
                                           C.POINTER(C.c_int)]
@@ -424,6 +429,49 @@ def dynamics_penalty(T, coeffs_colmajor, dyn=None, **kw):
     if rc != 0:
         raise SvsdfError(f"svsdf_dynamics_penalty: status {rc}: invalid limits or N < 1")
     return float(cost[0]), gT, gC
+
+
+class PosePenalty(C.Structure):
+    """svsdf_pose_penalty: the pose-sampled obstacle penalty's weight, samples per piece and gather box (svsdf_set_pose_penalty)."""
+    _fields_ = [("weight", C.c_double), ("integralIntervs", C.c_int), ("half", C.c_double * 3)]
+
+    def as_dict(self) -> dict:
+        return {"weight": self.weight, "integralIntervs": self.integralIntervs, "half": tuple(self.half)}
+
+
+POSE_PENALTY_KEYS = ("weight", "integralIntervs", "half")
+
+
+def pose_penalty(base=None, **kw) -> PosePenalty:
+    """A PosePenalty: star.yaml's values (svsdf_default_pose_penalty), then those of `base` (a PosePenalty or a dict with
+    POSE_PENALTY_KEYS), then kw.  half: one value for all three axes or three values."""
+    p = PosePenalty()
+    lib().svsdf_default_pose_penalty(C.byref(p))
+    vals = dict(base.as_dict() if isinstance(base, PosePenalty) else (base or {}))
+    vals.update(kw)
+    for k, v in vals.items():
+        if k not in POSE_PENALTY_KEYS:
+            raise ValueError(f"unknown pose penalty key {k!r} (expected one of {POSE_PENALTY_KEYS})")
+        if k == "half":
+            h = np.broadcast_to(np.asarray(v, dtype=np.float64), (3,))
+            for a in range(3):
+                p.half[a] = float(h[a])
+        else:
+            setattr(p, k, int(v) if k == "integralIntervs" else float(v))
+    return p
+
+
+def yaml_pose_penalty(yaml: dict) -> PosePenalty:
+    """The pose penalty of a yaml dict such as scenes.YAML: weight_p, integralIntervs and the gather box half size
+    kernel_size * occupancy_resolution / 2 (back_end_optimizer.hpp:898); keys it lacks keep star.yaml's values."""
+    vals = {}
+    if "weight_p" in yaml:
+        vals["weight"] = yaml["weight_p"]
+    if "integralIntervs" in yaml:
+        vals["integralIntervs"] = yaml["integralIntervs"]
+    if "kernel_size" in yaml and "occupancy_resolution" in yaml:
+        vals["half"] = yaml["kernel_size"] * yaml["occupancy_resolution"] / 2
+    return pose_penalty(vals)
 
 
 def _colmajor33(m):
@@ -673,6 +721,7 @@ class Context:
         self.P = 0
         self.safety_hor = float(safety_hor)  # the penalty's horizon: plan's certification lists the cells within it
         self.dynamics = None  # the limits set with set_dynamics (a dict with DYNAMICS_KEYS), or None
+        self.pose = None  # the pose penalty set with set_pose_penalty (a dict with POSE_PENALTY_KEYS), or None
 
     def close(self):
         if getattr(self, "h", None):
@@ -728,6 +777,40 @@ class Context:
         d = dynamics(None if dyn is ... else dyn, **kw)
         self._ck(lib().svsdf_set_dynamics(self.h, C.byref(d)), "svsdf_set_dynamics")
         self.dynamics = d.as_dict()
+
+    def set_pose_penalty(self, p=..., **kw):
+        """The pose-sampled obstacle penalty for every later evaluation and optimisation of this context (svsdf_set_pose_penalty):
+        e.g. set_pose_penalty() (star.yaml's values), set_pose_penalty(integralIntervs=16), set_pose_penalty(yaml_pose_penalty(
+        scenes.YAML)) or a dict.  It needs a 3-D map (set_map3d).  set_pose_penalty(None): no pose penalty (the default).  Invalid
+        values raise and keep the previous setting."""
+        if p is None:
+            if kw:
+                raise ValueError("set_pose_penalty(None) takes no values")
+            self._ck(lib().svsdf_set_pose_penalty(self.h, None), "svsdf_set_pose_penalty")
+            self.pose = None
+            return
+        q = pose_penalty(None if p is ... else p, **kw)
+        self._ck(lib().svsdf_set_pose_penalty(self.h, C.byref(q)), "svsdf_set_pose_penalty")
+        self.pose = q.as_dict()
+
+    def pose_penalty(self, T, coeffs_colmajor, p=None, samples=False, **kw):
+        """svsdf_pose_penalty_eval: the pose penalty of one trajectory against this context's 3-D map, on the device.  p (and kw):
+        the penalty's values as pose_penalty() takes them; by default the context's setting (star.yaml's values when none is set).
+        Returns (cost, gradT [N], gradC [18N column-major]), and with samples=True also the raw grad_cost_p records
+        [N (integralIntervs + 1), 4] (costp, gradp_x, gradp_y, grad_yaw), piece by piece."""
+        T = _f64(T).reshape(-1)
+        c = _f64(coeffs_colmajor).reshape(-1)
+        N = T.shape[0]
+        if c.shape[0] != 18 * N:
+            raise ValueError("coeffs must hold 18 N values (6N x 3 column-major)")
+        q = pose_penalty(self.pose if p is None else p, **kw)
+        cost, gT, gC = np.zeros(1), np.zeros(N), np.zeros(18 * N)
+        rec = np.zeros((N * (q.integralIntervs + 1), 4)) if samples else None
+        self._ck(lib().svsdf_pose_penalty_eval(self.h, N, _p(T), _p(c), C.byref(q), _p(cost), _p(gC), _p(gT),
+                                               _p(rec) if samples else None), "svsdf_pose_penalty_eval")
+        if samples:
+            return float(cost[0]), gT, gC, rec
+        return float(cost[0]), gT, gC
 
     def set_traj(self, T, coeffs_colmajor):
         T = _f64(T)
@@ -1148,11 +1231,14 @@ class TrajOptimizer:
     """Mirror of the reference's TrajOptimizer for the back-end SVSDF cost (back_end_optimizer.hpp)."""
 
     def __init__(self, shape="star", poly_params=(0.0, 0.0, 0.0), weight_p=60.0, safety_hor=0.7, rho=3.8, device=0,
-                 strict_fp=True, polygon=None, mesh=None, dynamics=None):
-        """dynamics: the back end's speed and yaw-rate limits (Context.set_dynamics), or None (no dynamics penalty)."""
+                 strict_fp=True, polygon=None, mesh=None, dynamics=None, pose_penalty=None):
+        """dynamics: the back end's speed and yaw-rate limits (Context.set_dynamics), or None (no dynamics penalty).  pose_penalty:
+        the pose-sampled obstacle penalty (Context.set_pose_penalty; a dict, a PosePenalty or {} for star.yaml's values), or None."""
         self.ctx = Context(shape, poly_params, weight_p, safety_hor, rho, device, strict_fp, polygon, mesh)
         if dynamics is not None:
             self.ctx.set_dynamics(dynamics)
+        if pose_penalty is not None:
+            self.ctx.set_pose_penalty(pose_penalty)
         self.sv_manager = SweptVolumeManager(self.ctx)
         self._points = None
         self.pieceN = 0
@@ -1175,6 +1261,13 @@ class TrajOptimizer:
 
     def setDynamics(self, dynamics=None):  # the vmax / omgmax / weight_v / weight_omg members of setParam (:884-896)
         self.ctx.set_dynamics(dynamics)
+
+    def setPosePenalty(self, pose_penalty=None):  # weight_p, integralIntervs and bdx / bdy / bdz of setParam (:884-898)
+        self.ctx.set_pose_penalty(pose_penalty)
+
+    def addTimeIntPenalty(self, T, coeffs_colmajor, p=None, **kw):
+        """The pose-sampled obstacle term of addTimeIntPenalty (back_end_optimizer.hpp:411-533) on the device: Context.pose_penalty."""
+        return self.ctx.pose_penalty(T, coeffs_colmajor, p, **kw)
 
     def setConditions(self, init_s, final_s, N):
         self.pieceN = N

@@ -39,6 +39,9 @@ UNITS = [
     ("svsdf_swept.cu", "svsdf_swept.o", ["-fmad=false"]),  # swept-volume mesher: vertices independent of the field's build
     ("svsdf_clearance.cu", "svsdf_clearance.o", ["-fmad=false"]),  # map clearance: cell centres round like svsdf_extract's
     ("svsdf_backend.cu", "svsdf_backend.o", ["-fmad=false"]),  # device L-BFGS / MINCO: the host unit's bits (it has -ffp-contract=off)
+    # the pose-sampled obstacle penalty (svsdf_set_pose_penalty), fast and strict
+    ("svsdf_pose.cu", "svsdf_pose_fast.o", ["-DSVSDF_NS=fast"]),
+    ("svsdf_pose.cu", "svsdf_pose_strict.o", ["-DSVSDF_NS=strict", "-fmad=false"]),
     # host threads for the batch A* bookkeeping; no a*b+c contraction in the float winding-number builder (host/fwn_bvh.hpp)
     ("svsdf_runtime.cpp", "svsdf_runtime.o", ["-Xcompiler", "-fopenmp", "-Xcompiler", "-ffp-contract=off"]),
 ]

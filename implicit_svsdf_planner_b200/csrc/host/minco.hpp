@@ -418,9 +418,62 @@ SVSDF_HD inline double dynamics_penalty(const DynamicsParams &p, int N, const do
     return cost;
 }
 
+// The pose-sampled obstacle penalty (svsdf_set_pose_penalty): weight_p and integralIntervs of addTimeIntPenalty's grad_cost_p term.
+struct PoseParams {
+    double weight;
+    int res;  // integralIntervs: samples j = 0 .. res per piece
+};
+// The chain rule of the pose penalty: addTimeIntPenalty's (back_end_optimizer.hpp:411-533) use of grad_cost_p (:956-1028), which the
+// reference computes and never applies.  rec: the per-sample records (costp, gradp_x, gradp_y, grad_yaw) the pose kernel wrote
+// (svsdf_pose.cu), N (res + 1) of them, piece-major.  b, T, gradC, gradT, partial and the return value as dynamics_penalty's; step,
+// s, node and alpha too.  A sample is active when costp > 0; then gP = weight (gradp_x, gradp_y, grad_yaw), pena = weight costp, and
+//   gradC[d][k] += beta0_k gP_d node step  (beta0 = (1, s, s^2, .., s^5))
+//   gradT[i]    += (gP . vel) alpha node step + node (1 / res) pena,  vel = beta1(s)^T c_i
+//   partial[i]  += node step pena
+// An inactive sample adds nothing.  Summation order as dynamics_penalty's: one lane owns a piece, its samples in ascending j, then the
+// partials in ascending i.
+template <class Team = SerialTeam>
+SVSDF_HD inline double pose_penalty(const PoseParams &p, int N, const double *T, const double *b, const double *rec, double *gradC,
+                                    double *gradT, double *partial, const Team &team = Team()) {
+    const int n = 6 * N, res = p.res;
+    const double integralFrac = 1.0 / res;
+    for (int i = team.lane(); i < N; i += team.size()) {
+        const double step = T[i] * integralFrac;
+        double part = 0.0;
+        for (int j = 0; j <= res; ++j) {
+            const double *r = rec + 4 * ((size_t)i * (res + 1) + j);
+            if (!(r[0] > 0.0)) continue;
+            const double gP[3] = {p.weight * r[1], p.weight * r[2], p.weight * r[3]}, pena = p.weight * r[0];
+            const double s1 = j * step, s2 = s1 * s1, s3 = s2 * s1, s4 = s2 * s2, s5 = s4 * s1;
+            const double node = (j == 0 || j == res) ? 0.5 : 1.0, alpha = j * integralFrac;
+            double dot = 0.0;
+            for (int d = 0; d < 3; ++d) {
+                const double *c = b + (size_t)d * n + 6 * i;
+                double *g = gradC + (size_t)d * n + 6 * i;
+                const double vel = c[1] + 2.0 * s1 * c[2] + 3.0 * s2 * c[3] + 4.0 * s3 * c[4] + 5.0 * s4 * c[5];
+                dot = d == 0 ? gP[0] * vel : dot + gP[d] * vel;
+                g[0] += 1.0 * gP[d] * node * step;
+                g[1] += s1 * gP[d] * node * step;
+                g[2] += s2 * gP[d] * node * step;
+                g[3] += s3 * gP[d] * node * step;
+                g[4] += s4 * gP[d] * node * step;
+                g[5] += s5 * gP[d] * node * step;
+            }
+            gradT[i] += dot * alpha * node * step + node * integralFrac * pena;
+            part += node * step * pena;
+        }
+        partial[i] = part;
+    }
+    team.sync();
+    double cost = 0.0;
+    for (int i = 0; i < N; ++i) cost += partial[i];
+    return cost;
+}
+
 // The host half of one back-end evaluation (back_end_optimizer.hpp:353-398) on flat storage of N pieces: times, gradByTimes,
-// partialGradByTimes (N each), partialGradByCoeffs and adj (18N each), gradByPoints (3 (N - 1)), dynPartial (N: the dynamics
-// penalty's per-piece costs).  Shared by the host evaluation (svsdf_runtime.cpp: HostEval) and the device back end (svsdf_backend.cu).
+// partialGradByTimes (N each), partialGradByCoeffs and adj (18N each), gradByPoints (3 (N - 1)), dynPartial (N: the pose and the
+// dynamics penalties' per-piece costs, one penalty after the other).  Shared by the host evaluation (svsdf_runtime.cpp: HostEval) and
+// the device back end (svsdf_backend.cu).
 struct BackendEvalView {
     MincoView m;
     double *times, *gradByTimes, *partialGradByTimes, *partialGradByCoeffs, *gradByPoints, *adj, *dynPartial;
@@ -439,20 +492,26 @@ SVSDF_HD inline double backend_forward(const BackendEvalView &E, const double *x
     team.sync();
     return energy;
 }
-// o: the device record [cost, gradC (18N), gradT (N), n_inside] of the trajectory backend_forward built; adds it, then the dynamics
-// penalty when dyn is not null (the reference's dyn_cost slot, back_end_optimizer.hpp:358, :387), propagates through MINCO and adds
-// rho * sum(T).  Returns the cost (every lane), g the gradient w.r.t. x.  pos_out: the safety term alone; other_out the rest.
+// o: the device record [cost, gradC (18N), gradT (N), n_inside] of the trajectory backend_forward built; adds it, then the pose penalty
+// when pose is not null (pose_rec: its sample records), then the dynamics penalty when dyn is not null (the reference's dyn_cost slot,
+// back_end_optimizer.hpp:358, :387), propagates through MINCO and adds rho * sum(T).  Returns the cost (every lane), g the gradient
+// w.r.t. x.  pos_out: the safety term and the pose penalty; other_out the rest.
 template <class Team = SerialTeam>
 SVSDF_HD inline double backend_backward(const BackendEvalView &E, double energy, const double *o, const double *x, double rho,
-                                        const DynamicsParams *dyn, double *g, double *pos_out, double *other_out, const Team &team = Team()) {
+                                        const PoseParams *pose, const double *pose_rec, const DynamicsParams *dyn, double *g, double *pos_out,
+                                        double *other_out, const Team &team = Team()) {
     const int N = E.m.N;
     double cost = energy;
     const double energy_cost = cost;
     cost += o[0];
     for (int e = team.lane(); e < 18 * N; e += team.size()) E.partialGradByCoeffs[e] += o[1 + e];
     for (int i = team.lane(); i < N; i += team.size()) E.partialGradByTimes[i] += o[1 + 18 * N + i];
-    const double pos_cost = cost - energy_cost;
     team.sync();
+    if (pose) {
+        cost += pose_penalty(*pose, N, E.times, E.m.b, pose_rec, E.partialGradByCoeffs, E.partialGradByTimes, E.dynPartial, team);
+        team.sync();  // every lane has read the partials before the dynamics penalty rewrites them
+    }
+    const double pos_cost = cost - energy_cost;
     if (dyn) cost += dynamics_penalty(*dyn, N, E.times, E.m.b, E.partialGradByCoeffs, E.partialGradByTimes, E.dynPartial, team);
     minco_propagate(E.m, E.partialGradByCoeffs, E.partialGradByTimes, E.adj, E.gradByPoints, E.gradByTimes, team);
     double tsum = 0.0;

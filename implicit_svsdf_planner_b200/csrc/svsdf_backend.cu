@@ -4,8 +4,8 @@
 // no contraction on either side, correctly rounded division and sqrt on both, so every problem gets svsdf_optimize's bits.
 //   k_backend_init:     problems enter slots; the machine starts and asks for its first evaluation
 //   k_backend_blob:     the round's trajectory blobs, byte for byte fill_blob's (the layer-1 lattice accumulated on one thread)
-//   k_backend_backward: the round's records (and the dynamics penalty, when it is on) through MINCO's adjoint into the machines,
-//                       which ask for the next evaluation or finish
+//   k_backend_backward: the round's records (and the pose and dynamics penalties, when they are on) through MINCO's adjoint into the
+//                       machines, which ask for the next evaluation or finish
 // Asking for an evaluation runs its forward half (tau -> T, MINCO, energy, partial gradients) and traj_layout's checks at once.
 #include <cmath>
 
@@ -191,8 +191,9 @@ __global__ void __launch_bounds__(kBackendWarps * 32, 1) k_backend_backward(cons
     if (it.rc == 0) {
         const double *o = records + it.out_off;
         double pos = 0.0, other = 0.0;
-        f = host::backend_backward(V.E, sl.energy, o, V.L.x, B.rho, B.dyn_on ? &B.dyn : nullptr, host::lbfgs_eval_grad(sl.M, V.L), &pos,
-                                   &other, team);
+        const double *pose_rec = B.pose_on ? B.pose_rec + 4 * it.pose_off : nullptr;
+        f = host::backend_backward(V.E, sl.energy, o, V.L.x, B.rho, B.pose_on ? &B.pose : nullptr, pose_rec, B.dyn_on ? &B.dyn : nullptr,
+                                   host::lbfgs_eval_grad(sl.M, V.L), &pos, &other, team);
         if (team.lane() == 0) {
             if (sl.good_evals++ == 0) {
                 B.result[sl.problem].f0 = f;

@@ -44,12 +44,16 @@ struct BackendRoundItem {
     int slot, rc;
     int64_t out_off;  // doubles into the round's records
     int64_t blob_off; // doubles into the round's blobs
+    int64_t pose_off; // records into BackendArgs::pose_rec (the pose penalty's, when it is on)
 };
 struct BackendArgs {
     host::LbfgsParams P;
     double rho;
     host::DynamicsParams dyn;     // the context's speed and yaw-rate limits (svsdf_set_dynamics), used when dyn_on
     int dyn_on;
+    int pose_on;                  // the context's pose penalty (svsdf_set_pose_penalty): its parameters and the round's sample records
+    host::PoseParams pose;
+    const double *pose_rec;
     int Nmax;
     int64_t slot_doubles;
     BackendSlot *slots;

@@ -50,6 +50,14 @@ SVSDF_DECLARE_LAUNCHERS(strict_scaled, strict_multi_scaled)
 SVSDF_DECLARE_RIGID_LAUNCHERS(fast, fast_multi)
 SVSDF_DECLARE_RIGID_LAUNCHERS(strict, strict_multi)
 #undef SVSDF_DECLARE_RIGID_LAUNCHERS
+// svsdf_set_pose_penalty (svsdf_pose.cu, built fast and strict): the sample records of A.n problems, grid.y = A.n; max_items: the most
+// samples, N (res + 1), of one problem.  Every analytic functor and the Polygon; the mesh functor is not supported.
+namespace fast {
+cudaError_t launch_pose(const PoseArgs &A, const ShapeParams &S, int max_items, cudaStream_t st);
+}
+namespace strict {
+cudaError_t launch_pose(const PoseArgs &A, const ShapeParams &S, int max_items, cudaStream_t st);
+}
 cudaError_t launch_extract_count(const ExtractArgs &E, int *block_counts, int n_blocks, int64_t *n_total,
                                  cudaStream_t stream);
 cudaError_t launch_extract_write(const ExtractArgs &E, const int *block_offsets, int n_blocks, double *out_xy,

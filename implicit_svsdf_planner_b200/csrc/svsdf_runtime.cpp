@@ -41,7 +41,8 @@ using namespace svsdf;
 
 // The host half of one back-end evaluation (back_end_optimizer.hpp:353-398), shared by svsdf_evaluate and the lock-step back end
 // (svsdf_optimize_lockstep).  forward(): tau -> T and MINCO (coefficients, energy and its partial gradients), before the device
-// evaluation; backward(): adds the device record and the dynamics penalty (dyn not null), propagates through MINCO and adds rho * sum(T).
+// evaluation; backward(): adds the device record, the pose penalty (pose not null) and the dynamics penalty (dyn not null), propagates
+// through MINCO and adds rho * sum(T).
 struct HostEval {
     host::MincoS3NU minco;
     int N = 0;
@@ -64,10 +65,11 @@ struct HostEval {
                                      partialGradByCoeffs.data(), gradByPoints.data(), adj.data(), dynPartial.data()};
     }
     void forward(const double *x) { energy = host::backend_forward(view(), x); }
-    // o: the device record [cost, gradC (18N), gradT (N), n_inside] of the trajectory forward() built
-    double backward(const double *o, const double *x, double rho, const host::DynamicsParams *dyn, double *g, double *pos_out,
-                    double *other_out) {
-        return host::backend_backward(view(), energy, o, x, rho, dyn, g, pos_out, other_out);
+    // o: the device record [cost, gradC (18N), gradT (N), n_inside] of the trajectory forward() built; pose_rec: its pose penalty's
+    // sample records (read when pose is not null)
+    double backward(const double *o, const double *x, double rho, const host::PoseParams *pose, const double *pose_rec,
+                    const host::DynamicsParams *dyn, double *g, double *pos_out, double *other_out) {
+        return host::backend_backward(view(), energy, o, x, rho, pose, pose_rec, dyn, g, pos_out, other_out);
     }
     // The final trajectory from the solver's returned iterate x (optimize_traj_lmbm does the same on success and failure,
     // back_end_optimizer.cpp:44-94) and the run's statistics.
@@ -236,6 +238,14 @@ struct svsdf_ctx {
     bool dyn_on = false;
     host::DynamicsParams dyn{};
     const host::DynamicsParams *dynamics() const { return dyn_on ? &dyn : nullptr; }
+    // the pose-sampled obstacle penalty (svsdf_set_pose_penalty): every back-end evaluation of this context adds it when pose_on; it
+    // gathers its cells from the 3-D map (map3d: the map came from svsdf_set_map3d).  d_pose_rec: the sample records of a call
+    bool pose_on = false;
+    host::PoseParams pose{};
+    double pose_half[3] = {0, 0, 0};
+    const host::PoseParams *pose_penalty() const { return pose_on ? &pose : nullptr; }
+    bool map3d = false;
+    DeviceBuffer<double> d_pose_rec;
     double gpu_ms_total = 0.0;
     bool time_kernels = false;
     int last_status = 0;
@@ -306,12 +316,13 @@ struct Kernels {
     decltype(&fast_multi::launch_pose_multi) pose_multi;
     decltype(&fast_multi::launch_compact_multi) compact_multi;
     decltype(&fast_multi::launch_finalize_multi) finalize_multi;
+    decltype(&fast::launch_pose) pose;
 };
 #define SVSDF_VARIANT(NS, SCALED)                                                                                      \
     {NS##SCALED::query_occupancy,  NS##SCALED::launch_cost_kernels, NS::launch_pose_table,                            \
      NS::launch_finalize,          NS::launch_shape_eval,           NS::launch_sincos,                                \
      NS##_multi##SCALED::launch_multi, NS##_multi::launch_pose_multi, NS##_multi::launch_compact_multi,              \
-     NS##_multi::launch_finalize_multi}
+     NS##_multi::launch_finalize_multi, NS::launch_pose}
 const Kernels kKernels[2][2] = {{SVSDF_VARIANT(fast, ), SVSDF_VARIANT(fast, _scaled)}, {SVSDF_VARIANT(strict, ), SVSDF_VARIANT(strict, _scaled)}};
 #undef SVSDF_VARIANT
 
@@ -676,20 +687,63 @@ int run_kernels(svsdf_ctx *ctx, const double *d_points, int64_t P, bool reduce, 
     return SVSDF_OK;
 }
 
-// R1 on the context's points; result (1 + 19N + 1 doubles) lands in ctx->h_out after the stream sync.
-int cost_grad_raw(svsdf_ctx *ctx, int N, const double *T, const double *coeffs) {
+// With the pose penalty on (svsdf_set_pose_penalty) the context needs a 3-D map: checked before any launch.
+int pose_ready(svsdf_ctx *ctx, const char *who) {
+    if (!ctx->pose_on || (ctx->map3d && ctx->map())) return SVSDF_OK;
+    ctx->err = std::string(who) + ": the pose penalty needs a 3-D map (svsdf_set_map3d)";
+    return SVSDF_ERR_NOT_READY;
+}
+
+// The pose penalty's sample records (4 doubles each) of n trajectories into rec: problem k's blob at blobs + prob[k].blob_off, its
+// N (res + 1) records from record prob[k].rec_off (prob null: one problem, blob at blobs, records from 0).  max_N: the most pieces.
+int launch_pose(svsdf_ctx *ctx, const host::PoseParams &pp, const double *half, const double *blobs, const PoseProblem *prob, int n,
+                int max_N, double *rec) {
+    PoseArgs A;
+    std::memset(&A, 0, sizeof(A));
+    A.map = ctx->map();
+    A.X = ctx->map_X; A.Y = ctx->map_Y; A.Z = ctx->map_Z; A.h = ctx->map_h; A.row_bytes = ctx->map_row_bytes;
+    A.layer = (int64_t)(A.X + 2 * A.h) * A.row_bytes;
+    A.res = ctx->map_res;
+    const double lo[3] = {ctx->map_ox, ctx->map_oy, ctx->map_oz};
+    const int size[3] = {A.X, A.Y, A.Z};
+    for (int a = 0; a < 3; ++a) {
+        A.lo[a] = lo[a];
+        A.hi[a] = lo[a] + (double)size[a] * A.res;  // boundary_xyzmax as extract_impl takes it
+        A.half[a] = half[a];
+    }
+    A.safety_hor = ctx->cp.safety_hor;
+    A.res_samples = pp.res;
+    A.n = n;
+    A.blobs = blobs;
+    A.prob = prob;
+    A.rec = rec;
+    CK(kernels(ctx).pose(A, ctx->shape, max_N * (pp.res + 1), ctx->stream));
+    ctx->launches += 1;
+    return SVSDF_OK;
+}
+
+// R1 on the context's points; result (1 + 19N + 1 doubles) lands in ctx->h_out after the stream sync.  pose: also the pose penalty's
+// sample records, right behind it in h_out (the same download).
+int cost_grad_raw(svsdf_ctx *ctx, int N, const double *T, const double *coeffs, bool pose = false) {
     if (!ctx->points() || ctx->P < 0) {
         ctx->err = "svsdf: query points not set";
         return SVSDF_ERR_NOT_READY;
     }
     int rc = upload_traj(ctx, N, T, coeffs, ctx->P);
     if (rc) return rc;
+    const int nout = 1 + 19 * N + 1;
+    const int npose = pose ? 4 * N * (ctx->pose.res + 1) : 0;
     if (ctx->time_kernels) CK(cudaEventRecord(ctx->ev0, ctx->stream));
+    if (pose) {
+        CK(ctx->d_out.reserve(nout + npose));
+        CK(ctx->h_out.reserve(nout + npose));
+        rc = launch_pose(ctx, ctx->pose, ctx->pose_half, ctx->d_blob, nullptr, 1, N, ctx->d_out + nout);
+        if (rc) return rc;
+    }
     rc = run_kernels(ctx, ctx->points(), ctx->P, true, true, nullptr, nullptr, nullptr, nullptr);
     if (rc) return rc;
     if (ctx->time_kernels) CK(cudaEventRecord(ctx->ev1, ctx->stream));
-    const int nout = 1 + 19 * N + 1;
-    CK(cudaMemcpyAsync(ctx->h_out, ctx->d_out, (size_t)nout * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->h_out, ctx->d_out, (size_t)(nout + npose) * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     if (ctx->time_kernels) {
         float ms = 0;
@@ -707,14 +761,20 @@ double evaluate_impl(svsdf_ctx *ctx, const double *x, double *g, int n) {
         ctx->last_status = SVSDF_ERR_NOT_READY;
         return NAN;
     }
-    ctx->n_evaluate++;
-    ctx->he.forward(x);
-    int rc = cost_grad_raw(ctx, N, ctx->he.times.data(), ctx->he.minco.getCoeffs());
+    int rc = pose_ready(ctx, "svsdf_evaluate");
     if (rc) {
         ctx->last_status = rc;
         return NAN;
     }
-    const double cost = ctx->he.backward(ctx->h_out, x, ctx->rho, ctx->dynamics(), g, &ctx->cost_pos, &ctx->cost_other);
+    ctx->n_evaluate++;
+    ctx->he.forward(x);
+    rc = cost_grad_raw(ctx, N, ctx->he.times.data(), ctx->he.minco.getCoeffs(), ctx->pose_on);
+    if (rc) {
+        ctx->last_status = rc;
+        return NAN;
+    }
+    const double cost = ctx->he.backward(ctx->h_out, x, ctx->rho, ctx->pose_penalty(), ctx->h_out + (1 + 19 * N + 1), ctx->dynamics(), g,
+                                         &ctx->cost_pos, &ctx->cost_other);
     ctx->cost_total = cost;
     ctx->last_status = SVSDF_OK;
     return cost;
@@ -728,6 +788,7 @@ struct MultiItem {
     int64_t P = 0;
     int stride = 2;
     double *out = nullptr;        // host record [cost, gradC (18N), gradT (N), n_inside]
+    double *pose_out = nullptr;   // not null: also the pose penalty's N (res + 1) sample records (svsdf_optimize_lockstep, pose on)
     int rc = SVSDF_OK;
 };
 
@@ -910,9 +971,20 @@ int run_multi(svsdf_ctx *ctx, MultiItem *items, int n, float *ms, const PointQue
     if (m == 0) return SVSDF_OK;
     int rc = plan_multi(ctx, pl);
     if (rc) return rc;
-    // packed inputs: problem table | CTA maps (sparse, batched) | blobs | points (x, y; not with pq)
+    // the pose penalty's problems: the items that want its records
+    std::vector<PoseProblem> pp;
+    std::vector<int> pose_item;
+    int64_t pose_tot = 0;
+    if (!pq)
+        for (int j = 0; j < m; ++j)
+            if (items[who[j]].pose_out) {
+                pp.push_back(PoseProblem{pl.pr[j].blob_off, pose_tot});
+                pose_item.push_back(j);
+                pose_tot += (int64_t)pl.pr[j].N * (ctx->pose.res + 1);
+            }
+    // packed inputs: problem table | CTA maps (sparse, batched) | blobs | points (x, y; not with pq) | pose problems
     const size_t o_blob = pl.head_bytes, o_pts = align16(o_blob + (size_t)blob_tot * 8),
-                 in_bytes = align16(o_pts + (pq ? 0 : (size_t)pt_tot * 16));
+                 o_pose = align16(o_pts + (pq ? 0 : (size_t)pt_tot * 16)), in_bytes = align16(o_pose + pp.size() * sizeof(PoseProblem));
     CK(ctx->h_multi_in.reserve(in_bytes));
     CK(ctx->d_multi_in.reserve(in_bytes));
     // the previous call's copy has completed (every call ends with a stream synchronise)
@@ -929,9 +1001,16 @@ int run_multi(svsdf_ctx *ctx, MultiItem *items, int n, float *ms, const PointQue
             for (int64_t i = 0; i < it.P; ++i) { xy[2 * i] = it.pts[i * it.stride]; xy[2 * i + 1] = it.pts[i * it.stride + 1]; }
         }
     }
-    CK(ctx->h_multi_out.reserve(pl.out_tot));
+    if (!pp.empty()) std::memcpy(h + o_pose, pp.data(), pp.size() * sizeof(PoseProblem));
+    CK(ctx->h_multi_out.reserve(pl.out_tot + 4 * pose_tot));
     CK(cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, ctx->stream));
     if (ms) CK(cudaEventRecord(ctx->ev0, ctx->stream));
+    if (!pp.empty()) {
+        CK(ctx->d_pose_rec.reserve((size_t)4 * pose_tot));
+        rc = launch_pose(ctx, ctx->pose, ctx->pose_half, reinterpret_cast<const double *>(d + o_blob),
+                         reinterpret_cast<const PoseProblem *>(d + o_pose), (int)pp.size(), pl.max_N, ctx->d_pose_rec);
+        if (rc) return rc;
+    }
     double *records = nullptr;
     rc = launch_plan(ctx, pl, d, reinterpret_cast<double *>(d + o_blob), pq ? pq->pts : reinterpret_cast<const double *>(d + o_pts), pq,
                      &records);
@@ -939,8 +1018,15 @@ int run_multi(svsdf_ctx *ctx, MultiItem *items, int n, float *ms, const PointQue
     if (pq) return SVSDF_OK;
     if (ms) CK(cudaEventRecord(ctx->ev1, ctx->stream));
     CK(cudaMemcpyAsync(ctx->h_multi_out, records, (size_t)pl.out_tot * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    if (!pp.empty())
+        CK(cudaMemcpyAsync(ctx->h_multi_out + pl.out_tot, ctx->d_pose_rec, (size_t)pose_tot * 32, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     if (ms) CK(cudaEventElapsedTime(ms, ctx->ev0, ctx->ev1));
+    for (size_t q = 0; q < pp.size(); ++q) {
+        const int j = pose_item[q];
+        std::memcpy(items[who[j]].pose_out, ctx->h_multi_out + pl.out_tot + 4 * pp[q].rec_off,
+                    (size_t)pl.pr[j].N * (ctx->pose.res + 1) * 32);
+    }
     int64_t inside = 0;
     for (int j = 0; j < m; ++j) {
         const int nout = 19 * pl.pr[j].N + 2;
@@ -1810,6 +1896,74 @@ int svsdf_dynamics_penalty(const svsdf_dynamics *dyn, int N, const double *T, co
     return SVSDF_OK;
 }
 
+static bool pose_penalty_valid(const svsdf_pose_penalty &p) {
+    const double v[4] = {p.weight, p.half[0], p.half[1], p.half[2]};
+    for (double e : v)
+        if (!std::isfinite(e)) return false;
+    return p.weight >= 0.0 && p.integralIntervs >= 1 && p.integralIntervs <= 64 && p.half[0] > 0.0 && p.half[1] > 0.0 && p.half[2] > 0.0;
+}
+
+void svsdf_default_pose_penalty(svsdf_pose_penalty *p) {
+    if (!p) return;
+    p->weight = 60.0;  // weight_p
+    p->integralIntervs = 4;
+    p->half[0] = p->half[1] = p->half[2] = 8.5;  // kernel_size * occupancy_resolution / 2 = 17 * 1.0 / 2
+}
+
+static int pose_penalty_check(svsdf_ctx *ctx, const svsdf_pose_penalty &p, const char *who) {
+    if (!pose_penalty_valid(p)) {
+        ctx->err = std::string(who) + ": needs finite values, weight >= 0, 1 <= integralIntervs <= 64 and half sizes > 0";
+        return SVSDF_ERR_INVALID;
+    }
+    if (ctx->shape.id == SH_MESH) {
+        ctx->err = std::string(who) + ": not available for the mesh functor";
+        return SVSDF_ERR_INVALID;
+    }
+    return SVSDF_OK;
+}
+
+int svsdf_set_pose_penalty(svsdf_ctx *ctx, const svsdf_pose_penalty *p) {
+    if (!ctx) return SVSDF_ERR_INVALID;
+    if (!p) {
+        ctx->pose_on = false;
+        return SVSDF_OK;
+    }
+    if (const int rc = pose_penalty_check(ctx, *p, "svsdf_set_pose_penalty")) return rc;
+    ctx->pose.weight = p->weight;
+    ctx->pose.res = p->integralIntervs;
+    for (int a = 0; a < 3; ++a) ctx->pose_half[a] = p->half[a];
+    ctx->pose_on = true;
+    return SVSDF_OK;
+}
+
+int svsdf_pose_penalty_eval(svsdf_ctx *ctx, int N, const double *T, const double *coeffs, const svsdf_pose_penalty *p, double *cost,
+                            double *gradC, double *gradT, double *samples_out) {
+    if (!ctx || !p || !cost || !gradC || !gradT) return SVSDF_ERR_INVALID;
+    if (const int rc = pose_penalty_check(ctx, *p, "svsdf_pose_penalty_eval")) return rc;
+    if (!ctx->map3d || !ctx->map()) {
+        ctx->err = "svsdf_pose_penalty_eval: needs a 3-D map (svsdf_set_map3d)";
+        return SVSDF_ERR_NOT_READY;
+    }
+    CK(cudaSetDevice(ctx->device));
+    int rc = upload_traj(ctx, N, T, coeffs, 0, false);
+    if (rc) return rc;
+    host::PoseParams pp;
+    pp.weight = p->weight;
+    pp.res = p->integralIntervs;
+    const size_t nrec = (size_t)4 * N * (pp.res + 1);
+    CK(ctx->d_pose_rec.reserve(nrec));
+    rc = launch_pose(ctx, pp, p->half, ctx->d_blob, nullptr, 1, N, ctx->d_pose_rec);
+    if (rc) return rc;
+    std::vector<double> rec(nrec), gc((size_t)18 * N, 0.0), gt(N, 0.0), partial(N, 0.0);
+    CK(cudaMemcpyAsync(rec.data(), ctx->d_pose_rec, nrec * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    *cost = host::pose_penalty(pp, N, T, coeffs, rec.data(), gc.data(), gt.data(), partial.data());
+    std::memcpy(gradC, gc.data(), sizeof(double) * 18 * N);
+    std::memcpy(gradT, gt.data(), sizeof(double) * N);
+    if (samples_out) std::memcpy(samples_out, rec.data(), nrec * sizeof(double));
+    return SVSDF_OK;
+}
+
 int svsdf_scale_matrix(const svsdf_scale *scale, double t, double S_out[9], double Sinv_out[9]) {
     if (!scale || !scale_valid(*scale) || !std::isfinite(t)) return SVSDF_ERR_INVALID;
     // the arithmetic of scale_inv (svsdf_kernels.cuh) and Eigen 3.3's size-3 inverse of diag(sx, sy, 1)
@@ -2641,7 +2795,7 @@ struct LockstepSlot {
     const svsdf_lockstep_problem *pr = nullptr;
     HostEval he;
     MultiItem item;
-    std::vector<double> out;
+    std::vector<double> out, pose_out;
     int last_status = SVSDF_OK;
     int evals = 0;
     double gpu_ms = 0.0;
@@ -2664,7 +2818,8 @@ static double lockstep_evaluate(void *inst, const double *x, double *g, const in
         return NAN;
     }
     double pos = 0.0, other = 0.0;
-    const double cost = s.he.backward(s.out.data(), x, s.ctx->rho, s.ctx->dynamics(), g, &pos, &other);
+    const double cost = s.he.backward(s.out.data(), x, s.ctx->rho, s.ctx->pose_penalty(), s.pose_out.data(), s.ctx->dynamics(), g, &pos,
+                                      &other);
     if (s.evals++ == 0 && s.pr->f0_out) *s.pr->f0_out = cost;
     s.last_status = SVSDF_OK;
     return cost;
@@ -2691,6 +2846,7 @@ int svsdf_optimize_lockstep(svsdf_ctx *ctx, const svsdf_lockstep_problem *proble
             return SVSDF_ERR_INVALID;
         }
     }
+    if (const int rc = pose_ready(ctx, "svsdf_optimize_lockstep")) return rc;
     ctx->lockstep_rounds = 0;
     ctx->round_eval_ms = ctx->round_backend_ms = 0.0;
     if (n == 0) return SVSDF_OK;
@@ -2728,6 +2884,10 @@ int svsdf_optimize_lockstep(svsdf_ctx *ctx, const svsdf_lockstep_problem *proble
         s.out.assign((size_t)19 * N + 2, 0.0);
         s.item = MultiItem();
         s.item.N = N; s.item.pts = p.points; s.item.P = p.P; s.item.stride = p.stride; s.item.out = s.out.data();
+        if (ctx->pose_on) {
+            s.pose_out.assign((size_t)4 * N * (ctx->pose.res + 1), 0.0);
+            s.item.pose_out = s.pose_out.data();
+        }
         s.last_status = SVSDF_OK;
         s.evals = 0;
         s.gpu_ms = 0.0;
@@ -2806,6 +2966,7 @@ int svsdf_optimize_device(svsdf_ctx *ctx, const svsdf_lockstep_problem *problems
         }
         Nmax = std::max(Nmax, p.N);
     }
+    if (const int rc = pose_ready(ctx, "svsdf_optimize_device")) return rc;
     ctx->lockstep_rounds = 0;
     ctx->round_eval_ms = ctx->round_backend_ms = 0.0;
     if (rounds_out) *rounds_out = 0;
@@ -2868,6 +3029,8 @@ int svsdf_optimize_device(svsdf_ctx *ctx, const svsdf_lockstep_problem *problems
     B.rho = ctx->rho;
     B.dyn_on = ctx->dyn_on ? 1 : 0;
     B.dyn = ctx->dyn;
+    B.pose_on = ctx->pose_on ? 1 : 0;
+    B.pose = ctx->pose;
     B.Nmax = Nmax;
     B.slot_doubles = slot_doubles;
     B.slots = ctx->d_be_slots;
@@ -2977,7 +3140,8 @@ int svsdf_optimize_device(svsdf_ctx *ctx, const svsdf_lockstep_problem *problems
         // 2. the round: every slot asking for an evaluation, planned as run_multi plans (each problem keeps its single call's grid)
         MultiPlan pl;
         std::vector<BackendRoundItem> items;
-        int64_t blob_tot = 0;
+        std::vector<PoseProblem> pp;  // the pose penalty's problems (pose on): every valid item's blob and records
+        int64_t blob_tot = 0, pose_tot = 0;
         round_probs.clear();
         round_valid_slots.clear();
         for (int s = 0; s < M; ++s) {
@@ -2988,6 +3152,7 @@ int svsdf_optimize_device(svsdf_ctx *ctx, const svsdf_lockstep_problem *problems
             it.rc = st[s].valid ? SVSDF_OK : SVSDF_ERR_INVALID;
             it.out_off = 0;
             it.blob_off = 0;
+            it.pose_off = 0;
             round_probs.push_back(k);
             if (it.rc == SVSDF_OK) {
                 const BlobLayout L = blob_layout(st[s].N, st[s].K1);
@@ -3001,6 +3166,11 @@ int svsdf_optimize_device(svsdf_ctx *ctx, const svsdf_lockstep_problem *problems
                 m.K1 = L.K1;
                 it.blob_off = blob_tot;
                 blob_tot += L.total;
+                if (ctx->pose_on) {
+                    it.pose_off = pose_tot;
+                    pp.push_back(PoseProblem{it.blob_off, pose_tot});
+                    pose_tot += (int64_t)m.N * (ctx->pose.res + 1);
+                }
                 pl.pr.push_back(m);
                 round_valid_slots.push_back(s);
             }
@@ -3015,19 +3185,21 @@ int svsdf_optimize_device(svsdf_ctx *ctx, const svsdf_lockstep_problem *problems
             for (BackendRoundItem &it : items) it.rc = rc;
             if (round_err == SVSDF_OK) round_err = rc;
             pl = MultiPlan();
+            pp.clear();
             round_valid_slots.clear();
         } else {
             for (int j = 0, v = 0; j < count; ++j)
                 if (items[j].rc == SVSDF_OK) items[j].out_off = pl.pr[v++].out_off;
         }
-        // 3. one small upload: the round items, the problem table and the CTA maps (the stage's earlier copies have completed)
-        const size_t bytes = o_head0 + pl.head_bytes;
+        // 3. one small upload: the round items, the problem table and the CTA maps, the pose problems (the stage's earlier copies have
+        // completed)
+        const size_t o_pose = o_head0 + pl.head_bytes, bytes = o_pose + pp.size() * sizeof(PoseProblem);
         CKB(ctx->h_be_round.reserve(bytes));
         CKB(ctx->d_be_round.reserve(bytes));
         std::memcpy(ctx->h_be_round + o_items, items.data(), (size_t)count * sizeof(BackendRoundItem));
         if (!pl.pr.empty()) pack_plan(pl, ctx->h_be_round + o_head0);
-        CKB(cudaMemcpyAsync(ctx->d_be_round + o_items, ctx->h_be_round + o_items, o_head0 - o_items + pl.head_bytes, cudaMemcpyHostToDevice,
-                            ctx->stream));
+        if (!pp.empty()) std::memcpy(ctx->h_be_round + o_pose, pp.data(), pp.size() * sizeof(PoseProblem));
+        CKB(cudaMemcpyAsync(ctx->d_be_round + o_items, ctx->h_be_round + o_items, bytes - o_items, cudaMemcpyHostToDevice, ctx->stream));
         const BackendRoundItem *d_items = reinterpret_cast<const BackendRoundItem *>(ctx->d_be_round + o_items);
         // 4. the launches: blobs, the evaluation, the records into the machines
         CKB(cudaEventRecord(ctx->ev0, ctx->stream));
@@ -3035,6 +3207,15 @@ int svsdf_optimize_device(svsdf_ctx *ctx, const svsdf_lockstep_problem *problems
             CKB(ctx->d_be_blobs.reserve(blob_tot));
             CKB(launch_backend_blob(B, d_items, count, ctx->d_be_blobs, ctx->stream));
             ctx->launches += 1;
+        }
+        if (!pp.empty()) {  // the pose penalty's records, read by k_backend_backward
+            CKB(ctx->d_pose_rec.reserve((size_t)4 * pose_tot));
+            B.pose_rec = ctx->d_pose_rec;
+            int max_N = 1;
+            for (const MultiProblem &m : pl.pr) max_N = std::max(max_N, m.N);
+            rc = launch_pose(ctx, ctx->pose, ctx->pose_half, ctx->d_be_blobs, reinterpret_cast<const PoseProblem *>(ctx->d_be_round + o_pose),
+                             (int)pp.size(), max_N, ctx->d_pose_rec);
+            if (rc) return fail(rc);
         }
         CKB(cudaEventRecord(ctx->evk[0], ctx->stream));
         double *records = nullptr;
@@ -3150,6 +3331,7 @@ static int set_map_meta(svsdf_ctx *ctx, int X, int Y, int kernel_size, double ox
     ctx->map_row_bytes = (Y + 2 * ctx->map_h + 7) / 8;
     ctx->map_ox = ox; ctx->map_oy = oy; ctx->map_oz = 0.0; ctx->map_res = res;
     ctx->map_Z = 1;
+    ctx->map3d = false;
     return SVSDF_OK;
 }
 
@@ -3209,6 +3391,7 @@ int svsdf_set_map3d(svsdf_ctx *ctx, const unsigned char *kernel_bytes, int X, in
     CK(cudaStreamSynchronize(ctx->stream));
     ctx->map_Z = Z;
     ctx->map_oz = origin_xyz[2];
+    ctx->map3d = true;
     return SVSDF_OK;
 }
 
@@ -3226,20 +3409,7 @@ static int extract_impl(svsdf_ctx *ctx, const char *who, const double *wp, int W
     const double lo[3] = {E.ox, E.oy, ctx->map_oz};
     const double hi[3] = {E.ox + (double)E.X * E.res, E.oy + (double)E.Y * E.res, ctx->map_oz + (double)Z * E.res};  // boundary_xyzmax
     const int size[3] = {E.X, E.Y, Z};
-    // clamped index box around a centre: corner = centre -+ half -> projInMap (PCSmap_manager.h:128-135) -> getGridIndex
-    // (Gridmap3D.cpp:137-174: floor, clamped to the last cell)
-    auto box = [&](const double *c, int idx[3][2]) {
-        for (int a = 0; a < 3; ++a)
-            for (int side = 0; side < 2; ++side) {
-                double v = c[a] + (side ? half[a] : -half[a]);
-                v = v < lo[a] ? lo[a] : v;
-                v = v > hi[a] ? hi[a] : v;
-                int i = (int)std::floor((v - lo[a]) / E.res);
-                i = i < 0 ? 0 : i;
-                i = i >= size[a] ? size[a] - 1 : i;
-                idx[a][side] = i;
-            }
-    };
+    auto box = [&](const double *c, int idx[3][2]) { map_index_box(c, half, lo, hi, size, E.res, idx); };
     int bz1[kMaxWaypoints + 1], bz2[kMaxWaypoints + 1];  // slot 0: the box around tmp_pos, slot w + 1: waypoint w
     {
         const double tmp_pos[3] = {999.0, 999.0, 999.0};  // plan_manager.cpp:152

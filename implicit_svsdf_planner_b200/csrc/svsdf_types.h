@@ -1,5 +1,6 @@
 // svsdf_types.h — POD types shared by the host runtime and the sm_90a kernels.
 #pragma once
+#include <math.h>
 #include <stdint.h>
 
 #if defined(__CUDACC__)
@@ -214,6 +215,44 @@ struct ExtractArgs {
     int n_keepout;
     double clearance;
     double keepout[2 * kMaxKeepout];
+};
+
+// The clamped index box of the voxels around a centre c (x, y, z) with half sizes half: corner = c -+ half -> projInMap
+// (PCSmap_manager.h:128-135: clamped to [lo, hi], hi = lo + size * res) -> getGridIndex (Gridmap3D.cpp:137-174: floor, clamped to
+// the last cell).  idx[a] = {first, last}, both inclusive.  Shared by the query-point extraction (host) and the pose-sampled
+// obstacle penalty (device), so both see the same cells.
+SVSDF_HD inline void map_index_box(const double c[3], const double half[3], const double lo[3], const double hi[3], const int size[3],
+                                   double res, int idx[3][2]) {
+    for (int a = 0; a < 3; ++a)
+        for (int side = 0; side < 2; ++side) {
+            double v = c[a] + (side ? half[a] : -half[a]);
+            v = v < lo[a] ? lo[a] : v;
+            v = v > hi[a] ? hi[a] : v;
+            int i = (int)floor((v - lo[a]) / res);
+            i = i < 0 ? 0 : i;
+            i = i >= size[a] ? size[a] - 1 : i;
+            idx[a][side] = i;
+        }
+}
+
+// The pose-sampled obstacle penalty (svsdf_set_pose_penalty; the reference's grad_cost_p, back_end_optimizer.hpp:956-1028): one
+// record (costp, gradp_x, gradp_y, grad_yaw) per sample j = 0 .. res of every piece, piece-major.  PoseProblem: where a problem's
+// trajectory blob starts (doubles into PoseArgs::blobs) and where its N (res + 1) records go (records into PoseArgs::rec).
+struct PoseProblem {
+    int64_t blob_off, rec_off;
+};
+struct PoseArgs {
+    const unsigned char *map;  // Z layers of (X + 2h) x row_bytes, MSB-first bits along y (svsdf_set_map3d)
+    int X, Y, Z, h, row_bytes;
+    int64_t layer;             // bytes per layer
+    double lo[3], hi[3], res;  // boundary_xyzmin, boundary_xyzmax (lo + size * res) and the voxel edge
+    double half[3];            // the gather box's half sizes (bdx / 2, bdy / 2, bdz / 2)
+    double safety_hor;
+    int res_samples;           // integralIntervs
+    int n;                     // problems (grid.y)
+    const double *blobs;
+    const PoseProblem *prob;   // [n]
+    double *rec;               // [..][4]
 };
 
 // svsdf_swept_contour (svsdf_swept.cu): the narrow-band marching-squares mesher

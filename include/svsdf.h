@@ -149,6 +149,40 @@ int svsdf_set_dynamics(svsdf_ctx *ctx, const svsdf_dynamics *dyn);
 int svsdf_dynamics_penalty(const svsdf_dynamics *dyn, int N, const double *T, const double *coeffs, double *cost, double *gradC,
                            double *gradT);
 
+/* ---- Pose-sampled obstacle penalty: the discrete-pose collision cost ---------------------------------------------------------
+ * The reference's second collision cost, which it computes and never applies: addTimeIntPenalty (back_end_optimizer.hpp:411-533) calls
+ * grad_cost_p (:956-1028) at the samples j = 0 .. integralIntervs of every piece.  At the sample's pose x = (x, y, yaw) it gathers the
+ * occupied voxels of the 3-D map in the box x -+ half (getPointsInAABB, PCSmap_manager.h:160-182; the box's z range is centred on the
+ * yaw, as in the reference), keeps those whose body-frame offset p_rel = Rz(yaw)^T (c - x) has every |p_rel_a| <= half_a, and sums
+ * smoothedL1(safety_hor - sdf(p_rel), 0.01) and its gradient in position and yaw over them.  The per-sample sums are integrated with
+ * the trapezoid rule: cost = sum over i, j of node step weight costp_ij, node = 1/2 at both ends of a piece, step = T_i /
+ * integralIntervs.  Unlike the SVSDF term, whose query points are fixed when they are set, the voxels are gathered afresh around the
+ * trajectory at every evaluation; between samples the body is not seen (a fast trajectory can pass an obstacle unpenalised).  The
+ * body is rigid here even under svsdf_set_scale (the reference passes St and never uses it); safety_hor is the context's.  The exact
+ * arithmetic and summation order: svsdf_pose.cu (the records) and host::pose_penalty (csrc/host/minco.hpp, the chain rule).
+ * Not available for the mesh functor. */
+typedef struct {
+    double weight;        /* weight_p */
+    int integralIntervs;  /* samples j = 0 .. integralIntervs per piece */
+    double half[3];       /* the gather box's half sizes: kernel_size * occupancy_resolution / 2 in the reference */
+} svsdf_pose_penalty;
+/* star.yaml's values: weight 60, integralIntervs 4, half 8.5 on each axis. */
+void svsdf_default_pose_penalty(svsdf_pose_penalty *p);
+/* NULL: no pose penalty (the default).  Otherwise every later svsdf_evaluate, svsdf_optimize, svsdf_optimize_batch (each context of
+ * the pool with its own setting), svsdf_optimize_lockstep and svsdf_optimize_device of this context adds the penalty after the
+ * safety term and before the dynamics penalty; svsdf_last_costs counts it in cost_pos.  These calls then need a 3-D map
+ * (svsdf_set_map3d) and return SVSDF_ERR_NOT_READY, before any launch, without one.  The values are copied.  Returns
+ * SVSDF_ERR_INVALID, and keeps the previous setting, for a non-finite value, weight < 0, integralIntervs outside 1 .. 64, a half
+ * size <= 0, or a context of the mesh functor. */
+int svsdf_set_pose_penalty(svsdf_ctx *ctx, const svsdf_pose_penalty *p);
+/* The penalty p of one trajectory (N pieces as svsdf_cost_grad takes it) against the context's 3-D map and shape, on the device:
+ * writes (not adds) the cost, gradC[18N] (column-major like coeffs) and gradT[N], with the bits the back ends add, and, when
+ * samples_out is not NULL, the N (integralIntervs + 1) raw sample records (costp, gradp_x, gradp_y, grad_yaw) of grad_cost_p, piece
+ * by piece.  p need not be the context's setting.  Returns SVSDF_ERR_INVALID for invalid values or trajectories (refused as
+ * svsdf_set_pose_penalty and svsdf_cost_grad refuse them) and SVSDF_ERR_NOT_READY without a 3-D map. */
+int svsdf_pose_penalty_eval(svsdf_ctx *ctx, int N, const double *T, const double *coeffs, const svsdf_pose_penalty *p, double *cost,
+                            double *gradC, double *gradT, double *samples_out);
+
 /* ---- Swept-volume outline and mesh: the planner's own field contoured on the GPU ---------------------------------------------
  * svsdf_swept_contour meshes the level set f(p) = iso of f = getSDFofSweptVolume<false,true> (exactly what svsdf_query(...,
  * outer_only = 1) returns, bit for bit per point) on the z = 0 plane, for the trajectory (N, T, coeffs) as svsdf_query takes it and

@@ -256,6 +256,9 @@ class TrajOptimizer {
     // the vmax / omgmax / weight_v / weight_omg / smoothingEps / integralIntervs members setParam reads (:884-896), penalised in the
     // callback's dyn_cost slot (svsdf_set_dynamics; nullptr: no dynamics penalty, the default)
     int setDynamics(const svsdf_dynamics *dyn) { return svsdf_set_dynamics(sv_manager->handle(), dyn); }
+    // weight_p, integralIntervs and the bdx / bdy / bdz box of setParam (:884-898): the pose-sampled obstacle term of addTimeIntPenalty
+    // (:411-533), added after the safety term (svsdf_set_pose_penalty; nullptr: no pose penalty, the default; needs a 3-D map)
+    int setPosePenalty(const svsdf_pose_penalty *p) { return svsdf_set_pose_penalty(sv_manager->handle(), p); }
     int setConditions(const double *initS, const double *finalS, int N) {
         pieceN = N; temporalDim = N; spatialDim = 3 * (N - 1);
         return svsdf_set_boundary(sv_manager->handle(), initS, finalS, N);
