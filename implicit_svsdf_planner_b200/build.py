@@ -22,6 +22,10 @@ ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-ccbin", "/usr/bin/g++"]
 COMMON += os.environ.get("SVSDF_EXTRA_NVCC_FLAGS", "").split()  # experiments, e.g. -DSVSDF_OUTER_MIN_CTAS=4
 
+# The host runtime's units (csrc/svsdf_runtime_*.cpp, DESIGN.md §1): host threads for the batch A* bookkeeping and the point
+# upload; no a*b+c contraction, which keeps HostEval, MINCO and the float winding-number builder (host/fwn_bvh.hpp) bit-exact.
+RUNTIME_FLAGS = ["-Xcompiler", "-fopenmp", "-Xcompiler", "-ffp-contract=off"]
+
 UNITS = [
     # (source, object, extra flags)
     ("svsdf_kernels_fast.cu", "svsdf_kernels_fast.o", []),
@@ -42,8 +46,8 @@ UNITS = [
     # the pose-sampled obstacle penalty (svsdf_set_pose_penalty), fast and strict
     ("svsdf_pose.cu", "svsdf_pose_fast.o", ["-DSVSDF_NS=fast"]),
     ("svsdf_pose.cu", "svsdf_pose_strict.o", ["-DSVSDF_NS=strict", "-fmad=false"]),
-    # host threads for the batch A* bookkeeping; no a*b+c contraction in the float winding-number builder (host/fwn_bvh.hpp)
-    ("svsdf_runtime.cpp", "svsdf_runtime.o", ["-Xcompiler", "-fopenmp", "-Xcompiler", "-ffp-contract=off"]),
+    *[(f"svsdf_runtime_{u}.cpp", f"svsdf_runtime_{u}.o", RUNTIME_FLAGS)
+      for u in ("context", "eval", "multi", "backend", "front", "swept", "map", "host")],
 ]
 HEADERS = [
     "svsdf_kernels.cuh",
@@ -53,6 +57,7 @@ HEADERS = [
     "svsdf_types.h",
     "svsdf_launch.h",
     "svsdf_backend.h",
+    "svsdf_runtime.h",
     "host/minco.hpp",
     "host/lbfgs.hpp",
     "host/astar.hpp",

@@ -472,7 +472,7 @@ SVSDF_HD inline double pose_penalty(const PoseParams &p, int N, const double *T,
 
 // The host half of one back-end evaluation (back_end_optimizer.hpp:353-398) on flat storage of N pieces: times, gradByTimes,
 // partialGradByTimes (N each), partialGradByCoeffs and adj (18N each), gradByPoints (3 (N - 1)), dynPartial (N: the pose and the
-// dynamics penalties' per-piece costs, one penalty after the other).  Shared by the host evaluation (svsdf_runtime.cpp: HostEval) and
+// dynamics penalties' per-piece costs, one penalty after the other).  Shared by the host evaluation (svsdf_runtime.h: HostEval) and
 // the device back end (svsdf_backend.cu).
 struct BackendEvalView {
     MincoView m;

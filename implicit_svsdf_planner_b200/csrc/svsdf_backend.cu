@@ -61,7 +61,7 @@ struct WarpTeam {
     __device__ void sync() const { __syncwarp(); }
 };
 
-// the forward half of the evaluation the machine asks for, and traj_layout's checks and lattice count (svsdf_runtime.cpp)
+// the forward half of the evaluation the machine asks for, and traj_layout's checks and lattice count (svsdf_runtime_eval.cpp)
 __device__ void ask_evaluation(const BackendArgs &B, int s, const SlotView &V, const WarpTeam &team) {
     const double energy = host::backend_forward(V.E, V.L.x, team);
     if (team.lane() != 0) return;

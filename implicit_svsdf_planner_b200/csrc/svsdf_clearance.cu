@@ -2,7 +2,7 @@
 // Compiled with -fmad=false: a cell centre is ((i + 0.5) res + ox, (j + 0.5) res + oy) rounded as k_extract_write rounds it, so the
 // points are bit for bit the ones svsdf_extract_points[3d] hands the back end.
 //
-// Pipeline (the host side is clearance_bands in svsdf_runtime.cpp; svsdf_map_clearance is its one-trajectory case):
+// Pipeline (the host side is clearance_bands in svsdf_runtime_swept.cpp; svsdf_map_clearance is its one-trajectory case):
 //   k_cl_count   the words of every problem's reach rectangle, one item per 32-cell word, row-major, padded to whole CTAs of 256
 //                (the CTAs of problem k follow those of problem k - 1, so the CTA order is problem order, then map order).  The
 //                problem's samples whose reach touches the CTA's cell-centre box go to a shared list; each item ORs its word over

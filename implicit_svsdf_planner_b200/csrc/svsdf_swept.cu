@@ -2,7 +2,7 @@
 // Compiled with -fmad=false, and every operation that makes a vertex is an explicit _rn intrinsic: the vertices depend on the
 // field only, whichever build (strict or fast) evaluated it.
 //
-// Pipeline (the host side is svsdf_swept_contour in svsdf_runtime.cpp):
+// Pipeline (the host side is svsdf_swept_contour in svsdf_runtime_swept.cpp):
 //   k_sw_classify  one CTA per 16 x 16 tile: the path samples whose reach touches the tile's 18 x 18 corner region go to a shared list;
 //                  each region corner is tested against that list only (unproven: within some sample's reach); a corner is needed
 //                  when one of the cells around it has an unproven corner.  Writes the need flags, NaN into the field, the tile's count.

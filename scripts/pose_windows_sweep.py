@@ -1,6 +1,6 @@
 """Device time of one cost + gradient evaluation with and without the layer-3 pose windows (SVSDF_FORCE_POSE_WINDOWS = 1 / 2), over
 the number of query points, on config 2's trajectory (8 pieces, K1 = 134) and on a 64-piece, 299.84 s one (K1 = 1999): the
-measurement behind the layer-3 rule of pose_windows() in csrc/svsdf_runtime.cpp.
+measurement behind the layer-3 rule of pose_windows() in csrc/svsdf_runtime_eval.cpp.
 
     python scripts/pose_windows_sweep.py [--repeats R] [--rounds K] [--out FILE]
 

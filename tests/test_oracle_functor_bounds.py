@@ -3,7 +3,7 @@
 1. Mesh far-field bound.  choiceTInit's layer 1 skips a lattice sample when |q| >= prune_rmin and
    sdf >= (|q| - rout) / prune_scale already exceeds the best value found.  For the mesh functor svsdf_create derives
    prune_rmin = rho0, rout ~ Rv and prune_scale = 1 / (1 - 2 omega) from the root of the winding-number hierarchy
-   (csrc/svsdf_runtime.cpp, the "Far-field bound" block): omega is a term-by-term bound of the root children's order-2
+   (csrc/svsdf_runtime_context.cpp, upload_mesh's "Far-field bound" block): omega is a term-by-term bound of the root children's order-2
    expansions beyond rho0.  It is restated here in numpy from api.mesh_fwn_host's children and rows and checked against the
    oracle's float winding number (bitwise the reference's): |w(q)| <= omega on dense rings of z = 0 points at
    |q| = rho0 (1 + 1e-6), 1.5 rho0 and 10 rho0, and sdf(q) >= (1 - 2 omega)(|q| - Rv) there.  Where omega >= 0.45 or is not
