@@ -51,7 +51,10 @@ UNITS = [
 ]
 HEADERS = [
     "svsdf_kernels.cuh",
+    "svsdf_kernels_single.cuh",
+    "svsdf_kernels_shared.cuh",
     "svsdf_kernels_multi.cuh",
+    "svsdf_kernels_multi_shared.cuh",
     "svsdf_shapes.cuh",
     "svsdf_sincos.cuh",
     "svsdf_types.h",

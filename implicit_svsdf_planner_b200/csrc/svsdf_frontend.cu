@@ -374,50 +374,25 @@ cudaError_t launch_astar_t(const ShapeParams &S, const FrontParams &F, const Sub
 
 }  // namespace
 
-// The analytic functors the front end is defined for; Polygon / mesh: the reference defines no rotated kernels for them
-#define SVSDF_FRONT_SHAPES(CASE)                                                                                                 \
-    CASE(SH_STAR) CASE(SH_HORSESHOE) CASE(SH_PIE) CASE(SH_PIE2) CASE(SH_ARC) CASE(SH_TUNNEL) CASE(SH_CUTDISK) CASE(SH_TRAPEZOID) \
-    CASE(SH_RHOMBUS) CASE(SH_HEART) CASE(SH_ROUNDEDX) CASE(SH_BIGX) CASE(SH_ROUNDEDCROSS) CASE(SH_VESICA) CASE(SH_MOON)         \
-    CASE(SH_UNEVENCAPSULE) CASE(SH_CIRCLE)
-
+// The analytic functors only (ShapeSet::analytic): svsdf_front_init refuses Polygon and mesh
 cudaError_t launch_front_cells(const ShapeParams &S, const FrontParams &F, const double *yaws, unsigned char *cells, cudaStream_t st) {
-    switch (S.id) {
-#define SVSDF_CASE(ID) \
-    case ID: return S.has_xform ? launch_cells_t<ID, true>(S, F, yaws, cells, st) : launch_cells_t<ID, false>(S, F, yaws, cells, st);
-        SVSDF_FRONT_SHAPES(SVSDF_CASE)
-#undef SVSDF_CASE
-        default: return cudaErrorInvalidValue;
-    }
+    return dispatch_shape<ShapeSet::analytic>(S, [&](auto id, auto xf) { return launch_cells_t<id.value, xf.value>(S, F, yaws, cells, st); });
 }
 
 cudaError_t launch_front_expand(const ShapeParams &S, const FrontParams &F, const SubSwParams &P, const unsigned char *map,
                                 const unsigned char *kbytes, int64_t n, const int *node_ij, const double *node_yaw, unsigned char *ok_out,
                                 double *child_yaw_out, unsigned char *parts_out, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
-    switch (S.id) {
-#define SVSDF_CASE(ID)                                                                                                              \
-    case ID:                                                                                                                        \
-        return S.has_xform ? launch_expand_t<ID, true>(S, F, P, map, kbytes, n, node_ij, node_yaw, ok_out, child_yaw_out, parts_out, st) \
-                           : launch_expand_t<ID, false>(S, F, P, map, kbytes, n, node_ij, node_yaw, ok_out, child_yaw_out, parts_out, st);
-        SVSDF_FRONT_SHAPES(SVSDF_CASE)
-#undef SVSDF_CASE
-        default: return cudaErrorInvalidValue;
-    }
+    return dispatch_shape<ShapeSet::analytic>(S, [&](auto id, auto xf) {
+        return launch_expand_t<id.value, xf.value>(S, F, P, map, kbytes, n, node_ij, node_yaw, ok_out, child_yaw_out, parts_out, st);
+    });
 }
 
 cudaError_t launch_front_astar(const ShapeParams &S, const FrontParams &F, const SubSwParams &P, const unsigned char *map,
                                const unsigned char *kbytes, const AstarArgs &A, int grid, int *ctas_per_sm, cudaStream_t st) {
-    switch (S.id) {
-#define SVSDF_CASE(ID)                                                                                            \
-    case ID:                                                                                                      \
-        return S.has_xform ? launch_astar_t<ID, true>(S, F, P, map, kbytes, A, grid, ctas_per_sm, st)             \
-                           : launch_astar_t<ID, false>(S, F, P, map, kbytes, A, grid, ctas_per_sm, st);
-        SVSDF_FRONT_SHAPES(SVSDF_CASE)
-#undef SVSDF_CASE
-        default: return cudaErrorInvalidValue;
-    }
+    return dispatch_shape<ShapeSet::analytic>(
+        S, [&](auto id, auto xf) { return launch_astar_t<id.value, xf.value>(S, F, P, map, kbytes, A, grid, ctas_per_sm, st); });
 }
-#undef SVSDF_FRONT_SHAPES
 
 cudaError_t launch_front_cspace(const FrontParams &F, const unsigned char *map, const unsigned *rowmask, unsigned *out, cudaStream_t st) {
     const int64_t n = (int64_t)F.kernel_count * F.X * F.out_words;

@@ -21,8 +21,11 @@
 //   * points found inside the swept volume (sdf <= 0) are compacted in index order and handled by k_gsip, one
 //     CTA per point, ring samples spread over the CTA's warps.
 //
-// This file is compiled twice (see svsdf_kernels_fast.cu / svsdf_kernels_strict.cu): with FMA contraction
-// (default) and with -fmad=false ("strict": same rounding sequence as the CPU, used to debug parity).
+// This file holds what every cost unit compiles: the device code and the kernel templates of k_outer / k_gsip, and the launch
+// helpers their launchers share.  Each unit (svsdf_kernels{,_scaled,_multi,_multi_scaled}_{fast,strict}.cu) includes it through the
+// launchers it carries: svsdf_kernels_single.cuh or svsdf_kernels_multi.cuh, and in the rigid units the kernels the scaled ones share
+// (svsdf_kernels_shared.cuh, svsdf_kernels_multi_shared.cuh).  Every unit is compiled with FMA contraction (fast) and with
+// -fmad=false ("strict": same rounding sequence as the CPU, used to debug parity).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -1001,15 +1004,6 @@ __device__ __forceinline__ void pose_window_entry(const double *blob, PoseRec *w
     dev::sincos_portable(yaw, sy, cy);
     out->x = x; out->y = y; out->c = cy; out->s = sy;
 }
-#if !defined(SVSDF_SCALED_UNIT) && !defined(SVSDF_MULTI_UNIT)
-// one thread per layer-1 sample, then one per pose-window record
-__global__ void k_pose_table(double *blob, PoseRec *w2, PoseRec *w3) {
-    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const int K1 = (int)blob[1];
-    if (e < K1) pose_table_entry(blob, (int)e);
-    else if (w2) pose_window_entry(blob, w2, w3, e - K1);
-}
-#endif
 
 // ------------------------------------------------------------------------------------------------
 // K1: outer solve for every point (+ penalty, chain rule and CTA reduction for outside points)
@@ -1254,11 +1248,6 @@ __device__ __forceinline__ void compact_body(const unsigned char *flag, int64_t 
     }
     if (tid == 0) *n_out = total;
 }
-#ifndef SVSDF_MULTI_UNIT
-__global__ void __launch_bounds__(1024) k_compact(const unsigned char *flag, int64_t P, int *list, int *n_out) {
-    compact_body(flag, P, list, n_out);
-}
-#endif
 
 // ------------------------------------------------------------------------------------------------
 // K2: interior branch of getTrueSDFofSweptVolume<true> (sw_manager.hpp:926-1017, SampleSet2D :41-124).
@@ -1414,7 +1403,7 @@ __global__ void __launch_bounds__(WARPS * 32, (WARPS == kWarpsPerBlock && SHAPE 
 // result is bit-reproducible.  The last CTA to finish (ticket counter) writes the output record:
 // out: [0] cost, [1 .. 18N] gradC in Eigen column-major order (d*6N + 6i + q), [1+18N .. 1+19N) gradT with the
 // reference's rule gradT(j) += gdT for all j < piece (back_end_optimizer.hpp:859-862), [1+19N] n_inside.
-// (k_finalize and the utility kernels below live in the rigid units only: the scaled units share them.)
+// (k_finalize itself, svsdf_kernels_shared.cuh, lives in the rigid units only: the scaled units share it.)
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ double warp_sum_fixed(double v) {
 #pragma unroll
@@ -1476,327 +1465,34 @@ __device__ __forceinline__ void finalize_body(const double *partials, int n_bloc
     }
 }
 
-#if !defined(SVSDF_SCALED_UNIT) && !defined(SVSDF_MULTI_UNIT)
-__global__ void __launch_bounds__(256) k_finalize(const double *partials, int n_blocks, int N, const int *n_inside,
-                                                  const double *gsip_contrib, const int *gsip_piece, double *tot,
-                                                  unsigned int *ticket, double *out) {
-    finalize_body(partials, n_blocks, N, n_inside ? *n_inside : 0, gsip_contrib, gsip_piece, tot, ticket, out, blockIdx.x, gridDim.x);
-}
-
 // ------------------------------------------------------------------------------------------------
-// Shape-functor batch kernels (BasicShape::getonlySDF / getonlyGrad1 over arrays of body-frame points)
+// Host-side helpers of the cost launchers.  A variant's kernel list K (CostKernels, MultiKernels) names its kernels: K::outer(batched),
+// the sparse or batched k_outer, and K::gsip(wide), the 8- or 22-warp k_gsip.
 // ------------------------------------------------------------------------------------------------
-template <int SHAPE, bool XFORM>
-__global__ void k_shape_sdf(const __grid_constant__ ShapeParams S, const double *rel_xy, int64_t n, double *out) {
-    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    out[i] = dev::shape_sdf<SHAPE, XFORM>(S, rel_xy[2 * i], rel_xy[2 * i + 1]);
-}
-template <int SHAPE, bool XFORM>
-__global__ void k_shape_grad(const __grid_constant__ ShapeParams S, const double *rel_xy, int64_t n, double *out3) {
-    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    double rx = rel_xy[2 * i], ry = rel_xy[2 * i + 1];
-    double gx, gy;
-    if (SHAPE == SH_POLYGON) {
-        dev::PolyHit H = dev::polygon_scan(S, rx, ry);
-        double vx = rx - H.cx, vy = ry - H.cy;
-        double z = vx * vx + vy * vy;
-        if (z > 0.0) { double nn = sqrt(z); vx /= nn; vy /= nn; }
-        if (H.rs % 2 != 0) { vx = -vx; vy = -vy; }
-        gx = vx; gy = vy;
-    } else if (SHAPE == SH_CIRCLE) {
-        dev::circle_grad1<XFORM>(S, rx, ry, gx, gy);
-    } else {
-        const double dx = 0.000001;
-        double t0 = rx, t1 = ry;
-        t0 -= dx;
-        double sdfold = dev::shape_sdf<SHAPE, XFORM>(S, t0, t1);
-        t0 += 2 * dx;
-        double gradx = dev::shape_sdf<SHAPE, XFORM>(S, t0, t1) - sdfold;
-        t0 = rx;
-        t1 -= dx;
-        sdfold = dev::shape_sdf<SHAPE, XFORM>(S, t0, t1);
-        t1 += 2 * dx;
-        double grady = dev::shape_sdf<SHAPE, XFORM>(S, t0, t1) - sdfold;
-        gx = gradx / (2 * dx);
-        gy = grady / (2 * dx);
-    }
-    out3[3 * i] = gx; out3[3 * i + 1] = gy; out3[3 * i + 2] = 0.0;
-}
-
-__global__ void k_sincos(const double *x, int64_t n, double *s, double *c) {
-    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    double sv, cv;
-    dev::sincos_portable(x[i], sv, cv);
-    s[i] = sv;
-    c[i] = cv;
-}
-
-// FP64 FMA peak micro-benchmark (roofline denominator; MEASURED_PEAKS.json has no FP64 figure)
-__global__ void __launch_bounds__(256) k_fp64_peak(double *out, int iters) {
-    double a0 = threadIdx.x * 1e-3, a1 = a0 + 1, a2 = a0 + 2, a3 = a0 + 3, a4 = a0 + 4, a5 = a0 + 5, a6 = a0 + 6, a7 = a0 + 7;
-    const double m = 0.999999, c = 1e-6;
-    for (int i = 0; i < iters; ++i) {
-        a0 = fma(a0, m, c); a1 = fma(a1, m, c); a2 = fma(a2, m, c); a3 = fma(a3, m, c);
-        a4 = fma(a4, m, c); a5 = fma(a5, m, c); a6 = fma(a6, m, c); a7 = fma(a7, m, c);
-    }
-    out[(int64_t)blockIdx.x * blockDim.x + threadIdx.x] = a0 + a1 + a2 + a3 + a4 + a5 + a6 + a7;
-}
-#endif  // SVSDF_SCALED_UNIT
-
-// ------------------------------------------------------------------------------------------------
-// Host-side launchers (shape dispatch).  The scaled translation units (SVSDF_SCALED_UNIT) instantiate only the deformable-
-// robot kernels k_outer_scaled / k_gsip_scaled; the rigid units only k_outer / k_gsip.
-// ------------------------------------------------------------------------------------------------
-#ifdef SVSDF_SCALED_UNIT
-constexpr bool kScaledUnit = true;
-#else
-constexpr bool kScaledUnit = false;
-#endif
-// the multi-problem units (svsdf_kernels_multi*.cu) bring their own launchers (svsdf_kernels_multi.cuh)
-#ifndef SVSDF_MULTI_UNIT
-
-struct LaunchCfg {
-    int grid_outer, grid_gsip;
-    size_t smem_outer, smem_gsip;
-    cudaStream_t stream;
-    cudaEvent_t after_outer;  // optional timing mark recorded right after k_outer
-    bool gsip_wide;           // use the 22-warp k_gsip variant
-};
-
-// k[0] sparse k_outer, k[1] batched k_outer, k[2] 8-warp k_gsip, k[3] 22-warp k_gsip
-template <int SHAPE, bool XFORM, bool SCALED>
-static void cost_kernels(const void *k[4]) {
-    if constexpr (SCALED) {
-        k[0] = (const void *)k_outer_scaled<SHAPE, XFORM, false>;
-        k[1] = (const void *)k_outer_scaled<SHAPE, XFORM, true>;
-        k[2] = (const void *)k_gsip_scaled<SHAPE, XFORM, kWarpsPerBlock>;
-        k[3] = (const void *)k_gsip_scaled<SHAPE, XFORM, kGsipWarps>;
-    } else {
-        k[0] = (const void *)k_outer<SHAPE, XFORM, false>;
-        k[1] = (const void *)k_outer<SHAPE, XFORM, true>;
-        k[2] = (const void *)k_gsip<SHAPE, XFORM, kWarpsPerBlock>;
-        k[3] = (const void *)k_gsip<SHAPE, XFORM, kGsipWarps>;
-    }
-}
-
-template <int SHAPE, bool XFORM, bool SCALED>
-static cudaError_t launch_shape(const KernelArgs &A, const ShapeParams &S, const ScaleSched *Z, const LaunchCfg &cfg, int N) {
-    cudaError_t e;
-    // the attribute is per device (a process may hold contexts on several GPUs): one flag per device ordinal
+// Opts K's four kernels in to kMaxDynSmemBytes of dynamic shared memory, once per device ordinal: the attribute is per device (a
+// process may hold contexts on several GPUs).
+template <class K>
+static cudaError_t raise_smem_cap() {
     static bool attr_set_dev[64] = {};
     int dev_ord = 0;
     cudaGetDevice(&dev_ord);
     bool &attr_set = attr_set_dev[dev_ord & 63];
-    if (!attr_set) {
-        const void *k[4];
-        cost_kernels<SHAPE, XFORM, SCALED>(k);
-        for (int i = 0; i < 4; ++i) {
-            e = cudaFuncSetAttribute(k[i], cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-            if (e != cudaSuccess) return e;
-        }
-        attr_set = true;
-    }
-    if constexpr (SCALED) {
-        if (A.batched) k_outer_scaled<SHAPE, XFORM, true><<<cfg.grid_outer, kWarpsPerBlock * 32, cfg.smem_outer, cfg.stream>>>(A, S, *Z);
-        else k_outer_scaled<SHAPE, XFORM, false><<<cfg.grid_outer, kWarpsPerBlock * 32, cfg.smem_outer, cfg.stream>>>(A, S, *Z);
-    } else {
-        if (A.batched) k_outer<SHAPE, XFORM, true><<<cfg.grid_outer, kWarpsPerBlock * 32, cfg.smem_outer, cfg.stream>>>(A, S);
-        else k_outer<SHAPE, XFORM, false><<<cfg.grid_outer, kWarpsPerBlock * 32, cfg.smem_outer, cfg.stream>>>(A, S);
-    }
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
-    if (cfg.after_outer) cudaEventRecord(cfg.after_outer, cfg.stream);
-    if (A.want_gsip) {
-        k_compact<<<1, 1024, 0, cfg.stream>>>(A.inside_flag, A.P, A.inside_list, A.n_inside);
-        // few inside points: one warp per ring sample (latency); many: 8-warp CTAs, two per SM (throughput)
-        if constexpr (SCALED) {
-            if (cfg.gsip_wide) k_gsip_scaled<SHAPE, XFORM, kGsipWarps><<<cfg.grid_gsip, kGsipWarps * 32, cfg.smem_gsip, cfg.stream>>>(A, S, *Z);
-            else k_gsip_scaled<SHAPE, XFORM, kWarpsPerBlock><<<cfg.grid_gsip, kWarpsPerBlock * 32, cfg.smem_gsip, cfg.stream>>>(A, S, *Z);
-        } else {
-            if (cfg.gsip_wide) k_gsip<SHAPE, XFORM, kGsipWarps><<<cfg.grid_gsip, kGsipWarps * 32, cfg.smem_gsip, cfg.stream>>>(A, S);
-            else k_gsip<SHAPE, XFORM, kWarpsPerBlock><<<cfg.grid_gsip, kWarpsPerBlock * 32, cfg.smem_gsip, cfg.stream>>>(A, S);
-        }
-        e = cudaGetLastError();
+    if (attr_set) return cudaSuccess;
+    for (const void *k : {(const void *)K::outer(false), (const void *)K::outer(true), (const void *)K::gsip(false), (const void *)K::gsip(true)}) {
+        const cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmemBytes);
         if (e != cudaSuccess) return e;
     }
-    (void)N;
+    attr_set = true;
     return cudaSuccess;
 }
 
-template <bool XFORM>
-static cudaError_t dispatch(const KernelArgs &A, const ShapeParams &S, const ScaleSched *Z, const LaunchCfg &cfg, int N) {
-    switch (S.id) {
-#define SVSDF_CASE(ID) \
-    case ID: return launch_shape<ID, XFORM, kScaledUnit>(A, S, Z, cfg, N);
-        SVSDF_CASE(SH_STAR)
-        SVSDF_CASE(SH_HORSESHOE)
-        SVSDF_CASE(SH_PIE)
-        SVSDF_CASE(SH_PIE2)
-        SVSDF_CASE(SH_ARC)
-        SVSDF_CASE(SH_TUNNEL)
-        SVSDF_CASE(SH_CUTDISK)
-        SVSDF_CASE(SH_TRAPEZOID)
-        SVSDF_CASE(SH_RHOMBUS)
-        SVSDF_CASE(SH_HEART)
-        SVSDF_CASE(SH_ROUNDEDX)
-        SVSDF_CASE(SH_BIGX)
-        SVSDF_CASE(SH_ROUNDEDCROSS)
-        SVSDF_CASE(SH_VESICA)
-        SVSDF_CASE(SH_MOON)
-        SVSDF_CASE(SH_UNEVENCAPSULE)
-        SVSDF_CASE(SH_CIRCLE)
-#undef SVSDF_CASE
-        case SH_POLYGON: return launch_shape<SH_POLYGON, false, kScaledUnit>(A, S, Z, cfg, N);
-        case SH_MESH: return launch_shape<SH_MESH, false, kScaledUnit>(A, S, Z, cfg, N);
-        default: return cudaErrorInvalidValue;
-    }
-}
-
-template <int SHAPE, bool XFORM>
-static cudaError_t occ_shape(int N, int blob_doubles, int *occ_outer, int *occ_gsip, int *chunk_outer) {
-    const size_t smem_outer = outer_smem_doubles(blob_doubles, N, 1) * sizeof(double), smem_gsip = (size_t)blob_doubles * sizeof(double);
-    const void *k[4];
-    cost_kernels<SHAPE, XFORM, kScaledUnit>(k);
-    for (int i = 0; i < 3; ++i) {
-        cudaError_t e = cudaFuncSetAttribute(k[i], cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-        if (e != cudaSuccess) return e;
-    }
-    // the two schedules are compiled to the same register cap (launch bounds); the batched kernel sizes the full wave
-    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ_outer, k[1], kWarpsPerBlock * 32, smem_outer);
-    if (e != cudaSuccess) return e;
-    // the largest chunk whose work area fits and leaves that residency alone (the grid is sized from it)
-    for (*chunk_outer = kOuterChunkMax; *chunk_outer > 1; --*chunk_outer) {
-        const size_t sc = outer_smem_doubles(blob_doubles, N, *chunk_outer) * sizeof(double);
-        int occ = 0;
-        if (sc > 200 * 1024) continue;
-        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k[1], kWarpsPerBlock * 32, sc);
-        if (e != cudaSuccess) return e;
-        if (occ == *occ_outer) break;
-    }
-    return cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ_gsip, k[2], kWarpsPerBlock * 32, smem_gsip);
-}
-
-// Resident CTAs per SM of k_outer / k_gsip for this shape and trajectory size: the host sizes the grids as
-// SMs x occupancy so that the warp-stride loops run as exactly one full wave (no partial second wave).  k_outer's is taken with a
-// chunk of 1; *chunk_outer is the largest chunk (<= kOuterChunkMax) at which it is still the same.
-cudaError_t query_occupancy(const ShapeParams &S, int N, int blob_doubles, int *occ_outer, int *occ_gsip, int *chunk_outer) {
-    const bool xf = S.has_xform != 0;
-    switch (S.id) {
-#define SVSDF_CASE(ID) \
-    case ID:                 \
-        return xf ? occ_shape<ID, true>(N, blob_doubles, occ_outer, occ_gsip, chunk_outer) \
-                  : occ_shape<ID, false>(N, blob_doubles, occ_outer, occ_gsip, chunk_outer);
-        SVSDF_CASE(SH_STAR)
-        SVSDF_CASE(SH_HORSESHOE)
-        SVSDF_CASE(SH_PIE)
-        SVSDF_CASE(SH_PIE2)
-        SVSDF_CASE(SH_ARC)
-        SVSDF_CASE(SH_TUNNEL)
-        SVSDF_CASE(SH_CUTDISK)
-        SVSDF_CASE(SH_TRAPEZOID)
-        SVSDF_CASE(SH_RHOMBUS)
-        SVSDF_CASE(SH_HEART)
-        SVSDF_CASE(SH_ROUNDEDX)
-        SVSDF_CASE(SH_BIGX)
-        SVSDF_CASE(SH_ROUNDEDCROSS)
-        SVSDF_CASE(SH_VESICA)
-        SVSDF_CASE(SH_MOON)
-        SVSDF_CASE(SH_UNEVENCAPSULE)
-        SVSDF_CASE(SH_CIRCLE)
-#undef SVSDF_CASE
-        case SH_POLYGON: return occ_shape<SH_POLYGON, false>(N, blob_doubles, occ_outer, occ_gsip, chunk_outer);
-        case SH_MESH: return occ_shape<SH_MESH, false>(N, blob_doubles, occ_outer, occ_gsip, chunk_outer);
-        default: return cudaErrorInvalidValue;
-    }
-}
-
-cudaError_t launch_cost_kernels(const KernelArgs &A, const ShapeParams &S, const ScaleSched *Z, int N, int grid_outer, int grid_gsip,
-                                cudaStream_t stream, cudaEvent_t after_outer, int gsip_wide) {
-    LaunchCfg cfg;
-    cfg.after_outer = after_outer;
-    cfg.gsip_wide = gsip_wide != 0;
-    cfg.grid_outer = grid_outer;
-    cfg.grid_gsip = grid_gsip;
-    cfg.smem_outer = outer_smem_doubles(A.blob_doubles, N, A.batched ? A.outer_chunk : 1) * sizeof(double);
-    cfg.smem_gsip = (size_t)A.blob_doubles * sizeof(double);
-    cfg.stream = stream;
-    return S.has_xform ? dispatch<true>(A, S, Z, cfg, N) : dispatch<false>(A, S, Z, cfg, N);
-}
-
-// the rigid units also bring the launchers every variant shares
-#ifndef SVSDF_SCALED_UNIT
-cudaError_t launch_pose_table(double *blob, int K1, PoseRec *w2, PoseRec *w3, cudaStream_t stream) {
-    const int64_t n = K1 + (w2 ? win2_records(K1) : 0) + (w3 ? win3_records(K1) : 0);
-    k_pose_table<<<(unsigned)((n + 127) / 128), 128, 0, stream>>>(blob, w2, w3);
+// Launches one of a variant's kernels on args; a deformable robot's (SCALED) take the scale schedule *Z after them.
+template <bool SCALED, class Kernel, class... Args>
+static cudaError_t launch_cost(Kernel k, int grid, int threads, size_t smem, cudaStream_t st, const ScaleSched *Z, const Args &...args) {
+    if constexpr (SCALED) k<<<grid, threads, smem, st>>>(args..., *Z);
+    else k<<<grid, threads, smem, st>>>(args...);
     return cudaGetLastError();
 }
-
-cudaError_t launch_finalize(const double *partials, int n_blocks, int N, const int *n_inside,
-                            const double *gsip_contrib, const int *gsip_piece, double *tot, unsigned int *ticket,
-                            double *out, cudaStream_t stream) {
-    const int nacc = 19 * N + 1;
-    k_finalize<<<(nacc + 7) / 8, 256, 0, stream>>>(partials, n_blocks, N, n_inside, gsip_contrib, gsip_piece, tot,
-                                                   ticket, out);
-    return cudaGetLastError();
-}
-
-template <int SHAPE, bool XFORM>
-static cudaError_t launch_shape_fn(const ShapeParams &S, const double *rel_xy, int64_t n, double *out, int grad,
-                                   cudaStream_t stream) {
-    int grid = (int)((n + 255) / 256);
-    if (grad) k_shape_grad<SHAPE, XFORM><<<grid, 256, 0, stream>>>(S, rel_xy, n, out);
-    else k_shape_sdf<SHAPE, XFORM><<<grid, 256, 0, stream>>>(S, rel_xy, n, out);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_shape_eval(const ShapeParams &S, const double *rel_xy, int64_t n, double *out, int grad,
-                              cudaStream_t stream) {
-    if (n == 0) return cudaSuccess;
-    switch (S.id) {
-#define SVSDF_CASE(ID)                                                                              \
-    case ID:                                                                                        \
-        return S.has_xform ? launch_shape_fn<ID, true>(S, rel_xy, n, out, grad, stream)             \
-                           : launch_shape_fn<ID, false>(S, rel_xy, n, out, grad, stream);
-        SVSDF_CASE(SH_STAR)
-        SVSDF_CASE(SH_HORSESHOE)
-        SVSDF_CASE(SH_PIE)
-        SVSDF_CASE(SH_PIE2)
-        SVSDF_CASE(SH_ARC)
-        SVSDF_CASE(SH_TUNNEL)
-        SVSDF_CASE(SH_CUTDISK)
-        SVSDF_CASE(SH_TRAPEZOID)
-        SVSDF_CASE(SH_RHOMBUS)
-        SVSDF_CASE(SH_HEART)
-        SVSDF_CASE(SH_ROUNDEDX)
-        SVSDF_CASE(SH_BIGX)
-        SVSDF_CASE(SH_ROUNDEDCROSS)
-        SVSDF_CASE(SH_VESICA)
-        SVSDF_CASE(SH_MOON)
-        SVSDF_CASE(SH_UNEVENCAPSULE)
-        SVSDF_CASE(SH_CIRCLE)
-#undef SVSDF_CASE
-        case SH_POLYGON: return launch_shape_fn<SH_POLYGON, false>(S, rel_xy, n, out, grad, stream);
-        case SH_MESH: return launch_shape_fn<SH_MESH, false>(S, rel_xy, n, out, grad, stream);
-        default: return cudaErrorInvalidValue;
-    }
-}
-
-cudaError_t launch_sincos(const double *x, int64_t n, double *s, double *c, cudaStream_t stream) {
-    if (n == 0) return cudaSuccess;
-    k_sincos<<<(int)((n + 255) / 256), 256, 0, stream>>>(x, n, s, c);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_fp64_peak(double *out, int grid, int iters, cudaStream_t stream) {
-    k_fp64_peak<<<grid, 256, 0, stream>>>(out, iters);
-    return cudaGetLastError();
-}
-
-#endif  // SVSDF_SCALED_UNIT
-#endif  // SVSDF_MULTI_UNIT
 
 }  // namespace SVSDF_NS
 }  // namespace svsdf

@@ -8,9 +8,9 @@
 //  * k_gsip_multi: one queue over the concatenated inside lists; slot s belongs to the problem k with ins_off[k] <= s < ins_off[k + 1].
 //  * k_finalize_multi: blockIdx.y = problem; k_finalize's fixed tree over the problem's grid, then its inside contributions in
 //    ascending point order.
-// Included by svsdf_kernels_multi_{fast,strict}.cu (rigid; these also carry the pose / compaction / finalize kernels) and
-// svsdf_kernels_multi_scaled_{fast,strict}.cu (SVSDF_SCALED_UNIT: the deformable-robot k_outer_multi / k_gsip_multi), after
-// svsdf_kernels.cuh with SVSDF_MULTI_UNIT defined.
+// Included by svsdf_kernels_multi_{fast,strict}.cu (rigid; these also carry the pose / compaction / finalize kernels of
+// svsdf_kernels_multi_shared.cuh) and svsdf_kernels_multi_scaled_{fast,strict}.cu; SVSDF_SCALED (0 / 1) selects the rigid or the
+// deformable-robot k_outer_multi / k_gsip_multi.
 #pragma once
 #include "svsdf_kernels.cuh"
 
@@ -122,161 +122,47 @@ __global__ void __launch_bounds__(WARPS * 32, (WARPS == kWarpsPerBlock && SHAPE 
     gsip_multi_body<SHAPE, XFORM, WARPS, true>(A, M, S, &Z);
 }
 
-#ifndef SVSDF_SCALED_UNIT
-// grid (ceil(max K1 / 128), n): one thread per (problem, layer-1 sample)
-__global__ void k_pose_table_multi(double *blobs, const __grid_constant__ MultiArgs M) {
-    const MultiProblem pr = M.prob[blockIdx.y];
-    pose_table_entry(blobs + pr.blob_off, blockIdx.x * blockDim.x + threadIdx.x);
-}
-
-// one CTA per problem; the last CTA to finish writes the slot offsets of the concatenated inside lists
-__global__ void __launch_bounds__(1024) k_compact_multi(const unsigned char *flag, int *list, const __grid_constant__ MultiArgs M) {
-    const MultiProblem pr = M.prob[blockIdx.x];
-    compact_body(flag + pr.flag_off, pr.P, list + pr.pt_off, M.ins_count + blockIdx.x);
-    __shared__ bool last;
-    __threadfence();
-    __syncthreads();
-    if (threadIdx.x == 0) last = (atomicAdd(M.compact_ticket, 1u) == gridDim.x - 1);
-    __syncthreads();
-    if (!last) return;
-    __threadfence();
-    if (threadIdx.x == 0) {  // n is at most a few thousand: a serial scan is a few microseconds
-        int s = 0;
-        for (int k = 0; k < M.n; ++k) {
-            M.ins_off[k] = s;
-            s += __ldcg(M.ins_count + k);
-        }
-        M.ins_off[M.n] = s;
-        *M.compact_ticket = 0u;
-    }
-}
-
-// grid (ceil(max(19N + 1) / 8), n): problem k uses the first ceil((19 N_k + 1) / 8) CTAs of its row
-__global__ void __launch_bounds__(256) k_finalize_multi(const double *partials, const double *gsip_contrib, const int *gsip_piece,
-                                                        const __grid_constant__ MultiArgs M) {
-    const int k = blockIdx.y;
-    const MultiProblem pr = M.prob[k];
-    const int nbx = (19 * pr.N + 1 + 7) / 8;
-    if ((int)blockIdx.x >= nbx) return;
-    const int off = M.ins_off[k];
-    finalize_body(partials + pr.part_off, pr.grid, pr.N, M.ins_off[k + 1] - off, gsip_contrib + 20 * (int64_t)off, gsip_piece + off,
-                  M.tot + pr.out_off, M.tickets + k, M.out + pr.out_off, blockIdx.x, nbx);
-}
-#endif
-
 // ---- launchers ------------------------------------------------------------------------------------------------------------------
+// the cost kernels of a multi-problem variant, as raise_smem_cap and launch_cost take them
+template <int SHAPE, bool XFORM, bool SCALED>
+struct MultiKernels {
+    static auto outer(bool batched) { return batched ? k_outer_multi<SHAPE, XFORM, true> : k_outer_multi<SHAPE, XFORM, false>; }
+    static auto gsip(bool wide) { return wide ? k_gsip_multi<SHAPE, XFORM, kGsipWarps> : k_gsip_multi<SHAPE, XFORM, kWarpsPerBlock>; }
+};
 template <int SHAPE, bool XFORM>
-static cudaError_t multi_attrs() {
-    static bool attr_set_dev[64] = {};
-    int dev_ord = 0;
-    cudaGetDevice(&dev_ord);
-    bool &attr_set = attr_set_dev[dev_ord & 63];
-    if (attr_set) return cudaSuccess;
-    const void *k[4];
-    if constexpr (kScaledUnit) {
-        k[0] = (const void *)k_outer_multi_scaled<SHAPE, XFORM, false>;
-        k[1] = (const void *)k_outer_multi_scaled<SHAPE, XFORM, true>;
-        k[2] = (const void *)k_gsip_multi_scaled<SHAPE, XFORM, kWarpsPerBlock>;
-        k[3] = (const void *)k_gsip_multi_scaled<SHAPE, XFORM, kGsipWarps>;
-    } else {
-        k[0] = (const void *)k_outer_multi<SHAPE, XFORM, false>;
-        k[1] = (const void *)k_outer_multi<SHAPE, XFORM, true>;
-        k[2] = (const void *)k_gsip_multi<SHAPE, XFORM, kWarpsPerBlock>;
-        k[3] = (const void *)k_gsip_multi<SHAPE, XFORM, kGsipWarps>;
+struct MultiKernels<SHAPE, XFORM, true> {
+    static auto outer(bool batched) { return batched ? k_outer_multi_scaled<SHAPE, XFORM, true> : k_outer_multi_scaled<SHAPE, XFORM, false>; }
+    static auto gsip(bool wide) {
+        return wide ? k_gsip_multi_scaled<SHAPE, XFORM, kGsipWarps> : k_gsip_multi_scaled<SHAPE, XFORM, kWarpsPerBlock>;
     }
-    for (int i = 0; i < 4; ++i) {
-        cudaError_t e = cudaFuncSetAttribute(k[i], cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-        if (e != cudaSuccess) return e;
-    }
-    attr_set = true;
-    return cudaSuccess;
-}
+};
 
 // what: 0 sparse k_outer_multi, 1 batched k_outer_multi, 2 k_gsip_multi (gsip_wide: the 22-warp variant; grid <= 0: resident
 // CTAs per SM x SMs of the chosen variant)
 template <int SHAPE, bool XFORM>
 static cudaError_t launch_multi_shape(int what, const KernelArgs &A, const MultiArgs &M, const ShapeParams &S, const ScaleSched *Z,
                                       int grid, size_t smem, int gsip_wide, int sm_count, cudaStream_t st) {
-    cudaError_t e = multi_attrs<SHAPE, XFORM>();
+    using K = MultiKernels<SHAPE, XFORM, SVSDF_SCALED>;
+    cudaError_t e = raise_smem_cap<K>();
     if (e != cudaSuccess) return e;
-    constexpr int TO = kWarpsPerBlock * 32;
-    if (what == 0 || what == 1) {
-        if constexpr (kScaledUnit) {
-            if (what == 1) k_outer_multi_scaled<SHAPE, XFORM, true><<<grid, TO, smem, st>>>(A, M, S, *Z);
-            else k_outer_multi_scaled<SHAPE, XFORM, false><<<grid, TO, smem, st>>>(A, M, S, *Z);
-        } else {
-            if (what == 1) k_outer_multi<SHAPE, XFORM, true><<<grid, TO, smem, st>>>(A, M, S);
-            else k_outer_multi<SHAPE, XFORM, false><<<grid, TO, smem, st>>>(A, M, S);
-        }
-        return cudaGetLastError();
-    }
-    const void *kg;
-    if constexpr (kScaledUnit) kg = gsip_wide ? (const void *)k_gsip_multi_scaled<SHAPE, XFORM, kGsipWarps> : (const void *)k_gsip_multi_scaled<SHAPE, XFORM, kWarpsPerBlock>;
-    else kg = gsip_wide ? (const void *)k_gsip_multi<SHAPE, XFORM, kGsipWarps> : (const void *)k_gsip_multi<SHAPE, XFORM, kWarpsPerBlock>;
-    const int threads = gsip_wide ? kGsipWarps * 32 : TO;
+    if (what == 0 || what == 1) return launch_cost<SVSDF_SCALED>(K::outer(what == 1), grid, kWarpsPerBlock * 32, smem, st, Z, A, M, S);
+    const auto kg = K::gsip(gsip_wide);
+    const int threads = (gsip_wide ? kGsipWarps : kWarpsPerBlock) * 32;
     if (grid <= 0) {
         int occ = 0;
         e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kg, threads, smem);
         if (e != cudaSuccess) return e;
         grid = gsip_wide ? sm_count : sm_count * (occ > 0 ? occ : 1);
     }
-    if constexpr (kScaledUnit) {
-        if (gsip_wide) k_gsip_multi_scaled<SHAPE, XFORM, kGsipWarps><<<grid, threads, smem, st>>>(A, M, S, *Z);
-        else k_gsip_multi_scaled<SHAPE, XFORM, kWarpsPerBlock><<<grid, threads, smem, st>>>(A, M, S, *Z);
-    } else {
-        if (gsip_wide) k_gsip_multi<SHAPE, XFORM, kGsipWarps><<<grid, threads, smem, st>>>(A, M, S);
-        else k_gsip_multi<SHAPE, XFORM, kWarpsPerBlock><<<grid, threads, smem, st>>>(A, M, S);
-    }
-    return cudaGetLastError();
+    return launch_cost<SVSDF_SCALED>(kg, grid, threads, smem, st, Z, A, M, S);
 }
 
 cudaError_t launch_multi(int what, const KernelArgs &A, const MultiArgs &M, const ShapeParams &S, const ScaleSched *Z, int grid, size_t smem,
                          int gsip_wide, int sm_count, cudaStream_t st) {
-    const bool xf = S.has_xform != 0;
-    switch (S.id) {
-#define SVSDF_CASE(ID)                                                                                      \
-    case ID:                                                                                                \
-        return xf ? launch_multi_shape<ID, true>(what, A, M, S, Z, grid, smem, gsip_wide, sm_count, st)     \
-                  : launch_multi_shape<ID, false>(what, A, M, S, Z, grid, smem, gsip_wide, sm_count, st);
-        SVSDF_CASE(SH_STAR)
-        SVSDF_CASE(SH_HORSESHOE)
-        SVSDF_CASE(SH_PIE)
-        SVSDF_CASE(SH_PIE2)
-        SVSDF_CASE(SH_ARC)
-        SVSDF_CASE(SH_TUNNEL)
-        SVSDF_CASE(SH_CUTDISK)
-        SVSDF_CASE(SH_TRAPEZOID)
-        SVSDF_CASE(SH_RHOMBUS)
-        SVSDF_CASE(SH_HEART)
-        SVSDF_CASE(SH_ROUNDEDX)
-        SVSDF_CASE(SH_BIGX)
-        SVSDF_CASE(SH_ROUNDEDCROSS)
-        SVSDF_CASE(SH_VESICA)
-        SVSDF_CASE(SH_MOON)
-        SVSDF_CASE(SH_UNEVENCAPSULE)
-        SVSDF_CASE(SH_CIRCLE)
-#undef SVSDF_CASE
-        case SH_POLYGON: return launch_multi_shape<SH_POLYGON, false>(what, A, M, S, Z, grid, smem, gsip_wide, sm_count, st);
-        case SH_MESH: return launch_multi_shape<SH_MESH, false>(what, A, M, S, Z, grid, smem, gsip_wide, sm_count, st);
-        default: return cudaErrorInvalidValue;
-    }
+    return dispatch_shape<ShapeSet::all>(S, [&](auto id, auto xf) {
+        return launch_multi_shape<id.value, xf.value>(what, A, M, S, Z, grid, smem, gsip_wide, sm_count, st);
+    });
 }
-
-#ifndef SVSDF_SCALED_UNIT
-cudaError_t launch_pose_multi(double *blobs, const MultiArgs &M, int max_K1, cudaStream_t st) {
-    k_pose_table_multi<<<dim3((max_K1 + 127) / 128, M.n), 128, 0, st>>>(blobs, M);
-    return cudaGetLastError();
-}
-cudaError_t launch_compact_multi(const unsigned char *flag, int *list, const MultiArgs &M, cudaStream_t st) {
-    k_compact_multi<<<M.n, 1024, 0, st>>>(flag, list, M);
-    return cudaGetLastError();
-}
-cudaError_t launch_finalize_multi(const double *partials, const double *gsip_contrib, const int *gsip_piece, const MultiArgs &M, int max_N,
-                                  cudaStream_t st) {
-    k_finalize_multi<<<dim3((19 * max_N + 1 + 7) / 8, M.n), 256, 0, st>>>(partials, gsip_contrib, gsip_piece, M);
-    return cudaGetLastError();
-}
-#endif
 
 }  // namespace SVSDF_NS
 }  // namespace svsdf

@@ -2,5 +2,6 @@
 // compaction and finalize kernels of a multi-problem evaluation.  Kept apart from the single-problem units so that those compile as
 // they did.
 #define SVSDF_NS strict_multi
-#define SVSDF_MULTI_UNIT 1
+#define SVSDF_SCALED 0
 #include "svsdf_kernels_multi.cuh"
+#include "svsdf_kernels_multi_shared.cuh"

@@ -2,5 +2,5 @@
 // scaled k_outer / k_gsip instantiations live here, so they compile in parallel with the rigid units and leave them as
 // they are.
 #define SVSDF_NS fast_scaled
-#define SVSDF_SCALED_UNIT 1
-#include "svsdf_kernels.cuh"
+#define SVSDF_SCALED 1
+#include "svsdf_kernels_single.cuh"

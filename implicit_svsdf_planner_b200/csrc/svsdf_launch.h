@@ -7,9 +7,9 @@
 
 namespace svsdf {
 // Launchers of every kernel variant: the single-problem unit NS (svsdf_kernels_{fast,strict}.cu, and for deformable robots
-// svsdf_kernels_scaled_{fast,strict}.cu) and its multi-problem unit MULTI (svsdf_kernels_multi*.cu, svsdf_cost_grad_multi).  Z, the
-// scale schedule, is read by the scaled units only.  launch_multi: what = 0 sparse / 1 batched k_outer_multi, 2 k_gsip_multi (grid <= 0:
-// one full wave of the chosen variant).
+// svsdf_kernels_scaled_{fast,strict}.cu; svsdf_kernels_single.cuh) and its multi-problem unit MULTI (svsdf_kernels_multi*.cu,
+// svsdf_cost_grad_multi; svsdf_kernels_multi.cuh).  Z, the scale schedule, is read by the scaled units only.  launch_multi: what = 0
+// sparse / 1 batched k_outer_multi, 2 k_gsip_multi (grid <= 0: one full wave of the chosen variant).
 #define SVSDF_DECLARE_LAUNCHERS(NS, MULTI)                                                                        \
     namespace NS {                                                                                               \
     cudaError_t query_occupancy(const ShapeParams &S, int N, int blob_doubles, int *occ_outer, int *occ_gsip,    \
@@ -28,8 +28,8 @@ SVSDF_DECLARE_LAUNCHERS(strict, strict_multi)
 SVSDF_DECLARE_LAUNCHERS(fast_scaled, fast_multi_scaled)
 SVSDF_DECLARE_LAUNCHERS(strict_scaled, strict_multi_scaled)
 #undef SVSDF_DECLARE_LAUNCHERS
-// Only the rigid units define these; the scaled variants use them too.  The multi-problem ones run the pose table, the compaction and the
-// finalize of every multi launch.
+// Only the rigid units define these (svsdf_kernels_shared.cuh, svsdf_kernels_multi_shared.cuh); the scaled variants use them too.  The
+// multi-problem ones run the pose table, the compaction and the finalize of every multi launch.
 #define SVSDF_DECLARE_RIGID_LAUNCHERS(NS, MULTI)                                                                  \
     namespace NS {                                                                                               \
     cudaError_t launch_pose_table(double *blob, int K1, PoseRec *w2, PoseRec *w3, cudaStream_t stream);          \

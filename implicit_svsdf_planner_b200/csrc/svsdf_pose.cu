@@ -164,30 +164,8 @@ cudaError_t launch_shape(const PoseArgs &A, const ShapeParams &S, int max_items,
 
 cudaError_t launch_pose(const PoseArgs &A, const ShapeParams &S, int max_items, cudaStream_t st) {
     if (A.n <= 0 || max_items <= 0) return cudaSuccess;
-    switch (S.id) {
-#define SVSDF_CASE(ID) \
-    case ID: return S.has_xform ? launch_shape<ID, true>(A, S, max_items, st) : launch_shape<ID, false>(A, S, max_items, st);
-        SVSDF_CASE(SH_STAR)
-        SVSDF_CASE(SH_HORSESHOE)
-        SVSDF_CASE(SH_PIE)
-        SVSDF_CASE(SH_PIE2)
-        SVSDF_CASE(SH_ARC)
-        SVSDF_CASE(SH_TUNNEL)
-        SVSDF_CASE(SH_CUTDISK)
-        SVSDF_CASE(SH_TRAPEZOID)
-        SVSDF_CASE(SH_RHOMBUS)
-        SVSDF_CASE(SH_HEART)
-        SVSDF_CASE(SH_ROUNDEDX)
-        SVSDF_CASE(SH_BIGX)
-        SVSDF_CASE(SH_ROUNDEDCROSS)
-        SVSDF_CASE(SH_VESICA)
-        SVSDF_CASE(SH_MOON)
-        SVSDF_CASE(SH_UNEVENCAPSULE)
-        SVSDF_CASE(SH_CIRCLE)
-#undef SVSDF_CASE
-        case SH_POLYGON: return launch_shape<SH_POLYGON, false>(A, S, max_items, st);
-        default: return cudaErrorInvalidValue;  // the mesh functor is refused by svsdf_set_pose_penalty
-    }
+    // the mesh functor is refused by svsdf_set_pose_penalty
+    return dispatch_shape<ShapeSet::no_mesh>(S, [&](auto id, auto xf) { return launch_shape<id.value, xf.value>(A, S, max_items, st); });
 }
 
 }  // namespace SVSDF_NS

@@ -141,7 +141,7 @@ OuterPlan outer_plan(const svsdf_ctx *ctx, int64_t P, const Occupancy &occ) {
 int outer_chunk(const svsdf_ctx *ctx, const Occupancy &occ, int64_t rounds, int blob, int N) {
     int64_t c = std::min<int64_t>(occ.chunk, rounds);
     if (ctx->hooks.force_outer_chunk > 0) c = std::min(ctx->hooks.force_outer_chunk, kOuterChunkMax);  // test hook
-    while (c > 1 && outer_smem_doubles(blob, N, (int)c) * sizeof(double) > 200 * 1024) --c;
+    while (c > 1 && outer_smem_doubles(blob, N, (int)c) * sizeof(double) > kMaxDynSmemBytes) --c;
     return (int)std::max<int64_t>(c, 1);
 }
 int64_t outer_rounds(int64_t P, int grid) {
@@ -202,7 +202,7 @@ int run_kernels(svsdf_ctx *ctx, const double *d_points, int64_t P, bool reduce, 
     if (gp.grid == 0) gp.grid = gp.wide ? ctx->sm_count : ctx->sm_count * occ.gsip;
     if (!gsip) CK(cudaMemsetAsync(ctx->d_n_inside, 0, sizeof(int), ctx->stream));
     size_t smem = outer_smem_doubles(A.blob_doubles, N, 1) * sizeof(double);
-    if (smem > 200 * 1024) {
+    if (smem > kMaxDynSmemBytes) {
         ctx->err = "svsdf: trajectory blob does not fit in shared memory";
         return SVSDF_ERR_INVALID;
     }

@@ -29,7 +29,7 @@ int plan_multi(svsdf_ctx *ctx, MultiPlan &pl) {
         if (batched) pl.max_rounds = std::max(pl.max_rounds, outer_rounds(m.P, G));
     }
     for (int b = 0; b < 2; ++b)
-        if (outer_smem_doubles(pl.smax_blob[b], pl.smax_N[b], 1) * sizeof(double) > 200 * 1024) {
+        if (outer_smem_doubles(pl.smax_blob[b], pl.smax_N[b], 1) * sizeof(double) > kMaxDynSmemBytes) {
             ctx->err = "svsdf: trajectory blob does not fit in shared memory";
             return SVSDF_ERR_INVALID;
         }

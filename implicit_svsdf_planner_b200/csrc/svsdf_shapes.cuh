@@ -3,6 +3,11 @@
 // Operation order follows the reference so that a -fmad=false build differs from the CPU only through
 // libm (sin/cos); every function takes the body-frame point AFTER the shape pre-transform.
 #pragma once
+#include <cuda_runtime.h>
+
+#include <type_traits>
+#include <utility>
+
 #include "svsdf_sincos.cuh"
 #include "svsdf_types.h"
 
@@ -674,4 +679,29 @@ __device__ __forceinline__ void circle_grad1(const ShapeParams &S, double rx, do
 }
 
 }  // namespace dev
+
+// The functors a kernel family is compiled for.  Each set's value is one past its last id (the ids are contiguous): every functor, every
+// functor but the mesh (the pose penalty), or the analytic ones (the A* front end: the reference has no rotated kernels for the others).
+enum class ShapeSet { all = SH_COUNT, no_mesh = SH_MESH, analytic = SH_POLYGON };
+
+template <int ID, class F>
+cudaError_t call_shape(const ShapeParams &S, F &f) {
+    if constexpr (ID < SH_POLYGON)  // only the analytic functors apply the pre-transform
+        if (S.has_xform) return f(std::integral_constant<int, ID>{}, std::true_type{});
+    return f(std::integral_constant<int, ID>{}, std::false_type{});
+}
+template <class F, int... IDS>
+cudaError_t dispatch_ids(const ShapeParams &S, F &f, std::integer_sequence<int, IDS...>) {
+    cudaError_t e = cudaErrorInvalidValue;
+    (void)((S.id == IDS && ((e = call_shape<IDS>(S, f)), true)) || ...);
+    return e;
+}
+
+// Host-side shape dispatch of every launcher: f(id, xform) with S's functor id and pre-transform flag as std::integral_constant, so
+// that f can instantiate its kernel on them.  An id outside SET returns cudaErrorInvalidValue.
+template <ShapeSet SET, class F>
+cudaError_t dispatch_shape(const ShapeParams &S, F &&f) {
+    return dispatch_ids(S, f, std::make_integer_sequence<int, (int)SET>{});
+}
+
 }  // namespace svsdf

@@ -134,6 +134,8 @@ constexpr int kOuterChunkMax = 4;
 SVSDF_HD inline size_t outer_smem_doubles(int blob_doubles, int N, int chunk) {
     return (size_t)blob_doubles + (size_t)kWarpsPerBlock * (19 * N + 1) + (size_t)chunk * kWarpsPerBlock * 128;
 }
+// the dynamic shared memory k_outer / k_gsip opt in to (cudaFuncAttributeMaxDynamicSharedMemorySize); the host refuses larger launches
+constexpr int kMaxDynSmemBytes = 200 * 1024;
 
 // Penalty parameters (star.yaml: weight_p 60, safety_hor 0.7; smoothedL1 mu = 0.01 is a literal in the
 // reference, back_end_optimizer.hpp:1052)
