@@ -371,7 +371,9 @@ def _scale(a, b=(0.0, 0.0), w=(0.0, 0.0), phi=(0.0, 0.0)) -> Scale:
 
 
 def scale_matrix(t, a, b=(0.0, 0.0), w=(0.0, 0.0), phi=(0.0, 0.0)):
-    """(S(t), St.inverse()) as 3 x 3 arrays, with the kernels' arithmetic (svsdf_scale_matrix)."""
+    """(S(t), St.inverse()) as 3 x 3 arrays, with the kernels' arithmetic (svsdf_scale_matrix).  Raises SvsdfError for a
+    schedule Context.set_scale refuses (per axis a - |b| >= 1e-6, a + |b| <= 1e6, |w| * 300 + |phi| < 1e6, all finite) or a
+    non-finite t."""
     z = _scale(a, b, w, phi)
     S, Si = np.empty(9), np.empty(9)
     rc = lib().svsdf_scale_matrix(C.byref(z), float(t), _p(S), _p(Si))
@@ -757,7 +759,9 @@ class Context:
 
     def set_scale(self, a=None, b=(0.0, 0.0), w=(0.0, 0.0), phi=(0.0, 0.0)):
         """Deformable robot: S(t) = diag(a_x + sin(w_x t + phi_x) b_x, a_y + sin(w_y t + phi_y) b_y, 1) for every later query,
-        cost and evaluation on this context (e.g. set_scale(**EXAMPLE_SCALE)).  set_scale(None): rigid again (the default)."""
+        cost and evaluation on this context (e.g. set_scale(**EXAMPLE_SCALE)).  set_scale(None): rigid again (the default).
+        Valid schedules are finite with, per axis, a - |b| >= 1e-6 and a + |b| <= 1e6 (every s(t) in [1e-6, 1e6]: St.inverse()
+        stays finite and non-zero) and |w| * 300 + |phi| < 1e6; anything else raises SvsdfError."""
         if a is None:
             self._ck(lib().svsdf_set_scale(self.h, None), "svsdf_set_scale")
             return

@@ -266,7 +266,10 @@ bool scale_valid(const svsdf_scale &z) {
         const double v[4] = {z.a[d], z.b[d], z.w[d], z.phi[d]};
         for (double x : v)
             if (!std::isfinite(x)) return false;
-        if (!(z.a[d] - std::fabs(z.b[d]) > 0.0)) return false;  // S(t) stays invertible: |sin| <= 1, rounding is monotone
+        // s_d(t) stays in [kScaleMin, kScaleMax] at every t (|sin| <= 1, rounding is monotone), so fl(sy * sx) is a normal
+        // number and the cofactor inverse 1/fl(sy * sx) and St^-1 are finite and non-zero.  a_d - |b_d| > 0 alone is not
+        // enough: a = 1e-160 makes fl(sy * sx) subnormal and 1/det = inf, a = 1e160 makes it inf and St^-1 = 0
+        if (!(z.a[d] - std::fabs(z.b[d]) >= kScaleMin && z.a[d] + std::fabs(z.b[d]) <= kScaleMax)) return false;
         if (!(std::fabs(z.w[d]) * kMaxDuration + std::fabs(z.phi[d]) < 1e6)) return false;
     }
     return true;
@@ -495,7 +498,7 @@ int svsdf_set_scale(svsdf_ctx *ctx, const svsdf_scale *scale) {
         return SVSDF_OK;
     }
     if (!scale_valid(*scale)) {
-        ctx->err = "svsdf_set_scale: schedule must be finite with a_d - |b_d| > 0 and |w_d| * 300 + |phi_d| < 1e6";
+        ctx->err = "svsdf_set_scale: schedule must be finite with a_d - |b_d| >= 1e-6, a_d + |b_d| <= 1e6 and |w_d| * 300 + |phi_d| < 1e6";
         return SVSDF_ERR_INVALID;
     }
     for (int d = 0; d < 2; ++d) {

@@ -80,7 +80,9 @@ struct ShapeParams {
 };
 
 // Deformable robot (svsdf_set_scale; the reference's getScale hook, sw_manager.hpp:495-503): per axis d = x, y
-// s_d(t) = a_d + sin(w_d t + phi_d) b_d, s_z = 1.  Passed by value to the scaled kernels only.
+// s_d(t) = a_d + sin(w_d t + phi_d) b_d, s_z = 1.  Passed by value to the scaled kernels only.  An accepted schedule keeps
+// every s_d(t) in [kScaleMin, kScaleMax] (svsdf_set_scale).
+constexpr double kScaleMin = 1e-6, kScaleMax = 1e6;
 struct ScaleSched {
     double a[2], b[2], w[2], phi[2];
 };

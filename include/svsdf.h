@@ -110,8 +110,11 @@ int svsdf_set_traj(svsdf_ctx *ctx, int N, const double *T, const double *coeffs)
 
 /* Deformable robots: the reference's `useScale` switch and its `getScale(t)` hook (sw_manager.hpp:17, :495-503) as a
  * schedule.  Per axis d = x, y: s_d(t) = a_d + sin(w_d t + phi_d) b_d; s_z = 1.  The reference's commented example is
- * a = (0.8, 0.8), b = (0.6, 0.4), w = (1.5, 1.8), phi = (-1.0, 0.0).  Valid: every value finite, a_d - |b_d| > 0 (S stays
- * invertible) and |w_d| * 300 + |phi_d| < 1e6 (the sin argument stays in the range of the fast reduction). */
+ * a = (0.8, 0.8), b = (0.6, 0.4), w = (1.5, 1.8), phi = (-1.0, 0.0).  Valid: every value finite, a_d - |b_d| >= 1e-6 and
+ * a_d + |b_d| <= 1e6 (every s_d(t) in [1e-6, 1e6], so det = sy sx is a normal number and St.inverse() is finite and non-zero;
+ * a_d - |b_d| > 0 alone admits a = 1e-160, whose det underflows, and a = 1e160, whose det overflows) and
+ * |w_d| * 300 + |phi_d| < 1e6 (the sin argument stays in the range of the fast reduction).  svsdf_scale_matrix applies the
+ * same test. */
 typedef struct svsdf_scale {
     double a[2], b[2], w[2], phi[2];
 } svsdf_scale;

@@ -74,8 +74,27 @@ void sorc_set_traj(void *h, int N, const double *T, const double *coeffs) {
 }
 double sorc_duration(void *h) { return ((ScaledOracle *)h)->sv.traj_duration; }
 void sorc_traj_pos(void *h, double t, double *p3) { ((ScaledOracle *)h)->sv.traj.getPos(t, p3); }
+void sorc_traj_vel(void *h, double t, double *v3) { ((ScaledOracle *)h)->sv.traj.getVel(t, v3); }
+// getSDFAtTimeStamp at one absolute time t: scaled != 0 the descent's getSDFAtTimeStamp<true>, scaled == 0 the rigid one of
+// the seed scan (choiceTInit stays rigid)
+double sorc_sdf_at(void *h, const double *p3, double t, int scaled) {
+    const ScaledSweptVolume &sv = ((ScaledOracle *)h)->sv;
+    return scaled ? sv.sdfAtS(p3, t) : sv.sdfAt(p3, t);
+}
 void sorc_gradient_descent(void *h, const double *p3, double tmin, double tmax, double x0, double *fx, double *x) {
     ((ScaledOracle *)h)->sv.gradientDescentS(tmin, tmax, x0, *fx, *x, p3);
+}
+// getSDFofSweptVolume<false,true> per point: the outer solve alone (body-frame gradient); pts stride 3
+void sorc_query_outer(void *h, int64_t P, const double *pts, double *sdf, double *tstar, double *grad3) {
+    ScaledOracle *o = (ScaledOracle *)h;
+#pragma omp parallel for num_threads(o->cp.threads) schedule(dynamic)
+    for (int64_t i = 0; i < P; ++i) {
+        double p[3] = {pts[3 * i], pts[3 * i + 1], pts[3 * i + 2]};
+        double g[3], ts = 0;
+        sdf[i] = o->sv.getSDFofSweptVolumeS(p, ts, g);
+        tstar[i] = ts;
+        grad3[3 * i] = g[0]; grad3[3 * i + 1] = g[1]; grad3[3 * i + 2] = g[2];
+    }
 }
 // getTrueSDFofSweptVolume<true> per point (world-frame direction for sdf <= 0); pts stride 3
 void sorc_query(void *h, int64_t P, const double *pts, double *sdf, double *tstar, double *grad3, int *rounds) {

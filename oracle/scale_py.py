@@ -62,7 +62,11 @@ def lib(variant: str = "default"):
         L.sorc_duration.restype = C.c_double
         L.sorc_duration.argtypes = [vp]
         L.sorc_traj_pos.argtypes = [vp, C.c_double, dp]
+        L.sorc_traj_vel.argtypes = [vp, C.c_double, dp]
+        L.sorc_sdf_at.restype = C.c_double
+        L.sorc_sdf_at.argtypes = [vp, dp, C.c_double, C.c_int]
         L.sorc_gradient_descent.argtypes = [vp, dp, C.c_double, C.c_double, C.c_double, dp, dp]
+        L.sorc_query_outer.argtypes = [vp, C.c_int64, dp, dp, dp, dp]
         L.sorc_query.argtypes = [vp, C.c_int64, dp, dp, dp, dp, C.POINTER(C.c_int)]
         L.sorc_cost_grad.restype = C.c_int64
         L.sorc_cost_grad.argtypes = [vp, C.c_int, dp, dp, dp, dp, dp, dp]
@@ -130,11 +134,29 @@ class ScaledOracle:
         self.L.sorc_traj_pos(self.h, float(t), _p(out))
         return out
 
+    def traj_vel(self, t):
+        out = np.empty(3)
+        self.L.sorc_traj_vel(self.h, float(t), _p(out))
+        return out
+
+    def sdf_at(self, p, t, scaled=True):
+        """getSDFAtTimeStamp at absolute time t: scaled (the descent's) or rigid (the seed scan's)."""
+        p = _f64(p)
+        return self.L.sorc_sdf_at(self.h, _p(p), float(t), int(bool(scaled)))
+
     def gradient_descent(self, p, tmin, tmax, x0):
         p = _f64(p)
         fx, x = C.c_double(), C.c_double()
         self.L.sorc_gradient_descent(self.h, _p(p), tmin, tmax, x0, C.cast(C.byref(fx), dp), C.cast(C.byref(x), dp))
         return fx.value, x.value
+
+    def query_outer(self, pts):
+        """The outer solve alone (choiceTInit rigid + the scaled descent): sdf, t*, body-frame gradient per point."""
+        pts = _f64(pts).reshape(-1, 3)
+        n = pts.shape[0]
+        sdf, ts, g = np.empty(n), np.empty(n), np.empty((n, 3))
+        self.L.sorc_query_outer(self.h, n, _p(pts), _p(sdf), _p(ts), _p(g))
+        return sdf, ts, g
 
     def query(self, pts):
         pts = _f64(pts).reshape(-1, 3)
