@@ -67,7 +67,7 @@ HEADERS = [
     "host/astar_flat.hpp",
     "host/fwn_bvh.hpp",
     "host/mid_end.hpp",
-    "host/rendezvous.hpp",
+    "host/lockstep.hpp",
     "../../include/svsdf.h",
 ]
 

@@ -1,13 +1,10 @@
 // svsdf_runtime_backend.cpp — the back-end optimisers: the host L-BFGS (svsdf_lbfgs_minimize, svsdf_optimize and its LMBM
 // plug-in, svsdf_optimize_batch), the lock-step back end (svsdf_optimize_lockstep) and the device back end (svsdf_optimize_device).
-#include <pthread.h>
-
 #include <algorithm>
 #include <chrono>
 #include <cmath>
-#include <functional>
 
-#include "host/rendezvous.hpp"
+#include "host/lockstep.hpp"
 #include "svsdf_runtime.h"
 
 extern "C" {
@@ -139,44 +136,17 @@ int svsdf_optimize_batch(svsdf_ctx *const *ctxs, int n_ctx, const svsdf_problem 
 }
 
 namespace {
-// One problem in flight of svsdf_optimize_lockstep: its thread, solver and host evaluation state.
+// One slot of svsdf_optimize_lockstep: the host evaluation state of the problem in it and its device record.
 struct LockstepSlot {
-    svsdf_ctx *ctx = nullptr;
-    host::Rendezvous *rv = nullptr;
-    std::function<void(const std::vector<int> &)> *fire = nullptr;
-    int index = 0;
-    const svsdf_lockstep_problem *pr = nullptr;
     HostEval he;
     MultiItem item;
     std::vector<double> out, pose_out;
+    double *f0_out = nullptr;
     int last_status = SVSDF_OK;
     int evals = 0;
     double gpu_ms = 0.0;
+    std::chrono::steady_clock::time_point t0;
 };
-
-static double lockstep_evaluate(void *inst, const double *x, double *g, const int n) {
-    LockstepSlot &s = *static_cast<LockstepSlot *>(inst);
-    const int N = s.he.N;
-    if (n != N + 3 * (N - 1)) {
-        s.last_status = SVSDF_ERR_NOT_READY;
-        return NAN;
-    }
-    s.he.forward(x);
-    s.item.T = s.he.times.data();
-    s.item.coeffs = s.he.minco.getCoeffs();
-    s.item.rc = SVSDF_OK;
-    s.rv->arrive(s.index, *s.fire);
-    if (s.item.rc != SVSDF_OK) {
-        s.last_status = s.item.rc;
-        return NAN;
-    }
-    double pos = 0.0, other = 0.0;
-    const double cost = s.he.backward(s.out.data(), x, s.ctx->rho, s.ctx->pose_penalty(), s.pose_out.data(), s.ctx->dynamics(), g, &pos,
-                                      &other);
-    if (s.evals++ == 0 && s.pr->f0_out) *s.pr->f0_out = cost;
-    s.last_status = SVSDF_OK;
-    return cost;
-}
 }  // namespace
 
 int svsdf_optimize_lockstep(svsdf_ctx *ctx, const svsdf_lockstep_problem *problems, int n, const svsdf_lbfgs_params *params, int max_in_flight,
@@ -195,28 +165,13 @@ int svsdf_optimize_lockstep(svsdf_ctx *ctx, const svsdf_lockstep_problem *proble
         return SVSDF_ERR_INVALID;
     }
     std::vector<LockstepSlot> slots(M);
-    host::Rendezvous rv(M);
+    std::vector<MultiItem> items;
     int round_err = SVSDF_OK;
-    // the round: every waiting slot's trajectory and points through one multi evaluation
-    std::function<void(const std::vector<int> &)> fire = [&](const std::vector<int> &ready) {
-        std::vector<MultiItem> items;
-        items.reserve(ready.size());
-        for (int s : ready) items.push_back(slots[s].item);
-        float ms = 0.0f;
-        int rc = run_multi(ctx, items.data(), (int)items.size(), ctx->time_kernels ? &ms : nullptr);
-        ctx->backend.round_eval_ms += ms;
-        for (size_t j = 0; j < ready.size(); ++j) {
-            LockstepSlot &s = slots[ready[j]];
-            s.item.rc = rc != SVSDF_OK ? rc : items[j].rc;
-            s.gpu_ms += ms;
-        }
-        if (rc != SVSDF_OK && round_err == SVSDF_OK) round_err = rc;
-    };
-    std::atomic<int> next{0};
-    auto solve = [&](LockstepSlot &s, int k) {
+    auto enter = [&](int slot, int k) {
+        LockstepSlot &s = slots[slot];
         const svsdf_lockstep_problem &p = problems[k];
-        const int N = p.N, nv = N + 3 * (N - 1);
-        s.pr = &p;
+        const int N = p.N;
+        s.t0 = std::chrono::steady_clock::now();
         s.he.setup(p.initS, p.finalS, N);
         s.out.assign((size_t)19 * N + 2, 0.0);
         s.item = MultiItem();
@@ -225,56 +180,53 @@ int svsdf_optimize_lockstep(svsdf_ctx *ctx, const svsdf_lockstep_problem *proble
             s.pose_out.assign((size_t)4 * N * (ctx->pose.res + 1), 0.0);
             s.item.pose_out = s.pose_out.data();
         }
+        s.f0_out = p.f0_out;
         s.last_status = SVSDF_OK;
         s.evals = 0;
         s.gpu_ms = 0.0;
-        host::Lbfgs solver(hp);
-        const auto t0 = std::chrono::steady_clock::now();
-        const host::LbfgsResult R = solver.minimize(p.opt_x, nv, lockstep_evaluate, &s, nullptr, nullptr);
-        const auto t1 = std::chrono::steady_clock::now();
-        s.he.finish(p.opt_x, R, std::chrono::duration<double>(t1 - t0).count(), s.gpu_ms * 1e-3, p.T_out, p.coeffs_out,
-                    stats_out ? &stats_out[k] : nullptr);
-        int ret = optimize_status(R.status);
-        if (s.last_status != SVSDF_OK) ret = s.last_status;
-        if (status_out) status_out[k] = ret;
+        return host::LockstepEntry{p.opt_x, N + 3 * (N - 1), hp};
     };
-    // A thread takes problems from the counter until none is left (going on with the next problem keeps its place among the live
-    // problems), and departs once, at the end.
-    struct ThreadArg { LockstepSlot *s; decltype(solve) *solve; host::Rendezvous *rv; std::function<void(const std::vector<int> &)> *fire;
-                       std::atomic<int> *next; int n; };
-    std::vector<ThreadArg> args(M);
-    auto body = [](void *a) -> void * {
-        ThreadArg &t = *static_cast<ThreadArg *>(a);
-        for (int k = t.next->fetch_add(1); k < t.n; k = t.next->fetch_add(1)) (*t.solve)(*t.s, k);
-        t.rv->depart(*t.fire);
-        return nullptr;
+    // the round: every slot's host forward half, one multi evaluation of all their trajectories and points, every slot's backward half
+    auto round = [&](std::vector<host::LockstepEval> &evals) {
+        const int count = (int)evals.size();
+        items.resize(count);
+#pragma omp parallel for schedule(dynamic)
+        for (int j = 0; j < count; ++j) {
+            LockstepSlot &s = slots[evals[j].slot];
+            s.he.forward(evals[j].x);
+            items[j] = s.item;
+            items[j].T = s.he.times.data();
+            items[j].coeffs = s.he.minco.getCoeffs();
+        }
+        float ms = 0.0f;
+        const int rc = run_multi(ctx, items.data(), count, &ms);
+        ctx->backend.round_eval_ms += ms;
+        if (rc != SVSDF_OK && round_err == SVSDF_OK) round_err = rc;
+#pragma omp parallel for schedule(dynamic)
+        for (int j = 0; j < count; ++j) {
+            host::LockstepEval &e = evals[j];
+            LockstepSlot &s = slots[e.slot];
+            s.gpu_ms += ms;
+            // a failed evaluation hands the machine NaN, and its error stays the problem's status unless a later one succeeds
+            s.last_status = rc != SVSDF_OK ? rc : items[j].rc;
+            if (s.last_status != SVSDF_OK) {
+                e.f = NAN;
+                continue;
+            }
+            double pos = 0.0, other = 0.0;
+            e.f = s.he.backward(s.out.data(), e.x, ctx->rho, ctx->pose_penalty(), s.pose_out.data(), ctx->dynamics(), e.g, &pos, &other);
+            if (s.evals++ == 0 && s.f0_out) *s.f0_out = e.f;
+        }
     };
-    ctx->time_kernels = true;
-    std::vector<pthread_t> th(M);
-    pthread_attr_t attr;
-    pthread_attr_init(&attr);
-    pthread_attr_setstacksize(&attr, (size_t)1 << 20);  // the solver and MINCO keep their arrays on the heap
-    int started = 0;
-    for (int s = 0; s < M; ++s) {
-        slots[s].ctx = ctx; slots[s].rv = &rv; slots[s].fire = &fire; slots[s].index = s;
-        args[s] = ThreadArg{&slots[s], &solve, &rv, &fire, &next, n};
-    }
-    for (int s = 0; s < M; ++s) {
-        if (pthread_create(&th[s], &attr, body, &args[s]) != 0) break;
-        ++started;
-    }
-    pthread_attr_destroy(&attr);
-    if (started < M) {
-        // fewer threads than slots (the system refused more): the missing slots leave without a problem — fewer problems in flight,
-        // the same results — and with no thread at all this thread runs slot 0
-        for (int s = std::max(started, 1); s < M; ++s) rv.depart(fire);
-        if (started == 0) body(&args[0]);
-    }
-    for (int s = 0; s < started; ++s) pthread_join(th[s], nullptr);
-    ctx->time_kernels = false;
-    ctx->backend.lockstep_rounds = rv.rounds();
-    if (round_err != SVSDF_OK) return round_err;
-    return SVSDF_OK;
+    auto leave = [&](int slot, int k, const host::LbfgsResult &R) {
+        LockstepSlot &s = slots[slot];
+        const svsdf_lockstep_problem &p = problems[k];
+        const double seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - s.t0).count();
+        s.he.finish(p.opt_x, R, seconds, s.gpu_ms * 1e-3, p.T_out, p.coeffs_out, stats_out ? &stats_out[k] : nullptr);
+        if (status_out) status_out[k] = s.last_status != SVSDF_OK ? s.last_status : optimize_status(R.status);
+    };
+    ctx->backend.lockstep_rounds = host::lockstep_run(n, M, enter, round, leave);
+    return round_err;
 }
 
 int svsdf_optimize_device(svsdf_ctx *ctx, const svsdf_lockstep_problem *problems, int n, const svsdf_lbfgs_params *params, int max_in_flight,

@@ -222,9 +222,9 @@ _ASTAR_REASON = {0: "start or goal outside the map", 2: "front end found no path
                  4: "path longer than max_path", -1: "front end internal guard"}
 
 
-# Problems from which the back end runs on the device (svsdf_optimize_device) rather than on host threads (svsdf_optimize_lockstep); both
-# give the same bits.  Measured on an H100 (tests/tools/run_optimize_device.py, DESIGN §7): the device wins at 427 and 843 problems
-# (1.9x, 1.3x) and loses at 216 (0.88x); at 109 the two are within the run-to-run spread.
+# Problems from which the back end runs on the device (svsdf_optimize_device) rather than on the host, with its machines advanced round
+# by round (svsdf_optimize_lockstep); both give the same bits.  Measured on an H100 (tests/tools/run_optimize_device.py, DESIGN §7): the
+# device wins at 427 and 843 problems (1.9x, 1.3x) and loses at 216 (0.88x); at 109 the two are within the run-to-run spread.
 DEVICE_BACK_END_MIN_PROBLEMS = 256
 
 

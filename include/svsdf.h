@@ -492,13 +492,14 @@ typedef struct {
 int svsdf_cost_grad_multi(svsdf_ctx *ctx, int n, const svsdf_multi_problem *problems);
 
 /* svsdf_optimize_lockstep: n back ends on one context, in lock-step.  Up to max_in_flight problems (<= 0: min(n, 1024)) are in flight,
- * each on its own host thread running the built-in L-BFGS (the solver of svsdf_optimize, unchanged); a thread that finishes takes the
- * next problem.  Each evaluation does its host half (tau -> T, MINCO, energy; afterwards the adjoint and rho * sum(T)) on its thread and
- * meets the others at a rendezvous: once every live problem is waiting, ONE svsdf_cost_grad_multi-style round evaluates all of them.
- * Per problem, opt_x, T_out, coeffs_out, status_out (svsdf_optimize's return value) and stats_out (final cost, iterations,
- * evaluations, status) equal svsdf_optimize on the same inputs bit for bit, whatever max_in_flight and the order in which problems are
- * taken; stats seconds / gpu_seconds are the problem's wall time and the device time of the rounds it took part in.  f0_out (optional)
- * receives the cost of the first evaluation, i.e. at the start point.  Inputs are checked like svsdf_optimize's (2 <= N <= 64, non-null
+ * each a machine of the built-in L-BFGS (the solver of svsdf_optimize, unchanged) in a slot; a problem that finishes hands its slot
+ * to the next.  The calling thread advances the machines round by round: every live problem asks for an evaluation, and ONE
+ * svsdf_cost_grad_multi-style round evaluates all of them, with each problem's host half (tau -> T, MINCO, energy; afterwards the
+ * adjoint and rho * sum(T)) and its solver step spread over OpenMP threads.  Per problem, opt_x, T_out, coeffs_out, status_out
+ * (svsdf_optimize's return value) and stats_out (final cost, iterations, evaluations, status) equal svsdf_optimize on the same
+ * inputs bit for bit, whatever max_in_flight and the order in which problems are taken; stats seconds / gpu_seconds are the problem's
+ * wall time (from entering its slot to leaving it) and the device time of the rounds it took part in.  f0_out (optional) receives
+ * the cost of the first evaluation, i.e. at the start point.  Inputs are checked like svsdf_optimize's (2 <= N <= 64, non-null
  * initS / finalS / opt_x, P >= 0, stride >= 2, points when P > 0): one invalid problem refuses the call.  A context with an LMBM library
  * (svsdf_set_lmbm_library) is refused with SVSDF_ERR_INVALID.  Returns SVSDF_OK, or the error of a failed round (every problem of that
  * round then ends with it, as svsdf_optimize ends on a failed evaluation).  svsdf_lockstep_rounds: the rounds of the last call. */
@@ -518,7 +519,7 @@ int svsdf_lockstep_rounds(const svsdf_ctx *ctx, int64_t *rounds);
 
 /* svsdf_optimize_device: svsdf_optimize_lockstep with the back end on the device.  Every problem in flight keeps its L-BFGS state, its
  * MINCO spline and its query points (uploaded once, when it enters a slot) in device memory; one warp per problem runs the host's own
- * solver and MINCO code (host/lbfgs.hpp, host/minco.hpp) between the evaluations, so no host thread per problem is needed.  A round is
+ * solver and MINCO code (host/lbfgs.hpp, host/minco.hpp) between the evaluations, so the machines never leave the device.  A round is
  * one small download of every slot's state, the host's launch plan (each problem keeps the grid of its single call), one small upload
  * and the launches; the launches per round do not depend on n.  Same problems, checks, refusals and results as svsdf_optimize_lockstep
  * (bit for bit svsdf_optimize per problem: opt_x, T_out, coeffs_out, f0_out, stats and status_out), plus: max_in_flight above 65535 is
@@ -532,7 +533,7 @@ int svsdf_optimize_device(svsdf_ctx *ctx, const svsdf_lockstep_problem *problems
                           svsdf_opt_stats *stats_out, int *status_out, int64_t *rounds_out);
 /* svsdf_round_times: device time (ms) of the rounds of the last svsdf_optimize_lockstep / svsdf_optimize_device call: the evaluation
  * kernels (pose table to finalize) and the back-end kernels (blobs and the device L-BFGS / MINCO; 0 for svsdf_optimize_lockstep, whose
- * back end runs on host threads). */
+ * machines are advanced round by round on the host). */
 int svsdf_round_times(const svsdf_ctx *ctx, double *eval_ms, double *backend_ms);
 
 /* ---- "next" row (SURVEY.md §8f rank 1): query-point construction on the device --------------------------------------

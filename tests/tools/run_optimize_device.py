@@ -1,6 +1,6 @@
-"""Back-end measurement: the lock-step back end on host threads (svsdf_optimize_lockstep) against the device back end
-(svsdf_optimize_device) on the inputs of run_plan_batch.py's four workloads (star scene and grid60 at n = 256 and 1024), taken from
-plan.plan_batch(back_end=False).  The two arms alternate in one process, three runs each, on one context; every problem's result must be
+"""Back-end measurement: the lock-step back end on the host, its machines advanced round by round (svsdf_optimize_lockstep), against
+the device back end (svsdf_optimize_device) on the inputs of run_plan_batch.py's four workloads (star scene and grid60 at n = 256 and
+1024), taken from plan.plan_batch(back_end=False).  The two arms alternate in one process, three runs each, on one context; every problem's result must be
 identical between them (status, iterations, evaluations, x, T, coefficients, cost at the start, final cost) or the script exits non-zero.
 Prints one JSON line per workload: median wall seconds of each arm, rounds and launches per round, and per round the device time of the
 evaluation kernels, of the back-end kernels and the remainder (host work, copies and gaps); with the GPU's name, power limit and max SM

@@ -3,7 +3,8 @@
   loop     plan.generate_traj per problem, one context (lock-step A* per problem, one back end at a time)
   pool     the plan_batch chain (device A* for all searches, extraction, mid end) with the back end on a pool of 3 contexts on the
            GPU: three host threads, each optimising one problem at a time with svsdf_optimize (the pool of svsdf_optimize_batch)
-  batch    plan.plan_batch: the same front and mid end, then ONE lock-step back end (svsdf_optimize_lockstep)
+  batch    plan.plan_batch: the same front and mid end, then ONE lock-step back end (svsdf_optimize_lockstep, its L-BFGS machines
+           advanced round by round on the host; svsdf_optimize_device from plan.DEVICE_BACK_END_MIN_PROBLEMS problems)
 
 Scenes: the reference's star scene (tests/golden/map_star_pcd.npz) and a 60 x 60 map at resolution 1.0 (seeded obstacles, density
 0.01, one z layer); seeded start / goal pairs on free cells.  Every problem's result must be identical in the three ways (path, N,
