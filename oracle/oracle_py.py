@@ -6,95 +6,85 @@ The product package (implicit_svsdf_planner_b200/) must never import this module
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SO = os.path.join(_HERE, "_build", "libsvsdf_oracle.so")
-_SO_FMA = os.path.join(_HERE, "_build", "libsvsdf_oracle_fma.so")
-_SO_GLIBC = os.path.join(_HERE, "_build", "libsvsdf_oracle_glibc.so")
-_VARIANTS = {"default": _SO, "fma": _SO_FMA, "glibc": _SO_GLIBC}
-_libs = {}
+from . import native
+
+_VARIANTS = {"default": "_build/libsvsdf_oracle.so", "fma": "_build/libsvsdf_oracle_fma.so", "glibc": "_build/libsvsdf_oracle_glibc.so"}
 
 dp = C.POINTER(C.c_double)
 
 
-def build(force: bool = False) -> str:
-    srcs = [os.path.join(_HERE, f) for f in ("oracle_capi.cpp", "svsdf_oracle.hpp", "minco_oracle.hpp", "shapes.hpp", "portable_sincos.hpp")]
-    stale = any((not os.path.exists(so)) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs)
-                for so in _VARIANTS.values())
-    if force or stale:
-        subprocess.check_call(["make", "-C", _HERE, "-s"])
-    return _SO
+def build() -> str:
+    native.make("oracle")
+    return native.path(_VARIANTS["default"])
 
 
 def lib(variant: str = "default"):
     """variant "default": portable (fdlibm) sin/cos, no FMA contraction — bit-compatible with the strict CUDA build;
     "glibc": std::sin/std::cos, no contraction (the reference's x86-64 behaviour; timed as the CPU baseline);
     "fma": glibc sin/cos with -ffp-contract=fast -mfma (what the same source does on FMA targets)."""
-    if variant not in _libs:
-        build()
-        L = C.CDLL(_VARIANTS[variant])
-        L.orc_sincos.argtypes = [C.c_int64, dp, dp, dp]
-        L.orc_atan2.argtypes = [C.c_int64, dp, dp, dp]
-        L.orc_create.restype = C.c_void_p
-        L.orc_create.argtypes = [C.c_char_p, dp, dp, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int]
-        L.orc_destroy.argtypes = [C.c_void_p]
-        L.orc_set_threads.argtypes = [C.c_void_p, C.c_int]
-        L.orc_set_points.argtypes = [C.c_void_p, dp, C.c_int64, C.c_int]
-        L.orc_set_traj.argtypes = [C.c_void_p, C.c_int, dp, dp]
-        L.orc_traj_duration.restype = C.c_double
-        L.orc_traj_duration.argtypes = [C.c_void_p]
-        L.orc_traj_pos.argtypes = [C.c_void_p, C.c_double, dp]
-        L.orc_traj_vel.argtypes = [C.c_void_p, C.c_double, dp]
-        L.orc_sdf_at.restype = C.c_double
-        L.orc_sdf_at.argtypes = [C.c_void_p, dp, C.c_double]
-        L.orc_choice_t_init.restype = C.c_double
-        L.orc_choice_t_init.argtypes = [C.c_void_p, dp, C.c_double]
-        L.orc_gradient_descent.argtypes = [C.c_void_p, dp, C.c_double, C.c_double, C.c_double, dp, dp]
-        L.orc_count_evals.argtypes = [C.c_void_p, C.c_int]
-        L.orc_eval_count.restype = C.c_uint64
-        L.orc_eval_count.argtypes = [C.c_void_p]
-        L.orc_query_outer.argtypes = [C.c_void_p, C.c_int64, dp, dp, dp, dp]
-        L.orc_query.argtypes = [C.c_void_p, C.c_int64, dp, dp, dp, dp, C.POINTER(C.c_int)]
-        L.orc_cost_grad.restype = C.c_int64
-        L.orc_cost_grad.argtypes = [C.c_void_p, C.c_int, dp, dp, dp, dp, dp, dp]
-        L.orc_time_cost_grad.restype = C.c_double
-        L.orc_time_cost_grad.argtypes = [C.c_void_p, C.c_int, dp, dp, C.c_int, C.c_int, dp]
-        L.orc_shape_sdf.argtypes = [C.c_char_p, dp, dp, C.c_int, C.c_int64, dp, dp]
-        L.orc_shape_grad1.argtypes = [C.c_char_p, dp, dp, C.c_int, C.c_int64, dp, dp]
-        L.orc_minco_forward.argtypes = [dp, dp, C.c_int, dp, dp, dp, dp, dp, dp]
-        L.orc_minco_propagate.argtypes = [dp, dp, C.c_int, dp, dp, dp, dp, dp, dp]
-        L.orc_forward_T.argtypes = [C.c_int, dp, dp]
-        L.orc_backward_T.argtypes = [C.c_int, dp, dp]
-        L.orc_set_conditions.argtypes = [C.c_void_p, dp, dp, C.c_int]
-        L.orc_evaluate.restype = C.c_double
-        L.orc_evaluate.argtypes = [C.c_void_p, dp, dp, C.c_int]
-        L.orc_last_costs.argtypes = [C.c_void_p, dp]
-        L.orc_get_coeffs.argtypes = [C.c_void_p, dp, dp]
-        L.orc_lbfgs.restype = C.c_int
-        L.orc_lbfgs.argtypes = [C.c_void_p, dp, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double, C.c_int, C.c_double, dp]
-        L.orc_mesh_eval.argtypes = [dp, dp, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int64, dp, dp]
-        L.orc_create_mesh.restype = C.c_void_p
-        L.orc_create_mesh.argtypes = [dp, dp, C.c_int, C.c_void_p, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int]
-        u8 = C.POINTER(C.c_uint8)
-        L.orc_shape_kernels.argtypes = [C.c_char_p, dp, C.c_int, C.c_int, C.c_double, C.c_double, dp, u8, u8]
-        L.orc_cspace.argtypes = [C.c_char_p, dp, C.c_int, C.c_int, C.c_double, C.c_double, u8, C.c_int, C.c_int, C.c_int, u8]
-        L.orc_check_kernel_value.argtypes = [C.c_char_p, dp, C.c_int, C.c_int, C.c_double, C.c_double, u8, C.c_int, C.c_int, C.c_int64, dp,
-                                             C.POINTER(C.c_int), u8, dp]
-        L.orc_expand_nodes.argtypes = [C.c_char_p, dp, C.c_int, C.c_int, C.c_double, C.c_double, u8, C.c_int, C.c_int, C.c_double, C.c_double,
-                                       C.c_double, C.c_int64, C.POINTER(C.c_int), dp, u8, dp, u8]
-        L.orc_astar.argtypes = [C.c_char_p, dp, C.c_int, C.c_int, C.c_double, u8, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int, dp,
-                                dp, C.c_int, dp, C.POINTER(C.c_int), C.POINTER(C.c_int)]
-        L.orc_points_in_aabb.restype = C.c_int64
-        L.orc_points_in_aabb.argtypes = [u8, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double,
-                                         C.c_double, dp, C.c_int64]
-        L.orc_max_threads.restype = C.c_int
-        L.orc_num_procs.restype = C.c_int
-        _libs[variant] = L
-    return _libs[variant]
+    return native.load(_VARIANTS[variant], _declare, build)
+
+
+def _declare(L):
+    L.orc_sincos.argtypes = [C.c_int64, dp, dp, dp]
+    L.orc_atan2.argtypes = [C.c_int64, dp, dp, dp]
+    L.orc_create.restype = C.c_void_p
+    L.orc_create.argtypes = [C.c_char_p, dp, dp, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int]
+    L.orc_destroy.argtypes = [C.c_void_p]
+    L.orc_set_threads.argtypes = [C.c_void_p, C.c_int]
+    L.orc_set_points.argtypes = [C.c_void_p, dp, C.c_int64, C.c_int]
+    L.orc_set_traj.argtypes = [C.c_void_p, C.c_int, dp, dp]
+    L.orc_traj_duration.restype = C.c_double
+    L.orc_traj_duration.argtypes = [C.c_void_p]
+    L.orc_traj_pos.argtypes = [C.c_void_p, C.c_double, dp]
+    L.orc_traj_vel.argtypes = [C.c_void_p, C.c_double, dp]
+    L.orc_sdf_at.restype = C.c_double
+    L.orc_sdf_at.argtypes = [C.c_void_p, dp, C.c_double]
+    L.orc_choice_t_init.restype = C.c_double
+    L.orc_choice_t_init.argtypes = [C.c_void_p, dp, C.c_double]
+    L.orc_gradient_descent.argtypes = [C.c_void_p, dp, C.c_double, C.c_double, C.c_double, dp, dp]
+    L.orc_count_evals.argtypes = [C.c_void_p, C.c_int]
+    L.orc_eval_count.restype = C.c_uint64
+    L.orc_eval_count.argtypes = [C.c_void_p]
+    L.orc_query_outer.argtypes = [C.c_void_p, C.c_int64, dp, dp, dp, dp]
+    L.orc_query.argtypes = [C.c_void_p, C.c_int64, dp, dp, dp, dp, C.POINTER(C.c_int)]
+    L.orc_cost_grad.restype = C.c_int64
+    L.orc_cost_grad.argtypes = [C.c_void_p, C.c_int, dp, dp, dp, dp, dp, dp]
+    L.orc_time_cost_grad.restype = C.c_double
+    L.orc_time_cost_grad.argtypes = [C.c_void_p, C.c_int, dp, dp, C.c_int, C.c_int, dp]
+    L.orc_shape_sdf.argtypes = [C.c_char_p, dp, dp, C.c_int, C.c_int64, dp, dp]
+    L.orc_shape_grad1.argtypes = [C.c_char_p, dp, dp, C.c_int, C.c_int64, dp, dp]
+    L.orc_minco_forward.argtypes = [dp, dp, C.c_int, dp, dp, dp, dp, dp, dp]
+    L.orc_minco_propagate.argtypes = [dp, dp, C.c_int, dp, dp, dp, dp, dp, dp]
+    L.orc_forward_T.argtypes = [C.c_int, dp, dp]
+    L.orc_backward_T.argtypes = [C.c_int, dp, dp]
+    L.orc_set_conditions.argtypes = [C.c_void_p, dp, dp, C.c_int]
+    L.orc_evaluate.restype = C.c_double
+    L.orc_evaluate.argtypes = [C.c_void_p, dp, dp, C.c_int]
+    L.orc_last_costs.argtypes = [C.c_void_p, dp]
+    L.orc_get_coeffs.argtypes = [C.c_void_p, dp, dp]
+    L.orc_lbfgs.restype = C.c_int
+    L.orc_lbfgs.argtypes = [C.c_void_p, dp, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double, C.c_int, C.c_double, dp]
+    L.orc_mesh_eval.argtypes = [dp, dp, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int64, dp, dp]
+    L.orc_create_mesh.restype = C.c_void_p
+    L.orc_create_mesh.argtypes = [dp, dp, C.c_int, C.c_void_p, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int]
+    u8 = C.POINTER(C.c_uint8)
+    L.orc_shape_kernels.argtypes = [C.c_char_p, dp, C.c_int, C.c_int, C.c_double, C.c_double, dp, u8, u8]
+    L.orc_cspace.argtypes = [C.c_char_p, dp, C.c_int, C.c_int, C.c_double, C.c_double, u8, C.c_int, C.c_int, C.c_int, u8]
+    L.orc_check_kernel_value.argtypes = [C.c_char_p, dp, C.c_int, C.c_int, C.c_double, C.c_double, u8, C.c_int, C.c_int, C.c_int64, dp,
+                                         C.POINTER(C.c_int), u8, dp]
+    L.orc_expand_nodes.argtypes = [C.c_char_p, dp, C.c_int, C.c_int, C.c_double, C.c_double, u8, C.c_int, C.c_int, C.c_double, C.c_double,
+                                   C.c_double, C.c_int64, C.POINTER(C.c_int), dp, u8, dp, u8]
+    L.orc_astar.argtypes = [C.c_char_p, dp, C.c_int, C.c_int, C.c_double, u8, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int, dp,
+                            dp, C.c_int, dp, C.POINTER(C.c_int), C.POINTER(C.c_int)]
+    L.orc_points_in_aabb.restype = C.c_int64
+    L.orc_points_in_aabb.argtypes = [u8, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double,
+                                     C.c_double, dp, C.c_int64]
+    L.orc_max_threads.restype = C.c_int
+    L.orc_num_procs.restype = C.c_int
 
 
 def _p(a):

@@ -1,5 +1,5 @@
 // oracle/oracle_scale_capi.cpp — TEST INFRASTRUCTURE ONLY: C entry points (for ctypes, oracle/scale_py.py) over the
-// oracle's deformable-robot path (svsdf_oracle_scale.hpp).  Built by oracle/scale.mk into _build/libsvsdf_oracle_scale.so
+// oracle's deformable-robot path (svsdf_oracle_scale.hpp).  Built by oracle/Makefile into _build/libsvsdf_oracle_scale.so
 // (portable sin/cos: the strict CUDA build's bits) and _build/libsvsdf_oracle_scale_glibc.so (glibc sin/cos).
 #include <omp.h>
 

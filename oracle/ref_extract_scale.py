@@ -1,4 +1,4 @@
-"""Generate the reference's own source for the deformable-robot pin build (oracle/scale.mk), under oracle/_ref/scaled/ (git-ignored).
+"""Generate the reference's own source for the deformable-robot pin build (`make -C oracle ref`), under oracle/_ref/scaled/ (git-ignored).
 
 TEST INFRASTRUCTURE.  Runs oracle/ref_extract.py unchanged into oracle/_ref/scaled/_ref/gen/ and then edits only the copy:
   * sw_methods.inc loses the verbatim getScale / getDotScale (sw_manager.hpp:495-518, the hook a user edits for a deforming

@@ -7,45 +7,40 @@ tests/golden/ref_pin_front.npz elsewhere (tests/golden/make_front_golden.py writ
 from __future__ import annotations
 
 import ctypes as C
-import os
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
+from . import native
+
 VARIANTS = ("glibc", "portable")
-_libs = {}
 dp = C.POINTER(C.c_double)
 u8p = C.POINTER(C.c_uint8)
 i32p = C.POINTER(C.c_int32)
 
 
-def so_path(variant: str) -> str:
-    return os.path.join(_HERE, "_ref", f"libref_front_{variant}.so")
-
-
 def available(variant: str = "portable") -> bool:
-    return os.path.exists(so_path(variant))
+    return native.available(f"_ref/libref_front_{variant}.so")
 
 
 def lib(variant: str = "portable"):
-    if variant not in _libs:
-        L = C.CDLL(so_path(variant))
-        L.rf_variant.restype = C.c_char_p
-        L.rf_create.restype = C.c_void_p
-        L.rf_create.argtypes = [C.c_char_p, dp, C.c_int, C.c_int, C.c_double, C.c_double, u8p, C.c_int, C.c_int, C.c_double, C.c_double]
-        L.rf_destroy.argtypes = [C.c_void_p]
-        L.rf_map_kernel.restype = C.c_int
-        L.rf_map_kernel.argtypes = [C.c_void_p, u8p]
-        L.rf_kernels.argtypes = [C.c_void_p, dp, u8p, u8p]
-        L.rf_kernel_conv.argtypes = [C.c_void_p, C.c_int, C.c_int64, i32p, u8p]
-        L.rf_check_kernel_value.argtypes = [C.c_void_p, C.c_int64, dp, i32p, u8p, dp]
-        L.rf_points_in_aabb.restype = C.c_int64
-        L.rf_points_in_aabb.argtypes = [C.c_void_p, C.c_double, C.c_double, C.c_double, C.c_double, dp, C.c_int64]
-        L.rf_expand.argtypes = [C.c_void_p, C.c_int64, i32p, dp, u8p, dp, u8p]
-        L.rf_astar.argtypes = [C.c_void_p, C.c_int, dp, dp, C.c_int, dp, i32p, i32p, u8p]
-        assert L.rf_variant().decode() == variant
-        _libs[variant] = L
-    return _libs[variant]
+    return native.load(f"_ref/libref_front_{variant}.so", lambda L: _declare(L, variant))
+
+
+def _declare(L, variant):
+    L.rf_variant.restype = C.c_char_p
+    L.rf_create.restype = C.c_void_p
+    L.rf_create.argtypes = [C.c_char_p, dp, C.c_int, C.c_int, C.c_double, C.c_double, u8p, C.c_int, C.c_int, C.c_double, C.c_double]
+    L.rf_destroy.argtypes = [C.c_void_p]
+    L.rf_map_kernel.restype = C.c_int
+    L.rf_map_kernel.argtypes = [C.c_void_p, u8p]
+    L.rf_kernels.argtypes = [C.c_void_p, dp, u8p, u8p]
+    L.rf_kernel_conv.argtypes = [C.c_void_p, C.c_int, C.c_int64, i32p, u8p]
+    L.rf_check_kernel_value.argtypes = [C.c_void_p, C.c_int64, dp, i32p, u8p, dp]
+    L.rf_points_in_aabb.restype = C.c_int64
+    L.rf_points_in_aabb.argtypes = [C.c_void_p, C.c_double, C.c_double, C.c_double, C.c_double, dp, C.c_int64]
+    L.rf_expand.argtypes = [C.c_void_p, C.c_int64, i32p, dp, u8p, dp, u8p]
+    L.rf_astar.argtypes = [C.c_void_p, C.c_int, dp, dp, C.c_int, dp, i32p, i32p, u8p]
+    assert L.rf_variant().decode() == variant
 
 
 def _p(a, t):

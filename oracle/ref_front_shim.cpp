@@ -1,6 +1,6 @@
 // oracle/ref_front_shim.cpp — TEST INFRASTRUCTURE: the REFERENCE'S OWN SOURCE of the A* front end, compiled where it lies.
 //
-// Builds oracle/_ref/libref_front_<variant>.so (git-ignored; `make -C oracle -f front.mk`, only where the reference tree exists):
+// Builds oracle/_ref/libref_front_<variant>.so (git-ignored; `make -C oracle ref`, only where the reference tree exists):
 //   * the shape classes and BasicShape::initShape: oracle/ref_shape_scaffold.inc over the fragments of oracle/ref_extract.py,
 //     exactly as in libref_path_*;
 //   * the node test and the search: oracle/_ref/front/gen/*.inc, cut VERBATIM by oracle/ref_extract_front.py —
@@ -17,7 +17,7 @@
 //   * generateMapKernel2D's buffer is copied into one with a zero byte of slack: kernelConv<true> reads one byte past the last row
 //     (sw_manager.hpp:1087); that byte only feeds bits the byte kernel masks out.
 //
-// Variants (front.mk): glibc (the reference as it runs on x86-64) and portable (-DREF_LIBM_PORTABLE: every sin/cos/atan2 in the
+// Variants (oracle/Makefile): glibc (the reference as it runs on x86-64) and portable (-DREF_LIBM_PORTABLE: every sin/cos/atan2 in the
 // reference text — AngleAxisd's in checkSubSWCollision and initShape, the shapes' constants — is the pinned fdlibm algorithm the
 // CUDA kernels implement, as in libref_path_portable).
 #include <algorithm>

@@ -1,6 +1,6 @@
 // oracle/ref_mid_shim.cpp — TEST INFRASTRUCTURE: the REFERENCE'S OWN SOURCE of the mid end, compiled where it lies.
 //
-// Builds oracle/_ref/libref_mid.so (git-ignored; `make -C oracle ref_mid`, only where /root/reference exists):
+// Builds oracle/_ref/libref_mid.so (git-ignored; `make -C oracle ref_path`, only where /root/reference exists):
 //   * `utils/minco.hpp`, `utils/trajectory.hpp`, `utils/flatness.hpp` and `utils/lbfgs.hpp` (the reference's patched L-BFGS) are
 //     #included WHOLE from /root/reference/src/utils/include;
 //   * OriTraj's member functions (planner_algorithm/mid_end.hpp: the tau / xi maps, smoothedL1, grad_cost_dir, addPosePenalty,

@@ -2,7 +2,7 @@
 // (sw_manager.hpp:17) and getScale = this project's schedule.  oracle/ref_extract_scale.py prepares oracle/_ref/scaled/ (a copy of
 // ref_path_shim.cpp next to the edited fragments); this file compiles that copy and adds the schedule's C entry points.
 // The scaled getStateOnTrajStamp(t, xt, Rt, St) asserts `time_stamp > traj_duration`, an inverted condition: inert only because
-// the build defines NDEBUG (oracle/scale.mk).
+// the build defines NDEBUG (oracle/Makefile).
 #include "_ref/scaled/ref_path_shim.cpp"
 
 extern "C" {

@@ -7,31 +7,26 @@ tests/golden/ref_pin_pose.npz elsewhere (tests/golden/make_pose_golden.py writes
 from __future__ import annotations
 
 import ctypes as C
-import os
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_libs = {}
+from . import native
+
 dp = C.POINTER(C.c_double)
 
 
-def so_path(variant: str) -> str:
-    return os.path.join(_HERE, "_ref", f"libref_pose_{variant}.so")
-
-
 def available(variant: str = "portable") -> bool:
-    return os.path.exists(so_path(variant))
+    return native.available(f"_ref/libref_pose_{variant}.so")
 
 
 def lib(variant: str = "portable"):
-    if variant not in _libs:
-        L = C.CDLL(so_path(variant))
-        L.rp_variant.restype = C.c_char_p
-        L.rp_grad_cost_p.argtypes = [C.c_char_p, dp, dp, C.c_int, C.POINTER(C.c_uint8), C.c_int, C.c_int, C.c_int, dp, C.c_double, dp,
-                                     C.c_double, C.c_int64, dp, dp]
-        _libs[variant] = L
-    return _libs[variant]
+    return native.load(f"_ref/libref_pose_{variant}.so", _declare)
+
+
+def _declare(L):
+    L.rp_variant.restype = C.c_char_p
+    L.rp_grad_cost_p.argtypes = [C.c_char_p, dp, dp, C.c_int, C.POINTER(C.c_uint8), C.c_int, C.c_int, C.c_int, dp, C.c_double, dp,
+                                 C.c_double, C.c_int64, dp, dp]
 
 
 def grad_cost_p(shape, poly_params, occ, lo, res, half, safety_hor, poses, polygon=None, variant="portable"):

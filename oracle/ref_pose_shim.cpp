@@ -1,7 +1,7 @@
 // oracle/ref_pose_shim.cpp — TEST INFRASTRUCTURE: the REFERENCE'S OWN SOURCE of the pose-sampled obstacle penalty, compiled where it
 // lies.
 //
-// Builds oracle/_ref/libref_pose_<variant>.so (git-ignored; `make -C oracle -f pose.mk`, only where the reference tree exists):
+// Builds oracle/_ref/libref_pose_<variant>.so (git-ignored; `make -C oracle ref`, only where the reference tree exists):
 //   * the shape classes: oracle/ref_shape_scaffold.inc over the fragments of oracle/ref_extract.py, as in libref_path_*;
 //   * GridMap3D's members and PCSmapManager::projInMap: the fragments of oracle/ref_extract_front.py, as in libref_front_*;
 //   * TrajOptimizer::smoothedL1 / grad_cost_p, SweptVolumeManager::posEva2Rel / getSDFWithGradWhenRobotAtState and
@@ -13,7 +13,7 @@
 //   * bdx, bdy, bdz = 2 half (grad_cost_p reads bdx / 2: exact).
 //   * `rotate` (back_end_optimizer.hpp:439) is declared uninitialised in addTimeIntPenalty; grad_cost_p sets five entries.  The caller
 //     here passes it zero-initialised, as the product takes it.
-// Variants (pose.mk): glibc (the reference as it runs on x86-64) and portable (-DREF_LIBM_PORTABLE: the pinned fdlibm sin / cos the
+// Variants (oracle/Makefile): glibc (the reference as it runs on x86-64) and portable (-DREF_LIBM_PORTABLE: the pinned fdlibm sin / cos the
 // CUDA kernels implement).
 #include <algorithm>
 #include <cmath>

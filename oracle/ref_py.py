@@ -8,72 +8,70 @@ same code and compare bit for bit; `tests/golden/make_ref_pin_golden.py` uses it
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
+from . import native
+
 VARIANTS = ("glibc", "portable", "glibc_r1", "glibc_r2")
-_libs = {}
 dp = C.POINTER(C.c_double)
 u8p = C.POINTER(C.c_uint8)
 
 
-def so_path(variant: str) -> str:
-    return os.path.join(_HERE, "_ref", f"libref_path_{variant}.so")
+def _so(variant: str) -> str:
+    return f"_ref/libref_path_{variant}.so"
 
 
 def available(variant: str = "glibc") -> bool:
-    return os.path.exists(so_path(variant))
+    return native.available(_so(variant))
 
 
 def build() -> None:
-    """make -C oracle ref_path (needs /root/reference)."""
-    subprocess.check_call(["make", "-C", _HERE, "-s", "ref_path"], stdout=subprocess.DEVNULL)
+    """The rigid path's pins and the mid end's (needs the reference tree)."""
+    native.make("ref_path")
 
 
 def lib(variant: str = "glibc"):
-    if variant not in _libs:
-        L = C.CDLL(so_path(variant))
-        L.ref_variant.restype = C.c_char_p
-        L.ref_redux_order.restype = C.c_int
-        L.ref_shape_sdf.argtypes = [C.c_char_p, dp, dp, C.c_int, C.c_int64, dp, dp]
-        L.ref_shape_grad1.argtypes = [C.c_char_p, dp, dp, C.c_int, C.c_int64, dp, dp]
-        L.ref_shape_kernels.argtypes = [C.c_char_p, dp, C.c_int, C.c_int, C.c_double, C.c_double, dp, u8p, u8p]
-        L.ref_smoothed_l1.argtypes = [C.c_int64, dp, C.c_double, dp, dp, u8p]
-        L.ref_create.restype = C.c_void_p
-        L.ref_create.argtypes = [C.c_char_p, dp, dp, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int]
-        L.ref_destroy.argtypes = [C.c_void_p]
-        L.ref_set_threads.argtypes = [C.c_void_p, C.c_int]
-        L.ref_set_points.argtypes = [C.c_void_p, dp, C.c_int64, C.c_int]
-        L.ref_set_traj.argtypes = [C.c_void_p, C.c_int, dp, dp]
-        L.ref_traj_duration.restype = C.c_double
-        L.ref_traj_duration.argtypes = [C.c_void_p]
-        L.ref_traj_pos.argtypes = [C.c_void_p, C.c_double, dp]
-        L.ref_traj_vel.argtypes = [C.c_void_p, C.c_double, dp]
-        L.ref_locate_piece.restype = C.c_int
-        L.ref_locate_piece.argtypes = [C.c_void_p, C.c_double, dp]
-        L.ref_sdf_at.restype = C.c_double
-        L.ref_sdf_at.argtypes = [C.c_void_p, dp, C.c_double]
-        L.ref_sdf_dot_at.restype = C.c_double
-        L.ref_sdf_dot_at.argtypes = [C.c_void_p, dp, C.c_double]
-        L.ref_choice_t_init.restype = C.c_double
-        L.ref_choice_t_init.argtypes = [C.c_void_p, dp, C.c_double]
-        L.ref_gradient_descent.argtypes = [C.c_void_p, dp, C.c_double, C.c_double, C.c_double, dp, dp]
-        L.ref_query_outer.argtypes = [C.c_void_p, C.c_int64, dp, dp, dp, dp]
-        L.ref_query.argtypes = [C.c_void_p, C.c_int64, dp, dp, dp, dp]
-        L.ref_cost_grad.argtypes = [C.c_void_p, C.c_int, dp, dp, dp, dp, dp]
-        L.ref_set_conditions.argtypes = [C.c_void_p, dp, dp, C.c_int]
-        L.ref_evaluate.restype = C.c_double
-        L.ref_evaluate.argtypes = [C.c_void_p, dp, dp, C.c_int]
-        L.ref_last_costs.argtypes = [C.c_void_p, dp]
-        L.ref_minco_forward.argtypes = [C.c_void_p, dp, dp, dp, dp, dp, dp]
-        L.ref_minco_propagate.argtypes = [C.c_void_p, dp, dp, dp, dp]
-        L.ref_forward_T.argtypes = [C.c_int, dp, dp]
-        L.ref_backward_T.argtypes = [C.c_int, dp, dp]
-        _libs[variant] = L
-    return _libs[variant]
+    return native.load(_so(variant), _declare)
+
+
+def _declare(L):
+    L.ref_variant.restype = C.c_char_p
+    L.ref_redux_order.restype = C.c_int
+    L.ref_shape_sdf.argtypes = [C.c_char_p, dp, dp, C.c_int, C.c_int64, dp, dp]
+    L.ref_shape_grad1.argtypes = [C.c_char_p, dp, dp, C.c_int, C.c_int64, dp, dp]
+    L.ref_shape_kernels.argtypes = [C.c_char_p, dp, C.c_int, C.c_int, C.c_double, C.c_double, dp, u8p, u8p]
+    L.ref_smoothed_l1.argtypes = [C.c_int64, dp, C.c_double, dp, dp, u8p]
+    L.ref_create.restype = C.c_void_p
+    L.ref_create.argtypes = [C.c_char_p, dp, dp, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int]
+    L.ref_destroy.argtypes = [C.c_void_p]
+    L.ref_set_threads.argtypes = [C.c_void_p, C.c_int]
+    L.ref_set_points.argtypes = [C.c_void_p, dp, C.c_int64, C.c_int]
+    L.ref_set_traj.argtypes = [C.c_void_p, C.c_int, dp, dp]
+    L.ref_traj_duration.restype = C.c_double
+    L.ref_traj_duration.argtypes = [C.c_void_p]
+    L.ref_traj_pos.argtypes = [C.c_void_p, C.c_double, dp]
+    L.ref_traj_vel.argtypes = [C.c_void_p, C.c_double, dp]
+    L.ref_locate_piece.restype = C.c_int
+    L.ref_locate_piece.argtypes = [C.c_void_p, C.c_double, dp]
+    L.ref_sdf_at.restype = C.c_double
+    L.ref_sdf_at.argtypes = [C.c_void_p, dp, C.c_double]
+    L.ref_sdf_dot_at.restype = C.c_double
+    L.ref_sdf_dot_at.argtypes = [C.c_void_p, dp, C.c_double]
+    L.ref_choice_t_init.restype = C.c_double
+    L.ref_choice_t_init.argtypes = [C.c_void_p, dp, C.c_double]
+    L.ref_gradient_descent.argtypes = [C.c_void_p, dp, C.c_double, C.c_double, C.c_double, dp, dp]
+    L.ref_query_outer.argtypes = [C.c_void_p, C.c_int64, dp, dp, dp, dp]
+    L.ref_query.argtypes = [C.c_void_p, C.c_int64, dp, dp, dp, dp]
+    L.ref_cost_grad.argtypes = [C.c_void_p, C.c_int, dp, dp, dp, dp, dp]
+    L.ref_set_conditions.argtypes = [C.c_void_p, dp, dp, C.c_int]
+    L.ref_evaluate.restype = C.c_double
+    L.ref_evaluate.argtypes = [C.c_void_p, dp, dp, C.c_int]
+    L.ref_last_costs.argtypes = [C.c_void_p, dp]
+    L.ref_minco_forward.argtypes = [C.c_void_p, dp, dp, dp, dp, dp, dp]
+    L.ref_minco_propagate.argtypes = [C.c_void_p, dp, dp, dp, dp]
+    L.ref_forward_T.argtypes = [C.c_int, dp, dp]
+    L.ref_backward_T.argtypes = [C.c_int, dp, dp]
 
 
 def _p(a):
@@ -267,18 +265,12 @@ class RefPath:
 
 
 # ---- mid end: the reference's OriTraj (oracle/ref_mid_shim.cpp -> oracle/_ref/libref_mid.so) ----
-_MID = None
-
-
 def mid_available() -> bool:
-    return os.path.exists(os.path.join(_HERE, "_ref", "libref_mid.so"))
+    return native.available("_ref/libref_mid.so")
 
 
 def _mid_lib():
-    global _MID
-    if _MID is None:
-        _MID = C.CDLL(os.path.join(_HERE, "_ref", "libref_mid.so"))
-    return _MID
+    return native.load("_ref/libref_mid.so", lambda L: None)
 
 
 def mid_cost(cfg, N, init_cm, final_cm, Q_cm, rot_cm, x):

@@ -9,18 +9,12 @@ Schedules are 8 values: a_x, a_y, b_x, b_y, w_x, w_y, phi_x, phi_y.
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-from . import ref_py
+from . import native, ref_py
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SO = {"default": os.path.join(_HERE, "_build", "libsvsdf_oracle_scale.so"),
-       "glibc": os.path.join(_HERE, "_build", "libsvsdf_oracle_scale_glibc.so")}
-_SRCS = ("oracle_scale_capi.cpp", "svsdf_oracle_scale.hpp", "svsdf_oracle.hpp", "minco_oracle.hpp", "shapes.hpp", "portable_sincos.hpp")
-_libs = {}
+_VARIANTS = {"default": "_build/libsvsdf_oracle_scale.so", "glibc": "_build/libsvsdf_oracle_scale_glibc.so"}
 dp = C.POINTER(C.c_double)
 
 
@@ -32,46 +26,42 @@ def _p(a):
     return a.ctypes.data_as(dp) if a is not None else None
 
 
-def build(force: bool = False) -> None:
-    srcs = [os.path.join(_HERE, f) for f in _SRCS]
-    stale = any((not os.path.exists(so)) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs) for so in _SO.values())
-    if force or stale:
-        subprocess.check_call(["make", "-C", _HERE, "-f", "scale.mk", "-s"])
+def build() -> None:
+    native.make("scale")
 
 
 def build_ref() -> None:
-    """make -C oracle -f scale.mk ref (needs the reference tree)."""
-    subprocess.check_call(["make", "-C", _HERE, "-f", "scale.mk", "-s", "ref"], stdout=subprocess.DEVNULL)
+    """The reference's own code with useScale on (needs the reference tree)."""
+    native.make("ref_scaled")
 
 
 def lib(variant: str = "default"):
-    if variant not in _libs:
-        build()
-        L = C.CDLL(_SO[variant])
-        vp = C.c_void_p
-        L.sorc_create.restype = vp
-        L.sorc_create.argtypes = [C.c_char_p, dp, dp, C.c_int, C.c_double, C.c_double, C.c_int]
-        L.sorc_create_mesh.restype = vp
-        L.sorc_create_mesh.argtypes = [dp, dp, C.c_int, vp, C.c_int, C.c_double, C.c_double, C.c_int]
-        L.sorc_destroy.argtypes = [vp]
-        L.sorc_set_threads.argtypes = [vp, C.c_int]
-        L.sorc_set_scale.argtypes = [vp, dp]
-        L.sorc_scale_at.argtypes = [dp, C.c_double, dp, dp]
-        L.sorc_set_points.argtypes = [vp, dp, C.c_int64, C.c_int]
-        L.sorc_set_traj.argtypes = [vp, C.c_int, dp, dp]
-        L.sorc_duration.restype = C.c_double
-        L.sorc_duration.argtypes = [vp]
-        L.sorc_traj_pos.argtypes = [vp, C.c_double, dp]
-        L.sorc_traj_vel.argtypes = [vp, C.c_double, dp]
-        L.sorc_sdf_at.restype = C.c_double
-        L.sorc_sdf_at.argtypes = [vp, dp, C.c_double, C.c_int]
-        L.sorc_gradient_descent.argtypes = [vp, dp, C.c_double, C.c_double, C.c_double, dp, dp]
-        L.sorc_query_outer.argtypes = [vp, C.c_int64, dp, dp, dp, dp]
-        L.sorc_query.argtypes = [vp, C.c_int64, dp, dp, dp, dp, C.POINTER(C.c_int)]
-        L.sorc_cost_grad.restype = C.c_int64
-        L.sorc_cost_grad.argtypes = [vp, C.c_int, dp, dp, dp, dp, dp, dp]
-        _libs[variant] = L
-    return _libs[variant]
+    return native.load(_VARIANTS[variant], _declare, build)
+
+
+def _declare(L):
+    vp = C.c_void_p
+    L.sorc_create.restype = vp
+    L.sorc_create.argtypes = [C.c_char_p, dp, dp, C.c_int, C.c_double, C.c_double, C.c_int]
+    L.sorc_create_mesh.restype = vp
+    L.sorc_create_mesh.argtypes = [dp, dp, C.c_int, vp, C.c_int, C.c_double, C.c_double, C.c_int]
+    L.sorc_destroy.argtypes = [vp]
+    L.sorc_set_threads.argtypes = [vp, C.c_int]
+    L.sorc_set_scale.argtypes = [vp, dp]
+    L.sorc_scale_at.argtypes = [dp, C.c_double, dp, dp]
+    L.sorc_set_points.argtypes = [vp, dp, C.c_int64, C.c_int]
+    L.sorc_set_traj.argtypes = [vp, C.c_int, dp, dp]
+    L.sorc_duration.restype = C.c_double
+    L.sorc_duration.argtypes = [vp]
+    L.sorc_traj_pos.argtypes = [vp, C.c_double, dp]
+    L.sorc_traj_vel.argtypes = [vp, C.c_double, dp]
+    L.sorc_sdf_at.restype = C.c_double
+    L.sorc_sdf_at.argtypes = [vp, dp, C.c_double, C.c_int]
+    L.sorc_gradient_descent.argtypes = [vp, dp, C.c_double, C.c_double, C.c_double, dp, dp]
+    L.sorc_query_outer.argtypes = [vp, C.c_int64, dp, dp, dp, dp]
+    L.sorc_query.argtypes = [vp, C.c_int64, dp, dp, dp, dp, C.POINTER(C.c_int)]
+    L.sorc_cost_grad.restype = C.c_int64
+    L.sorc_cost_grad.argtypes = [vp, C.c_int, dp, dp, dp, dp, dp, dp]
 
 
 def scale_at(sched, t, variant="default"):

@@ -13,7 +13,7 @@
 //   * the interior branch (:916-1018) runs the scaled outer solve; its velocity fallback and ring do not change;
 //   * the chain rule (back_end_optimizer.hpp:827, 1050) uses St = getScale(t*): sdf_grad = -L' (-(St^-1)^T rotate g); the
 //     yaw term (:1062) has no St^-1 (exact only at St = I) and gdT no dS/dt term.
-// tests/test_oracle_scale.py pins it bit for bit on the reference's own code built that way (oracle/scale.mk).
+// tests/test_oracle_scale.py pins it bit for bit on the reference's own code built that way (`make -C oracle ref`).
 #pragma once
 #include "minco_oracle.hpp"
 #include "svsdf_oracle.hpp"

@@ -6,36 +6,29 @@ returns a SimpleNamespace with vertices (V x 2), segments (S x 2), triangles (F 
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 import types
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SO = os.path.join(_HERE, "_build", "libsvsdf_oracle_swept.so")
-_SRCS = ("swept_capi.cpp", "swept_oracle.hpp", "swept.mk")
-_lib = None
+from . import native
+
+_SO = "_build/libsvsdf_oracle_swept.so"
 
 
-def build(force: bool = False) -> None:
-    srcs = [os.path.join(_HERE, f) for f in _SRCS]
-    if force or not os.path.exists(_SO) or any(os.path.getmtime(s) > os.path.getmtime(_SO) for s in srcs):
-        subprocess.check_call(["make", "-C", _HERE, "-f", "swept.mk", "-s"])
+def build() -> None:
+    native.make("swept")
 
 
 def lib():
-    global _lib
-    if _lib is None:
-        build()
-        L = C.CDLL(_SO)
-        L.sw_contour.restype = C.c_void_p
-        L.sw_contour.argtypes = [C.POINTER(C.c_double), C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_double, C.c_double,
-                                 C.POINTER(C.c_int64)]
-        L.sw_copy.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.sw_free.argtypes = [C.c_void_p]
-        _lib = L
-    return _lib
+    return native.load(_SO, _declare, build)
+
+
+def _declare(L):
+    L.sw_contour.restype = C.c_void_p
+    L.sw_contour.argtypes = [C.POINTER(C.c_double), C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_double, C.c_double,
+                             C.POINTER(C.c_int64)]
+    L.sw_copy.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.sw_free.argtypes = [C.c_void_p]
 
 
 def swept_contour(field, i0, j0, h, iso):

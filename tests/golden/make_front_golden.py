@@ -1,5 +1,5 @@
 """Writes tests/golden/ref_pin_front.npz: the reference's own A* front end (oracle/_ref/libref_front_portable.so, built by
-oracle/front.mk where the reference tree exists) on the case matrix of tests/front_cases.py.  Large outputs (kernels, the
+`make -C oracle ref` where the reference tree exists) on the case matrix of tests/front_cases.py.  Large outputs (kernels, the
 configuration-space map, the AABB point lists, the packed map) are SHA-256 digests; node-test outputs and paths are stored
 whole.  Running it again writes the same bytes.  Also checks that the glibc variant gives the same booleans, yaws and paths.
 

@@ -1,7 +1,7 @@
 """Golden vectors for the mesh functor's winding number, from the REFERENCE's own code.
 
 Runs in the build container only (needs /root/reference):  python tests/golden/make_fwn_golden.py
-  1. `make -C oracle ref` compiles the reference's fast-winding-number implementation (the HDK UT_SolidAngle<float,float>
+  1. `make -C oracle ref` compiles, among the other reference pins, the reference's fast-winding-number implementation (the HDK UT_SolidAngle<float,float>
      behind igl::fast_winding_number; src/utils/include/igl/FastWindingNumberForSoups.h) from the source where it lies
      into oracle/_ref/libref_fwn.so (git-ignored), behind the shim oracle/ref_fwn_shim.cpp.
   2. The reference's shipped meshes src/plan_manager/shapes/{star,sdHorseshoe}.obj are read, the BVH is built exactly as

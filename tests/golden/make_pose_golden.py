@@ -1,5 +1,5 @@
 """Write tests/golden/ref_pin_pose.npz: the REFERENCE'S OWN grad_cost_p (oracle/_ref/libref_pose_portable.so, built by
-`make -C oracle -f pose.mk` where the reference tree exists) at a set of sample poses, for the machines without the reference.
+`make -C oracle ref` where the reference tree exists) at a set of sample poses, for the machines without the reference.
 
 Cases: two maps (the reference's star map, map_star_pcd.npz at its resolution and threshold, half 8.5 = kernel_size 17 x 1.0 / 2 on
 every axis; and a seeded five-layer map with half (3, 2, 0.5)) x every analytic shape and the Polygon x poly_params (0, 0, 0) and
@@ -64,7 +64,7 @@ def poses(occ, lo, res, half, name, shape, rng):
 
 
 def main():
-    assert ref_pose_py.available("portable"), "build oracle/_ref/libref_pose_portable.so first (make -C oracle -f pose.mk)"
+    assert ref_pose_py.available("portable"), "build oracle/_ref/libref_pose_portable.so first (make -C oracle ref)"
     rng = np.random.default_rng(7)
     out = {}
     case = []

@@ -2,7 +2,7 @@
 on the edge scenes of the outer solve and of the interior branch under schedules at the limits of what svsdf_set_scale
 accepts.
 
-    make -C oracle -f scale.mk ref && python tests/golden/make_scale_edges_golden.py [out.npz]     (needs the reference tree)
+    make -C oracle ref && python tests/golden/make_scale_edges_golden.py [out.npz]     (needs the reference tree)
 
 The trajectories are the rigid edge scenes (tests/golden/make_outer_edges_golden.py, make_gsip_edges_golden.py), imported,
 not copied.  Schedules (a_x, a_y, b_x, b_y, w_x, w_y, phi_x, phi_y):

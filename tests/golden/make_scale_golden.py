@@ -1,6 +1,6 @@
 """Generate tests/golden/ref_pin_scale.npz: outputs of THE REFERENCE'S OWN CODE for a deformable robot.
 
-    make -C oracle -f scale.mk ref && python tests/golden/make_scale_golden.py [out.npz]     (only where the reference tree exists)
+    make -C oracle ref && python tests/golden/make_scale_golden.py [out.npz]     (only where the reference tree exists)
 
 oracle/_ref/libref_path_scaled_{glibc,portable}.so are the reference's source (oracle/ref_extract_scale.py,
 oracle/ref_path_scaled_shim.cpp): its `useScale` switch turned on and this project's schedule supplying getScale(t) =

@@ -2,7 +2,7 @@
 
 The reference side is kernelConv / visit_kernels_by_distance / checkKernelValue / checkSubSWCollision (sw_manager.hpp),
 getPointsInAABB2D / projInMap (PCSmap_manager.h), the GridMap3D index and centre helpers, and AstarGetSucc /
-AstarPathSearch / getPath (front_end_Astar.hpp), cut verbatim and compiled by oracle/front.mk (portable sin/cos).  It runs
+AstarPathSearch / getPath (front_end_Astar.hpp), cut verbatim and compiled by `make -C oracle ref` (portable sin/cos).  It runs
 live where oracle/_ref/libref_front_portable.so exists, and is read from tests/golden/ref_pin_front.npz otherwise.  The case
 matrix is tests/front_cases.py: every shape with and without a pre-transform, resolutions 0.1 to 2.5, half boxes from under one
 cell to 160 cells, edge and corner nodes, the edges of the father-yaw index, and a search scene per shape.

@@ -5,8 +5,8 @@ signature (lmbm.h:206-209), so its address is handed to lmbm_optimize as is — 
     python tests/tools/run_lmbm_gpu.py [--points 400 --pieces 8 --clearance 2.6 --seed-map 777 --max-evals 400] [--trace out.npz]
                                        [--lib PATH]
 
-By default it needs oracle/_ref/lmbm.so (copied there by __graft_entry__.build() where the reference checkout is present;
-git-ignored) and a libgfortran.so.5 (scipy bundles one; symlinked into oracle/_ref/), and re-executes itself with
+By default it needs oracle/_ref/lmbm.so (copied there by `make -C oracle ref`, which __graft_entry__.build() runs where the reference
+checkout is present; git-ignored) and a libgfortran.so.5 (scipy bundles one; symlinked into oracle/_ref/), and re-executes itself with
 LD_LIBRARY_PATH set.  --lib runs any other library exporting lmbm::lmbm_optimize instead (tests/cpp/lmbm_standin.cpp).  --trace records every (x, f) through a thin Python wrapper instead (slower; used by the tests).
 Prints one JSON line."""
 import argparse
