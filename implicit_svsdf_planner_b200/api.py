@@ -241,7 +241,7 @@ EXPORTED_SYMBOLS = [
     "svsdf_front_init", "svsdf_front_get_kernels", "svsdf_front_cspace", "svsdf_front_check_kernel_value", "svsdf_front_expand", "svsdf_front_astar",
     "svsdf_front_astar_device", "svsdf_set_scale", "svsdf_scale_matrix",
     "svsdf_cost_grad_multi", "svsdf_optimize_lockstep", "svsdf_lockstep_rounds", "svsdf_optimize_device", "svsdf_round_times", "svsdf_swept_contour", "svsdf_swept_free",
-    "svsdf_map_clearance", "svsdf_clearance_free", "svsdf_map_clearance_multi",
+    "svsdf_map_clearance", "svsdf_clearance_free", "svsdf_map_clearance_multi", "svsdf_swept_contour_multi",
     "svsdf_default_dynamics", "svsdf_set_dynamics", "svsdf_dynamics_penalty",
     "svsdf_default_pose_penalty", "svsdf_set_pose_penalty", "svsdf_pose_penalty_eval",
 ]
@@ -343,8 +343,32 @@ def lib():
     L.svsdf_clearance_free.restype = None
     L.svsdf_map_clearance_multi.argtypes = [vp, C.c_int, C.POINTER(ClearanceProblem), C.c_double, C.POINTER(ClearanceOut),
                                             C.POINTER(C.c_int)]
+    L.svsdf_swept_contour_multi.argtypes = [vp, C.c_int, C.POINTER(ClearanceProblem), C.POINTER(SweptParams), C.POINTER(SweptMesh),
+                                            C.POINTER(C.c_int)]
     _lib = L
     return L
+
+
+def _swept_params(h, iso, box, want_field, max_corners) -> SweptParams:
+    prm = SweptParams()
+    prm.h, prm.iso, prm.max_corners, prm.want_field = float(h), float(iso), int(max_corners), int(bool(want_field))
+    if box is not None:
+        prm.has_box = 1
+        prm.box = (C.c_double * 4)(*[float(v) for v in box])
+    return prm
+
+
+def _take_swept(m: SweptMesh, h, iso) -> SweptContour:
+    """A SweptContour copied out of the library's svsdf_swept_mesh, which is then released."""
+    try:
+        V, S, F = m.n_vertices, m.n_segments, m.n_triangles
+        verts = np.ctypeslib.as_array(m.vertices, shape=(V, 2)).copy() if V else np.empty((0, 2))
+        segs = np.ctypeslib.as_array(m.segments, shape=(S, 2)).copy() if S else np.empty((0, 2), dtype=np.int32)
+        tris = np.ctypeslib.as_array(m.triangles, shape=(F, 3)).copy() if F else np.empty((0, 3), dtype=np.int32)
+        field = np.ctypeslib.as_array(m.field, shape=(m.ny, m.nx)).copy() if m.field else None
+        return SweptContour(m.i0, m.j0, m.nx, m.ny, h, iso, verts, segs, tris, m.clipped, m.n_evaluated, field)
+    finally:
+        lib().svsdf_swept_free(C.byref(m))
 
 
 def _f64(a):
@@ -827,23 +851,30 @@ class Context:
         never clipped)."""
         T = _f64(T)
         c = _f64(coeffs_colmajor).reshape(-1)
-        prm = SweptParams()
-        prm.h, prm.iso, prm.max_corners, prm.want_field = float(h), float(iso), int(max_corners), int(bool(want_field))
-        if box is not None:
-            prm.has_box = 1
-            prm.box = (C.c_double * 4)(*[float(v) for v in box])
+        prm = _swept_params(h, iso, box, want_field, max_corners)
         m = SweptMesh()
-        L = lib()
-        self._ck(L.svsdf_swept_contour(self.h, T.shape[0], _p(T), _p(c), C.byref(prm), C.byref(m)), "svsdf_swept_contour")
-        try:
-            V, S, F = m.n_vertices, m.n_segments, m.n_triangles
-            verts = np.ctypeslib.as_array(m.vertices, shape=(V, 2)).copy() if V else np.empty((0, 2))
-            segs = np.ctypeslib.as_array(m.segments, shape=(S, 2)).copy() if S else np.empty((0, 2), dtype=np.int32)
-            tris = np.ctypeslib.as_array(m.triangles, shape=(F, 3)).copy() if F else np.empty((0, 3), dtype=np.int32)
-            field = np.ctypeslib.as_array(m.field, shape=(m.ny, m.nx)).copy() if m.field else None
-            return SweptContour(m.i0, m.j0, m.nx, m.ny, h, iso, verts, segs, tris, m.clipped, m.n_evaluated, field)
-        finally:
-            L.svsdf_swept_free(C.byref(m))
+        self._ck(lib().svsdf_swept_contour(self.h, T.shape[0], _p(T), _p(c), C.byref(prm), C.byref(m)), "svsdf_swept_contour")
+        return _take_swept(m, h, iso)
+
+    def swept_contour_multi(self, trajs, h, iso=0.0, box=None, want_field=False, max_corners=0) -> list:
+        """svsdf_swept_contour_multi: swept_contour of every trajectory in trajs (a list of (T, coeffs_colmajor)) with the same h, iso,
+        box (None: each its own automatic box), want_field and max_corners, in one set of launches, each the bits of its own
+        swept_contour call.  Returns one entry per trajectory: a SweptContour, or an SvsdfError for a trajectory whose single call would
+        have failed with a non-finite value.  An invalid parameter or trajectory raises for the whole call."""
+        n = len(trajs)
+        arr = (ClearanceProblem * max(n, 1))()
+        keep = []
+        for k, (T, co) in enumerate(trajs):
+            T, co = _f64(T).reshape(-1), _f64(co).reshape(-1)
+            arr[k].N, arr[k].T, arr[k].coeffs = T.shape[0], _p(T), _p(co)
+            keep += [T, co]
+        prm = _swept_params(h, iso, box, want_field, max_corners)
+        outs = (SweptMesh * max(n, 1))()
+        status = np.zeros(max(n, 1), dtype=np.int32)
+        self._ck(lib().svsdf_swept_contour_multi(self.h, n, arr, C.byref(prm), outs, status.ctypes.data_as(C.POINTER(C.c_int))),
+                 "svsdf_swept_contour_multi")
+        return [_take_swept(outs[k], h, iso) if status[k] == 0 else
+                SvsdfError(f"svsdf_swept_contour_multi: problem {k}: status {int(status[k])}") for k in range(n)]
 
     def map_clearance(self, T, coeffs_colmajor, d_max=math.inf) -> Clearance:
         """svsdf_map_clearance: the swept-volume SDF (svsdf_query's value, interior depth included) of this trajectory at the centre of

@@ -62,8 +62,9 @@ cudaError_t launch_extract_count(const ExtractArgs &E, int *block_counts, int n_
                                  cudaStream_t stream);
 cudaError_t launch_extract_write(const ExtractArgs &E, const int *block_offsets, int n_blocks, double *out_xy,
                                  int64_t cap, cudaStream_t stream);
-// svsdf_swept_contour (svsdf_swept.cu).  what: 0 classify + count per tile, 1 compact, 2 scatter the values (+ non-finite flag),
-// 3 marching-squares counts, 4 emit vertices, 5 emit segments and triangles; scan: exclusive prefix of `channels` rows of n counts
+// svsdf_swept_contour[_multi] (svsdf_swept.cu), over every problem of A.prob.  what: 0 classify + count per tile, 1 compact, 2 scatter
+// the values, 3 marching-squares counts (+ per-problem totals, non-finite and clipped flags), 4 emit vertices, 5 emit segments and
+// triangles; scan: exclusive prefix of `channels` rows of n counts
 // (row stride n + 1, the total lands at [n] and at totals[ch]) in one CTA.
 cudaError_t launch_swept(int what, const SweptArgs &A, cudaStream_t st);
 cudaError_t launch_swept_scan(int *counts, int n, int channels, int *totals, cudaStream_t st);

@@ -406,11 +406,14 @@ struct MultiItem {
     int rc = SVSDF_OK;
 };
 
-// svsdf_map_clearance_multi's evaluation: the items' points already on the device (concatenated in item order; MultiItem::pts and
-// ::out are not used) and svsdf_query's per-point values at the same places, instead of the cost and gradient.
+// svsdf_map_clearance_multi's and svsdf_swept_contour_multi's evaluation: the items' points already on the device (concatenated in
+// item order; MultiItem::pts and ::out are not used) and svsdf_query's per-point values at the same places, instead of the cost and
+// gradient (tstar may be null).  outer_only: svsdf_query(outer_only = 1)'s values, the outer solve alone (no k_compact_multi, no
+// k_gsip_multi).
 struct PointQuery {
     const double *pts;
     double *sdf, *tstar;
+    bool outer_only = false;
 };
 
 // The planning and launch sequence of one multi evaluation, shared by run_multi and svsdf_optimize_device.  The caller fills each
@@ -431,7 +434,7 @@ struct MultiPlan {
 int plan_multi(svsdf_ctx *ctx, MultiPlan &pl);
 void pack_plan(const MultiPlan &pl, unsigned char *h);
 // The launches of a planned evaluation whose packed head is at d (device) and blobs at d_blobs: k_pose_table_multi, k_outer_multi per
-// schedule that occurs, k_compact_multi, k_gsip_multi and (not with pq) k_finalize_multi.  *records: the per-problem records [cost,
+// schedule that occurs, k_compact_multi and k_gsip_multi (not with pq->outer_only) and k_finalize_multi (not with pq).  *records: the per-problem records [cost,
 // gradC (18N), gradT (N), n_inside] at out_off (device).
 int launch_plan(svsdf_ctx *ctx, const MultiPlan &pl, const unsigned char *d, double *d_blobs, const double *d_points, const PointQuery *pq,
                 double **records);

@@ -75,7 +75,8 @@ int launch_plan(svsdf_ctx *ctx, const MultiPlan &pl, const unsigned char *d, dou
     A.partials = reinterpret_cast<double *>(sc + s_part);
     A.want_reduce = pq ? 0 : 1;
     if (pq) { A.out_sdf = pq->sdf; A.out_tstar = pq->tstar; }
-    A.want_gsip = 1;
+    const bool outer_only = pq && pq->outer_only;
+    A.want_gsip = outer_only ? 0 : 1;
     A.inside_flag = sc + s_flag;
     A.inside_tstar = reinterpret_cast<double *>(sc + s_ts);
     A.inside_list = reinterpret_cast<int *>(sc + s_list);
@@ -106,6 +107,10 @@ int launch_plan(svsdf_ctx *ctx, const MultiPlan &pl, const unsigned char *d, dou
         ++launches;
     }
     M.cta_map = nullptr;
+    if (outer_only) {  // the per-point values are written; nothing else runs
+        ctx->launches += launches;
+        return SVSDF_OK;
+    }
     CK(K.compact_multi(A.inside_flag, A.inside_list, M, ctx->stream));
     const GsipPlan gp = gsip_plan(ctx, pq ? -1 : ctx->multi_last_inside);  // the variant svsdf_query would pick
     CK(K.multi(2, A, M, ctx->shape, Z, gp.grid, (size_t)pl.max_blob * sizeof(double), gp.wide, ctx->sm_count, ctx->stream));

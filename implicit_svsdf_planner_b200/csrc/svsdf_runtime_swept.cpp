@@ -65,128 +65,189 @@ int64_t lattice_ceil(double x, double h) {
     while ((double)(i - 1) * h >= x) --i;
     return i;
 }
-}  // namespace
 
-int svsdf_swept_contour(svsdf_ctx *ctx, int N, const double *T, const double *coeffs, const svsdf_swept_params *prm,
-                        svsdf_swept_mesh *out) {
-    if (!ctx || !prm || !out) return SVSDF_ERR_INVALID;
-    std::memset(out, 0, sizeof(*out));
-    auto invalid = [&](const char *msg) {
+// svsdf_swept_contour (multi = false, n = 1, status_out unused: the status is returned) and svsdf_swept_contour_multi: every check
+// before any launch, then the mesher's kernels over the concatenation of the n problems (svsdf_swept.cu) in one set of launches.  The
+// outer solve of the needed corners is the single call's own (run_kernels, outer only) or, for n problems, the multi-problem one
+// (run_multi, outer only), which gives every point the same bits.
+int swept_run(svsdf_ctx *ctx, bool multi, int n, const svsdf_clearance_problem *problems, const svsdf_swept_params *prm,
+              svsdf_swept_mesh *out, int *status_out) {
+    const std::string who = multi ? "svsdf_swept_contour_multi" : "svsdf_swept_contour";
+    auto invalid = [&](const std::string &msg) {
         ctx->err = msg;
         return SVSDF_ERR_INVALID;
     };
     const double h = prm->h, iso = prm->iso;
-    if (!(std::isfinite(h) && h > 0.0)) return invalid("svsdf_swept_contour: h must be finite and > 0");
-    if (!std::isfinite(iso)) return invalid("svsdf_swept_contour: iso must be finite");
+    if (!(std::isfinite(h) && h > 0.0)) return invalid(who + ": h must be finite and > 0");
+    if (!std::isfinite(iso)) return invalid(who + ": iso must be finite");
     const int64_t cap = prm->max_corners == 0 ? kSweptDefaultCorners : prm->max_corners;
-    if (cap < 4 || cap > kSweptMaxCorners) return invalid("svsdf_swept_contour: max_corners must be 0 or in 4 .. 2^28");
-    BlobLayout L;
-    double D = 0.0;
-    const char *msg = nullptr;
-    if (traj_layout(N, T, coeffs, L, D, &msg) != SVSDF_OK) return invalid(msg);
-    for (int64_t e = 0; e < 18 * (int64_t)N; ++e)
-        if (!std::isfinite(coeffs[e])) return invalid("svsdf_swept_contour: non-finite trajectory coefficient");
+    if (cap < 4 || cap > kSweptMaxCorners) return invalid(who + ": max_corners must be 0 or in 4 .. 2^28");
+    if (prm->has_box) {
+        const double *b = prm->box;
+        if (!(std::isfinite(b[0]) && std::isfinite(b[1]) && std::isfinite(b[2]) && std::isfinite(b[3]))) return invalid(who + ": non-finite box");
+        if (b[0] > b[2] || b[1] > b[3]) return invalid(who + ": inverted box");
+    }
     // rho: body-frame radius beyond which the shape functor is provably > iso (sdf >= (|q| - R) / prune_scale for |q| >= prune_rmin)
     const ShapeParams &S = ctx->shape;
     const bool bounded = S.rout < 1e299;
+    if (!prm->has_box && !bounded) return invalid(who + ": the shape has no far-field bound; give a box");
     const double rho = bounded ? std::max(std::max(S.prune_rmin, S.rout + S.prune_scale * iso), 0.0) : INFINITY;
-    std::vector<double> samp;
-    swept_samples(ctx, N, T, coeffs, D, rho, samp);
-    const int n_samp = (int)(samp.size() / 3);
-    if (n_samp > kSweptMaxSamples) return invalid("svsdf_swept_contour: too many path samples");
-    double bx0, by0, bx1, by1;
-    if (prm->has_box) {
-        bx0 = prm->box[0]; by0 = prm->box[1]; bx1 = prm->box[2]; by1 = prm->box[3];
-        if (!(std::isfinite(bx0) && std::isfinite(by0) && std::isfinite(bx1) && std::isfinite(by1)))
-            return invalid("svsdf_swept_contour: non-finite box");
-        if (bx0 > bx1 || by0 > by1) return invalid("svsdf_swept_contour: inverted box");
-    } else {
-        if (!bounded) return invalid("svsdf_swept_contour: the shape has no far-field bound; give a box");
-        bx0 = by0 = INFINITY;
-        bx1 = by1 = -INFINITY;
-        for (int k = 0; k < n_samp; ++k) {
-            const double x = samp[3 * k], y = samp[3 * k + 1], r = samp[3 * k + 2];
-            bx0 = std::min(bx0, x - r); bx1 = std::max(bx1, x + r);
-            by0 = std::min(by0, y - r); by1 = std::max(by1, y + r);
+    // per problem: its samples and grid; tiles and whole marching-squares blocks in problem order
+    std::vector<SweptProblem> tab(n);
+    std::vector<double> samp_all, samp;
+    int64_t corners = 0, tiles = 0, blocks = 0;
+    for (int k = 0; k < n; ++k) {
+        const svsdf_clearance_problem &q = problems[k];
+        const std::string at = multi ? who + ": problem " + std::to_string(k) + ": " : std::string();
+        auto bad = [&](const std::string &msg) { return invalid(at + (multi ? msg : who + ": " + msg)); };
+        BlobLayout L;
+        double D = 0.0;
+        const char *msg = nullptr;
+        if (traj_layout(q.N, q.T, q.coeffs, L, D, &msg) != SVSDF_OK) return invalid(at + msg);
+        for (int64_t e = 0; e < 18 * (int64_t)q.N; ++e)
+            if (!std::isfinite(q.coeffs[e])) return bad("non-finite trajectory coefficient");
+        swept_samples(ctx, q.N, q.T, q.coeffs, D, rho, samp);
+        const int n_samp = (int)(samp.size() / 3);
+        if (n_samp > kSweptMaxSamples) return bad("too many path samples");
+        double bx0, by0, bx1, by1;
+        if (prm->has_box) {
+            bx0 = prm->box[0]; by0 = prm->box[1]; bx1 = prm->box[2]; by1 = prm->box[3];
+        } else {
+            bx0 = by0 = INFINITY;
+            bx1 = by1 = -INFINITY;
+            for (int s = 0; s < n_samp; ++s) {
+                const double x = samp[3 * s], y = samp[3 * s + 1], r = samp[3 * s + 2];
+                bx0 = std::min(bx0, x - r); bx1 = std::max(bx1, x + r);
+                by0 = std::min(by0, y - r); by1 = std::max(by1, y + r);
+            }
+            // strictly beyond every reach, whatever the rounding of the subtractions above
+            const double pad = 1e-9 * (1.0 + std::max(std::max(std::fabs(bx0), std::fabs(bx1)), std::max(std::fabs(by0), std::fabs(by1))));
+            bx0 -= pad; by0 -= pad; bx1 += pad; by1 += pad;
         }
-        // strictly beyond every reach, whatever the rounding of the subtractions above
-        const double pad = 1e-9 * (1.0 + std::max(std::max(std::fabs(bx0), std::fabs(bx1)), std::max(std::fabs(by0), std::fabs(by1))));
-        bx0 -= pad; by0 -= pad; bx1 += pad; by1 += pad;
+        const double lim = 0x1p50;
+        if (!(std::fabs(bx0) / h < lim && std::fabs(bx1) / h < lim && std::fabs(by0) / h < lim && std::fabs(by1) / h < lim))
+            return bad("box too large for the lattice of h");
+        const int64_t i0 = lattice_floor(bx0, h), j0 = lattice_floor(by0, h);
+        const int64_t i1 = std::max(lattice_ceil(bx1, h), i0 + 1), j1 = std::max(lattice_ceil(by1, h), j0 + 1);
+        const int64_t nx64 = i1 - i0 + 1, ny64 = j1 - j0 + 1;
+        if (nx64 > cap || ny64 > cap || nx64 * ny64 > cap) return bad("box has more corners than max_corners");
+        SweptProblem &g = tab[k];
+        std::memset(&g, 0, sizeof(g));
+        g.i0 = i0; g.j0 = j0; g.nx = (int)nx64; g.ny = (int)ny64;
+        g.tiles_x = (g.nx + kSweptTile - 1) / kSweptTile;
+        g.nblk = (int)((nx64 * ny64 + kSweptBlock - 1) / kSweptBlock);
+        g.tile0 = tiles;
+        g.blk0 = blocks;
+        g.samp0 = (int)(samp_all.size() / 3);
+        g.n_samp = n_samp;
+        samp_all.insert(samp_all.end(), samp.begin(), samp.end());
+        tiles += (int64_t)g.tiles_x * ((g.ny + kSweptTile - 1) / kSweptTile);
+        blocks += g.nblk;
+        corners += nx64 * ny64;
     }
-    const double lim = 0x1p50;
-    if (!(std::fabs(bx0) / h < lim && std::fabs(bx1) / h < lim && std::fabs(by0) / h < lim && std::fabs(by1) / h < lim))
-        return invalid("svsdf_swept_contour: box too large for the lattice of h");
-    const int64_t i0 = lattice_floor(bx0, h), j0 = lattice_floor(by0, h);
-    const int64_t i1 = std::max(lattice_ceil(bx1, h), i0 + 1), j1 = std::max(lattice_ceil(by1, h), j0 + 1);
-    const int64_t nx64 = i1 - i0 + 1, ny64 = j1 - j0 + 1;
-    if (nx64 > cap || ny64 > cap || nx64 * ny64 > cap) return invalid("svsdf_swept_contour: box has more corners than max_corners");
-    const int nx = (int)nx64, ny = (int)ny64;
-    const int64_t n = nx64 * ny64;
+    // Band positions, the per-CTA prefixes (k_sw_scan) and the CTA indices are int32; tiles and blocks are no more than the corners.  A
+    // single call (at most 2^28 corners) is never refused here.
+    if (corners > 2147483647LL) return invalid(who + ": the problems' grids hold more than 2^31 - 1 corners");
+    if (n == 0) return SVSDF_OK;
     CK(cudaSetDevice(ctx->device));
 
     SweptArgs A;
     std::memset(&A, 0, sizeof(A));
-    A.i0 = i0; A.j0 = j0; A.nx = nx; A.ny = ny; A.h = h; A.iso = iso;
-    A.tiles_x = (nx + kSweptTile - 1) / kSweptTile;
-    A.tiles_y = (ny + kSweptTile - 1) / kSweptTile;
-    const int tiles = A.tiles_x * A.tiles_y;
-    const int nblk = (int)((n + kSweptBlock - 1) / kSweptBlock);
-    A.n_samp = n_samp;
-    // per corner: need (n bytes), field (n doubles), vertex ids (3 n ints)
-    const size_t off_field = align16((size_t)n), off_vid = off_field + align16((size_t)n * 8);
-    CK(ctx->swept.d_corner.reserve(off_vid + (size_t)n * 12));
+    A.n_prob = n;
+    A.h = h; A.iso = iso;
+    A.tiles = (int)tiles;
+    A.n_blocks = (int)blocks;
+    // per corner of the concatenation (whole blocks): need (1 byte), field (8), vertex ids (12)
+    const size_t C = (size_t)blocks * kSweptBlock;
+    const size_t off_field = align16(C), off_vid = off_field + align16(C * 8);
+    CK(ctx->swept.d_corner.reserve(off_vid + C * 12));
     A.need = ctx->swept.d_corner;
     A.field = reinterpret_cast<double *>(ctx->swept.d_corner + off_field);
     A.vid = reinterpret_cast<int *>(ctx->swept.d_corner + off_vid);
-    // small: header [0] non-finite, [1] clipped, [2..6] channel totals, [7] needed corners; samples; tile counts; per-CTA counts
-    const size_t off_samp = 64, off_tile = off_samp + align16(samp.size() * 8), off_blk = off_tile + align16((size_t)(tiles + 1) * 4);
-    CK(ctx->swept.d_small.reserve(off_blk + (size_t)5 * (nblk + 1) * 4));
+    // small: header ([2..6] channel totals, [7] needed corners) | per-problem status [n][8] | problem table | samples (these four go up
+    // in one copy) | tile counts | per-CTA counts
+    const size_t off_stat = 64, off_tab = align16(off_stat + (size_t)n * 32), off_samp = align16(off_tab + tab.size() * sizeof(SweptProblem)),
+                 up = off_samp + samp_all.size() * 8, off_tile = align16(up), off_blk = off_tile + align16((size_t)(tiles + 1) * 4);
+    CK(ctx->swept.d_small.reserve(off_blk + (size_t)5 * (blocks + 1) * 4));
     int *d_hdr = reinterpret_cast<int *>(ctx->swept.d_small.get());
-    A.status = d_hdr;
+    A.stat = reinterpret_cast<int *>(ctx->swept.d_small + off_stat);
+    A.prob = reinterpret_cast<const SweptProblem *>(ctx->swept.d_small + off_tab);
     A.samp = reinterpret_cast<double *>(ctx->swept.d_small + off_samp);
     A.tile_off = reinterpret_cast<int *>(ctx->swept.d_small + off_tile);
     A.blk = reinterpret_cast<int *>(ctx->swept.d_small + off_blk);
-    CK(ctx->h_stage.reserve(64 + samp.size() * 8));
-    std::memset(ctx->h_stage, 0, 64);
-    std::memcpy(ctx->h_stage + 64, samp.data(), samp.size() * 8);
-    CK(cudaMemcpyAsync(ctx->swept.d_small, ctx->h_stage, 64 + samp.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
+    CK(ctx->h_stage.reserve(up));
+    std::memset(ctx->h_stage, 0, off_tab);
+    std::memcpy(ctx->h_stage + off_tab, tab.data(), tab.size() * sizeof(SweptProblem));
+    if (!samp_all.empty()) std::memcpy(ctx->h_stage + off_samp, samp_all.data(), samp_all.size() * 8);
     cudaStream_t st = ctx->stream;
+    CK(cudaMemcpyAsync(ctx->swept.d_small, ctx->h_stage, up, cudaMemcpyHostToDevice, st));
     // classify the tiles and their corners, count and compact the needed corners
     CK(launch_swept(0, A, st));
-    CK(launch_swept_scan(A.tile_off, tiles, 1, d_hdr + 7, st));
-    int hdr[8];
-    CK(cudaMemcpyAsync(ctx->h_stage, d_hdr, sizeof(hdr), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    std::memcpy(hdr, ctx->h_stage, sizeof(hdr));
-    const int64_t P = hdr[7];
+    CK(launch_swept_scan(A.tile_off, A.tiles, 1, d_hdr + 7, st));
+    std::vector<int> stat(8 * (size_t)n + 16);  // header, then the problems' status
+    auto download_status = [&]() -> int {
+        CK(cudaMemcpyAsync(ctx->h_stage, d_hdr, off_stat + (size_t)n * 32, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        std::memcpy(stat.data(), ctx->h_stage, off_stat + (size_t)n * 32);
+        return SVSDF_OK;
+    };
+    int rc = download_status();
+    if (rc) return rc;
+    const int *pst = stat.data() + 16;  // problem k's status at pst[8 k]
     ctx->launches += 2;
-    CK(ctx->swept.d_point.reserve((size_t)std::max<int64_t>(P, 1) * 28 + 32));
+    const int64_t P = stat[7];
+    const size_t P1 = (size_t)std::max<int64_t>(P, 1);
+    CK(ctx->swept.d_point.reserve(P1 * 32 + 32));
     A.P = P;
     A.pts = reinterpret_cast<double *>(ctx->swept.d_point.get());
-    A.val = reinterpret_cast<double *>(ctx->swept.d_point + (size_t)std::max<int64_t>(P, 1) * 16);
-    A.idx = reinterpret_cast<int *>(ctx->swept.d_point + (size_t)std::max<int64_t>(P, 1) * 24);
+    A.val = reinterpret_cast<double *>(ctx->swept.d_point + P1 * 16);
+    A.idx = reinterpret_cast<int64_t *>(ctx->swept.d_point + P1 * 24);
     if (P > 0) {
-        // the outer solve of svsdf_query (outer_only = 1) on the mesher's own points: the same kernels, so the same bits per point
         CK(launch_swept(1, A, st));
-        int rc = upload_traj(ctx, N, T, coeffs, P);
-        if (rc) return rc;
-        rc = run_kernels(ctx, A.pts, P, false, false, const_cast<double *>(A.val), nullptr, nullptr, nullptr);
-        if (rc) return rc;
+        double *val = const_cast<double *>(A.val);
+        if (!multi) {
+            // the outer solve of svsdf_query (outer_only = 1) on the mesher's own points: the same kernels, so the same bits per point
+            rc = upload_traj(ctx, problems[0].N, problems[0].T, problems[0].coeffs, P);
+            if (rc) return rc;
+            rc = run_kernels(ctx, A.pts, P, false, false, val, nullptr, nullptr, nullptr);
+            if (rc) return rc;
+        } else {
+            // the problems with needed corners, in problem order: their points are the concatenation's, in the same order; each keeps
+            // the decomposition of its single call, and the outer solve's per-point values do not depend on it
+            std::vector<MultiItem> items;
+            for (int k = 0; k < n; ++k) {
+                if (pst[8 * k + 7] == 0) continue;
+                MultiItem it;
+                it.N = problems[k].N; it.T = problems[k].T; it.coeffs = problems[k].coeffs; it.P = pst[8 * k + 7];
+                items.push_back(it);
+            }
+            PointQuery pq{A.pts, val, nullptr};
+            pq.outer_only = true;
+            rc = run_multi(ctx, items.data(), (int)items.size(), nullptr, &pq);
+            if (rc) return rc;
+            for (const MultiItem &it : items)
+                if (it.rc != SVSDF_OK) return invalid(who + ": a problem was refused by the evaluation");
+        }
         CK(launch_swept(2, A, st));
         ctx->launches += 2;
     }
     // marching squares: counts, their prefix, then vertices, segments and triangles
     CK(launch_swept(3, A, st));
-    CK(launch_swept_scan(A.blk, nblk, 5, d_hdr + 2, st));
-    CK(cudaMemcpyAsync(ctx->h_stage, d_hdr, sizeof(hdr), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    std::memcpy(hdr, ctx->h_stage, sizeof(hdr));
+    CK(launch_swept_scan(A.blk, A.n_blocks, 5, d_hdr + 2, st));
+    rc = download_status();
+    if (rc) return rc;
     ctx->launches += 2;
-    if (hdr[0]) {
+    if (!multi && pst[0]) {
         ctx->err = "svsdf_swept_contour: non-finite field value";
         return SVSDF_ERR_NONFINITE;
     }
-    const int64_t V = (int64_t)hdr[2] + hdr[3] + hdr[4], Sg = hdr[5], F = hdr[6];
+    // the outputs of every problem (the scan's int32 prefixes included) must stay in int32: one problem's always do (at most 2^28 corners)
+    int64_t tot[5] = {0, 0, 0, 0, 0};
+    for (int k = 0; k < n; ++k)
+        for (int ch = 0; ch < 5; ++ch) tot[ch] += pst[8 * k + 2 + ch];
+    for (int ch = 0; ch < 5; ++ch)
+        if (tot[ch] > 2147483647LL) return invalid(who + ": the problems' outlines have more than 2^31 - 1 vertices, segments or triangles");
+    const int64_t V = tot[0] + tot[1] + tot[2], Sg = tot[3], F = tot[4];
     const size_t b_verts = (size_t)V * 16, b_segs = (size_t)Sg * 8, b_tris = (size_t)F * 12;
     const size_t o_segs = align16(b_verts), o_tris = o_segs + align16(b_segs), o_end = o_tris + align16(b_tris);
     CK(ctx->swept.d_out.reserve(o_end + 16));
@@ -196,30 +257,73 @@ int svsdf_swept_contour(svsdf_ctx *ctx, int N, const double *T, const double *co
     CK(launch_swept(4, A, st));
     CK(launch_swept(5, A, st));
     ctx->launches += 2;
-    const size_t b_field = prm->want_field ? (size_t)n * 8 : 0;
+    const SweptProblem &last = tab[n - 1];
+    const size_t b_field = prm->want_field ? ((size_t)last.blk0 * kSweptBlock + (size_t)last.nx * last.ny) * 8 : 0;
     CK(ctx->h_stage.reserve(o_end + b_field + 16));
     unsigned char *hs = ctx->h_stage;
     if (o_end) CK(cudaMemcpyAsync(hs, ctx->swept.d_out, o_end, cudaMemcpyDeviceToHost, st));
     if (b_field) CK(cudaMemcpyAsync(hs + o_end, A.field, b_field, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
-    out->i0 = i0; out->j0 = j0; out->nx = nx; out->ny = ny;
-    out->n_vertices = V; out->n_segments = Sg; out->n_triangles = F;
-    out->clipped = hdr[1] ? 1 : 0;
-    out->n_evaluated = P;
-    out->vertices = static_cast<double *>(std::malloc(b_verts + 16));
-    out->segments = static_cast<int32_t *>(std::malloc(b_segs + 16));
-    out->triangles = static_cast<int32_t *>(std::malloc(b_tris + 16));
-    out->field = b_field ? static_cast<double *>(std::malloc(b_field)) : nullptr;
-    if (!out->vertices || !out->segments || !out->triangles || (b_field && !out->field)) {
-        svsdf_swept_free(out);
-        ctx->err = "svsdf_swept_contour: out of host memory";
+    // every problem's arrays, as the single call allocates them; a problem with a non-finite value gets none
+    int64_t v0 = 0, s0 = 0, f0 = 0;
+    for (int k = 0; k < n; ++k) {
+        const SweptProblem &g = tab[k];
+        const int *ps = pst + 8 * k;
+        const int64_t Vk = (int64_t)ps[2] + ps[3] + ps[4], Sk = ps[5], Fk = ps[6];
+        const int64_t vk = v0, sk = s0, fk = f0;
+        v0 += Vk; s0 += Sk; f0 += Fk;
+        if (ps[0]) {
+            status_out[k] = SVSDF_ERR_NONFINITE;
+            continue;
+        }
+        svsdf_swept_mesh *o = &out[k];
+        const size_t bf = prm->want_field ? (size_t)g.nx * g.ny * 8 : 0;
+        o->vertices = static_cast<double *>(std::malloc((size_t)Vk * 16 + 16));
+        o->segments = static_cast<int32_t *>(std::malloc((size_t)Sk * 8 + 16));
+        o->triangles = static_cast<int32_t *>(std::malloc((size_t)Fk * 12 + 16));
+        o->field = bf ? static_cast<double *>(std::malloc(bf)) : nullptr;
+        if (!o->vertices || !o->segments || !o->triangles || (bf && !o->field)) {
+            for (int j = 0; j <= k; ++j) {
+                svsdf_swept_free(&out[j]);
+                if (multi) status_out[j] = SVSDF_ERR_INVALID;
+            }
+            ctx->err = who + ": out of host memory";
+            return SVSDF_ERR_INVALID;
+        }
+        o->i0 = g.i0; o->j0 = g.j0; o->nx = g.nx; o->ny = g.ny;
+        o->n_vertices = Vk; o->n_segments = Sk; o->n_triangles = Fk;
+        o->clipped = ps[1] ? 1 : 0;
+        o->n_evaluated = ps[7];
+        std::memcpy(o->vertices, hs + (size_t)vk * 16, (size_t)Vk * 16);
+        std::memcpy(o->segments, hs + o_segs + (size_t)sk * 8, (size_t)Sk * 8);
+        std::memcpy(o->triangles, hs + o_tris + (size_t)fk * 12, (size_t)Fk * 12);
+        if (bf) std::memcpy(o->field, hs + o_end + (size_t)g.blk0 * kSweptBlock * 8, bf);
+        if (multi) status_out[k] = SVSDF_OK;
+    }
+    return SVSDF_OK;
+}
+}  // namespace
+
+int svsdf_swept_contour(svsdf_ctx *ctx, int N, const double *T, const double *coeffs, const svsdf_swept_params *prm,
+                        svsdf_swept_mesh *out) {
+    if (!ctx || !prm || !out) return SVSDF_ERR_INVALID;
+    std::memset(out, 0, sizeof(*out));
+    const svsdf_clearance_problem p{N, T, coeffs};
+    return swept_run(ctx, false, 1, &p, prm, out, nullptr);
+}
+
+int svsdf_swept_contour_multi(svsdf_ctx *ctx, int n, const svsdf_clearance_problem *problems, const svsdf_swept_params *params,
+                              svsdf_swept_mesh *out, int *status_out) {
+    if (!ctx) return SVSDF_ERR_INVALID;
+    if (n < 0 || n > kMaxMultiProblems || !params || (n > 0 && (!problems || !out || !status_out))) {
+        ctx->err = "svsdf_swept_contour_multi: needs 0 <= n <= 65535, the parameters and the problem, output and status arrays";
         return SVSDF_ERR_INVALID;
     }
-    std::memcpy(out->vertices, hs, b_verts);
-    std::memcpy(out->segments, hs + o_segs, b_segs);
-    std::memcpy(out->triangles, hs + o_tris, b_tris);
-    if (b_field) std::memcpy(out->field, hs + o_end, b_field);
-    return SVSDF_OK;
+    for (int k = 0; k < n; ++k) {
+        std::memset(&out[k], 0, sizeof(out[k]));
+        status_out[k] = SVSDF_ERR_INVALID;
+    }
+    return swept_run(ctx, true, n, problems, params, out, status_out);
 }
 
 void svsdf_swept_free(svsdf_swept_mesh *mesh) {

@@ -259,29 +259,37 @@ struct PoseArgs {
     double *rec;               // [..][4]
 };
 
-// svsdf_swept_contour (svsdf_swept.cu): the narrow-band marching-squares mesher
+// svsdf_swept_contour[_multi] (svsdf_swept.cu): the narrow-band marching-squares mesher of n problems (n = 1: the single call).
+// Problem k owns tiles tile0 .. (the classify / compact CTAs) and whole marching-squares blocks blk0 .. blk0 + nblk - 1; its corners
+// start at corner kSweptBlock * blk0 of the concatenation, so one k_sw_scan over the blocks gives every problem its own prefix.
 constexpr int kSweptTile = 16;           // classification / compaction tile: 16 x 16 corners, one CTA of 256 threads
 constexpr int kSweptMaxSamples = 2112;   // path samples: at most ceil(T_i / 0.15) per piece, D < 300 s, N <= 64
 constexpr int kSweptBlock = 1024;        // corners per CTA of the marching-squares passes (256 threads x 4)
-struct SweptArgs {
+struct SweptProblem {
     int64_t i0, j0;
     int nx, ny;
-    int tiles_x, tiles_y;
+    int tiles_x, nblk;         // tiles per row; marching-squares blocks (ceil(nx ny / kSweptBlock))
+    int64_t tile0, blk0;       // first tile, first block
+    int samp0, n_samp;         // its samples in SweptArgs::samp
+};
+struct SweptArgs {
+    int n_prob;
+    const SweptProblem *prob;  // [n_prob], tile0 and blk0 ascending
+    int *stat;                 // [n_prob][8]: [0] non-finite value seen, [1] clipped, [2..6] channel totals, [7] needed corners
     double h, iso;
-    int n_samp;
-    const double *samp;        // [n_samp][3]: sample x, y and its reach (a corner farther than reach from every sample is > iso)
-    unsigned char *need;       // [ny][nx] corner is evaluated
-    double *field;             // [ny][nx]
+    const double *samp;        // [..][3]: sample x, y and its reach (a corner farther than reach from every sample is > iso)
+    unsigned char *need;       // per corner of the concatenation: corner is evaluated
+    double *field;             // per corner
     int *tile_off;             // [tiles + 1] needed corners per tile, then their exclusive prefix (k_sw_scan)
-    double *pts;               // [P][2] needed corners (tile-major, row-major in a tile)
-    int *idx;                  // [P] their field index
+    double *pts;               // [P][2] needed corners (problem by problem, tile-major, row-major in a tile)
+    int64_t *idx;              // [P] their corner index in the concatenation
     const double *val;         // [P] their values (the evaluation's output)
     int64_t P;
     int *blk;                  // [5][n_blocks + 1] per-CTA counts of the marching-squares channels, then their prefix
-    int *status;               // [0] non-finite value seen, [1] clipped
-    int *vid;                  // [ny][nx][3] vertex of the horizontal edge, the vertical edge and the corner
-    double *verts;             // [V][2]
-    int *segs, *tris;          // [S][2], [F][3]
+    int *vid;                  // per corner [3]: vertex (local to its problem) of the horizontal edge, the vertical edge and the corner
+    double *verts;             // [V][2], problem by problem
+    int *segs, *tris;          // [S][2], [F][3], problem by problem; vertex ids local to the problem
+    int tiles, n_blocks;       // over all problems
 };
 
 // svsdf_map_clearance[_multi] (svsdf_clearance.cu): the occupied map columns near n trajectories.  Problem k covers the words of its

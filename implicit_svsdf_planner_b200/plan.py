@@ -77,12 +77,14 @@ def rot_z(yaw: float) -> np.ndarray:
 def generate_traj(ctx: "api.Context", cmap: CloudMap, start_xy, goal_xy, kernel_size: int = scenes.YAML["kernel_size"], kernel_yaw_num: int = 18,
                   front_end_safeh: float = 0.0, traj_parlength: float = 3.0, inittime: float = scenes.YAML["inittime"],
                   mid_cfg: Optional["api.MidConfig"] = None, lbfgs_params=None, max_path: int = 4096, certify: bool = False,
-                  repair: int = 0) -> dict:
+                  repair: int = 0, outline: Optional[dict] = None) -> dict:
     """generatePath + generateTraj for one start / goal on the map `cmap` (the context's shape is the robot).  certify=True adds
     `clearance` (see certificate) to a result that reached the back end.  repair=R > 0 (implies certify) then runs up to R repair rounds
     (see Repair): the top-level trajectory keys and `clearance` describe the final trajectory, `repair` what the rounds did, and
     the context's resident points are the last query set.  When the context has dynamics set (Context.set_dynamics), the back end
-    penalises them and a result that reached it gains `dynamics` (dynamics_report of the final trajectory)."""
+    penalises them and a result that reached it gains `dynamics` (dynamics_report of the final trajectory).  outline=dict(h=...,
+    iso=0.0) adds `outline` to a result that reached the back end: the swept region of the final trajectory (after repair) as
+    Context.swept_contour(T, coeffs, h, iso) returns it."""
     X, Y, Z = cmap.occ.shape
     res = cmap.res
     ctx.set_map3d(pack_map_kernel3d(cmap.occ, kernel_size), X, Y, Z, kernel_size, cmap.boundary_min, res)
@@ -122,7 +124,19 @@ def generate_traj(ctx: "api.Context", cmap: CloudMap, start_xy, goal_xy, kernel_
         out["clearance"] = certificate(ctx, T, b)
     if ctx.dynamics is not None:
         out["dynamics"] = dynamics_report(ctx.dynamics, T, b)
+    if outline is not None:
+        out["outline"] = ctx.swept_contour(T, np.asarray(b).reshape(-1), outline["h"], outline.get("iso", 0.0))
     return out
+
+
+def outline_all(ctx: "api.Context", results: list, outline: dict) -> list:
+    """swept_contour_multi of every result's trajectory with outline's h and iso (default 0), in one set of launches.  A problem whose
+    outline fails raises, as generate_traj's swept_contour does."""
+    outs = ctx.swept_contour_multi([(r["T"], np.asarray(r["coeffs"]).reshape(-1)) for r in results], outline["h"], outline.get("iso", 0.0))
+    for o in outs:
+        if isinstance(o, Exception):
+            raise o
+    return outs
 
 
 # samples per piece of dynamics_report's lattice
@@ -236,7 +250,7 @@ def plan_batch(ctx: "api.Context", cmap: CloudMap, starts, goals, kernel_size: i
                front_end_safeh: float = 0.0, traj_parlength: float = 3.0, inittime: float = scenes.YAML["inittime"],
                mid_cfg: Optional["api.MidConfig"] = None, lbfgs_params=None, max_path: int = 4096, max_in_flight: int = 0,
                workers: Optional[int] = None, stats: Optional[dict] = None, back_end: bool = True, certify: bool = False,
-               repair: int = 0) -> list:
+               repair: int = 0, outline: Optional[dict] = None) -> list:
     """generate_traj for n start / goal pairs on one map: one device A* launch for all searches (svsdf_front_astar_device), per problem the
     waypoints, the query points (extract_points3d, on the context) and the warm start (mid_get_ori_traj, on a thread pool: the mid end is
     host code and ctypes releases the GIL), then ONE lock-step back end for every problem whose mid end succeeded (svsdf_optimize_device
@@ -250,7 +264,9 @@ def plan_batch(ctx: "api.Context", cmap: CloudMap, starts, goals, kernel_size: i
     certify=True adds generate_traj's `clearance` to every problem that went through the back end (one svsdf_map_clearance_multi for
     all of them, after the back end; stats then also holds its wall seconds, certify_s).  repair=R > 0 (implies certify) adds
     generate_traj(repair=R)'s keys and bits: each round is one lock-step back end over the problems that gained cells and one
-    svsdf_map_clearance_multi over them (stats: repair_s, the rounds' wall seconds, and repair_rounds)."""
+    svsdf_map_clearance_multi over them (stats: repair_s, the rounds' wall seconds, and repair_rounds).  outline=dict(h=..., iso=0.0)
+    adds generate_traj(outline=...)'s `outline`, with its bits, to every problem that went through the back end: one
+    svsdf_swept_contour_multi for all of them, after repair (stats: outline_s, its wall seconds)."""
     st = np.asarray(starts, dtype=np.float64).reshape(-1, 2)
     go = np.asarray(goals, dtype=np.float64).reshape(-1, 2)
     n = st.shape[0]
@@ -360,6 +376,12 @@ def plan_batch(ctx: "api.Context", cmap: CloudMap, starts, goals, kernel_size: i
         for p in back:
             r = out[p["q"]]
             r["dynamics"] = dynamics_report(ctx.dynamics, r["T"], r["coeffs"])
+    if outline is not None:
+        t7 = time.perf_counter()
+        for p, o in zip(back, outline_all(ctx, [out[p["q"]] for p in back], outline)):
+            out[p["q"]]["outline"] = o
+        if stats is not None:
+            stats["outline_s"] = time.perf_counter() - t7
     return out
 
 

@@ -293,6 +293,19 @@ typedef struct {
 int svsdf_map_clearance_multi(svsdf_ctx *ctx, int n, const svsdf_clearance_problem *problems, double d_max, svsdf_clearance *out,
                               int *status_out);
 
+/* svsdf_swept_contour_multi: svsdf_swept_contour of n trajectories in one set of launches, with one set of parameters (h, iso,
+ * max_corners, want_field and the box: has_box = 1 gives every problem that box, has_box = 0 each its own automatic box).  out[k] is
+ * bit for bit svsdf_swept_contour(ctx, N_k, T_k, coeffs_k, params, ...) on the same context (grid, vertices, segments, triangles with
+ * problem-local vertex ids, clipped, n_evaluated, field); status_out[k] is the status that call returns, SVSDF_OK or
+ * SVSDF_ERR_NONFINITE (then out[k] holds nothing).  Release each out[k] with svsdf_swept_free.
+ *   0 <= n <= 65535; n = 0 does nothing.  Refused before any work (SVSDF_ERR_INVALID, nothing allocated) for any parameter or
+ *   trajectory the single call refuses, a shape without a far-field bound and no box, or when the problems' grids hold more than
+ *   2^31 - 1 corners together (never for n = 1).  The number of kernel launches does not depend on n or the grids (none of the
+ *   evaluation's when no problem needs a corner); the host synchronises three times.  The context's resident points, last_n_inside
+ *   and everything svsdf_cost_grad and svsdf_cost_grad_multi depend on keep their values. */
+int svsdf_swept_contour_multi(svsdf_ctx *ctx, int n, const svsdf_clearance_problem *problems, const svsdf_swept_params *params,
+                              svsdf_swept_mesh *out, int *status_out);
+
 /* R2: per-point swept-volume SDF query on the trajectory given by (N, T, coeffs).
  * pts: P x 3 (x, y, z) host doubles (z ignored).  Outputs (host, may be NULL): sdf[P], tstar[P], grad3[3P]
  * (body-frame FD gradient for sdf > 0; world-frame unit direction for the interior branch, exactly what the
